@@ -8,9 +8,12 @@ decode-only, 32-token image prefix + 128 generated tokens").  Reported per JSON 
   e2e        the same metric through the reference-facing C ABI (minigpt4_encode_image / minigpt4_begin_chat_image /
              128 x minigpt4_end_chat_image) with HOST buffers; host<->device copies and per-token sync inside the timing
   encode_ms  image-encode latency (device, CUDA events) and encode_e2e_ms (wall clock through the ABI)
-  roofline   decode dequant-matvec family: algorithmic weight bytes / CUDA-event time per launch vs MEASURED_PEAKS hbm_gbs
-  cpu_baseline  the CPU oracle (a restatement of the reference's ggml path) on this box's host cores, bounded sample
-`--impl reference` times that CPU path alone (the reference itself cannot be built here: DESIGN.md "Oracle").
+  roofline   decode dequant-matvec family: algorithmic weight bytes / CUDA-event time per launch vs the HBM peak (MEASURED_PEAKS.json
+             hbm_gbs when that file exists, else the H100 SXM data-sheet figure)
+  cpu_baseline  the CPU oracle (a restatement of the reference's ggml path) on the host's cores, bounded sample
+`--impl reference` times that CPU path alone (the reference itself cannot be built offline: DESIGN.md "Oracle").
+`--dump-outputs DIR` writes what the last timed step computed (image embedding, chained greedy ids, final logits, the ABI leg's text) as DIR/<name>.npy;
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 N > 1 (torchrun): default --mode replicas = one independent decode stream per GPU (the path is per-session work; no data-path
 collective; "scaling": "weak"); --mode tp = the optional tensor-parallel LLaMA step of north_star ("strong").
 """
@@ -89,7 +92,7 @@ def ensure_models(size: str, wtype: str, blocks: int):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index: int):
@@ -111,6 +114,7 @@ class ClockSampler:
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
+        self.proc.wait()
         sm = [float(r[1]) for r in self.rows if len(r) >= 8 and r[1].replace(".", "").isdigit()]
         mx = [float(r[2]) for r in self.rows if len(r) >= 8 and r[2].replace(".", "").isdigit()]
         reasons = set()
@@ -129,17 +133,7 @@ def measured_peaks() -> tuple[float, str]:
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def measured_traffic(kernel: str):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture (dram__bytes_read.sum +
-    dram__bytes_write.sum; profiles/traffic.json, written from the .ncu-rep of the same build), or None."""
-    p = ROOT / "profiles" / "traffic.json"
-    try:
-        return float(json.loads(p.read_text())[kernel]["dram_bytes_per_launch"])
-    except Exception:
-        return None
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 def host_cpus() -> int:
@@ -264,6 +258,8 @@ def main():
     ap.add_argument("--cpu-tokens", type=int, default=0, help="decode tokens of the CPU legs (default: 32)")
     ap.add_argument("--cpu-encode-every-step", action="store_true")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the last timed step returned as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--mode", default="replicas", choices=["replicas", "tp"],
                     help="N>1: 'replicas' = one independent decode stream per GPU, no data-path collective (weak scaling, default); "
                          "'tp' = one stream, LLaMA layers tensor-parallel over the GPUs with an NCCL sum per row-split matmul (strong scaling)")
@@ -315,8 +311,8 @@ def main():
             import torch
             torch.cuda.synchronize(); dist.barrier(); torch.cuda.synchronize()
 
-    def step(timed: bool):
-        """returns dict: encode_dev_ms, chain_ms, turn_s (whole turn through the ABI), ttft_s, decode_s, ids"""
+    def step(keep: bool):
+        """returns dict: encode_dev_ms, chain_ms, turn_s (whole turn through the ABI), ttft_s, decode_s, ids (+ a copy of the embedding rows if keep)"""
         # -- e2e leg: ONE chat turn through the reference ABI with host buffers, wall clock around all of it:
         #    image H2D + encode + embedding D2H | system prompt | embedding H2D + prefix + prompt | 128 x (decode step + 4-byte D2H + id_to_token)
         lib.minigpt4_reset_chat(ctx)
@@ -336,8 +332,9 @@ def main():
         rows = np.ctypeslib.as_array(emb.data, shape=(emb.n_embeddings,)).reshape(32, -1)
         tp0 = time.perf_counter(); ext.eval_embd(ctx, rows); ext.flush(ctx); prefix_ms = (time.perf_counter() - tp0) * 1e3
         ids, chain_ms = ext.decode_chain(ctx, N_GEN)
+        kept = {"emb": rows.copy()} if keep else {}
         lib.minigpt4_free_embedding(emb)
-        return {"enc_dev": enc_dev, "enc_wall": (t_enc - t0) * 1e3, "chain_ms": chain_ms, "turn_s": t_end - t0, "ttft_s": t_first - t0,
+        return {**kept, "enc_dev": enc_dev, "enc_wall": (t_enc - t0) * 1e3, "chain_ms": chain_ms, "turn_s": t_end - t0, "ttft_s": t_first - t0,
                 "prefill_s": t_pre - t_enc, "decode_s": t_end - t_pre, "prefix_ms": prefix_ms, "ids": ids, "toks": toks}
 
     for _ in range(args.warmup):
@@ -347,11 +344,18 @@ def main():
     barrier()
     sampler.start()
     t_begin = time.perf_counter()
-    res = [step(True) for _ in range(args.steps)]
+    res = [step(bool(args.dump_outputs) and i == args.steps - 1) for i in range(args.steps)]
     barrier()
     wall = time.perf_counter() - t_begin
     clocks = sampler.stop()
     launches = ext.stats(ctx).kernel_launches - launches0
+    if args.dump_outputs and rank == 0:   # what a caller of the timed path received in the last step
+        out = Path(args.dump_outputs)
+        out.mkdir(parents=True, exist_ok=True)
+        np.save(out / "image_embedding.npy", np.asarray(res[-1]["emb"], np.float32))
+        np.save(out / "chain_token_ids.npy", np.asarray(res[-1]["ids"], np.float64))
+        np.save(out / "final_logits.npy", ext.logits(ctx))   # device state is still that of the last step's chain
+        np.save(out / "e2e_text_utf8.npy", np.frombuffer("".join(res[-1]["toks"]).encode("utf-8"), np.uint8).astype(np.float32))   # the ABI leg's 128 token strings, as bytes
 
     chain_ms = sum(r["chain_ms"] for r in res); turn_s = sum(r["turn_s"] for r in res); dec_s = sum(r["decode_s"] for r in res)
     enc_dev = float(np.mean([r["enc_dev"] for r in res])); enc_wall = float(np.mean([r["enc_wall"] for r in res]))
@@ -377,7 +381,7 @@ def main():
         us = chain_ms * 1e3 / (args.steps * N_GEN)  # per launch on one GPU (max over ranks)
         ach = st.llm_weight_bytes_per_token / us * 1e-3
         roofline = {"bound": "hbm", "kernel": f"decode_megakernel<{args.wtype}> (1 launch per token: {st.n_layer} x [qkv, attention, wo, gate_up, down] + output/arg-max)",
-                    "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": measured_traffic(f"decode_megakernel_{args.size}_{args.wtype}"), "peak_source": peak_src,
+                    "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src,
                     "bytes_per_launch": st.llm_weight_bytes_per_token, "us_per_launch": us}
     else:
         kinds = ["qkv", "wo", "gate_up", "down", "output"]
@@ -396,9 +400,9 @@ def main():
     line = {"metric": metric_name(args.size, args.wtype), "value": value, "unit": "tokens/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": wall * 1e3 / args.steps, "higher_is_better": True,
             "scaling": "weak" if streams > 1 or world == 1 else "strong", "vs_baseline": None,
-            "dtype": "int8 x int4 dot (Q8_1 x Q4_1) f32-accumulate decode and prefill (tcgen05 kind::i8); f16 x f16 -> f32 tcgen05 encode", "data": "synthetic",
+            "dtype": "int8 x int4 dot (Q8_1 x Q4_1) f32-accumulate decode and prefill (wgmma s8); f16 x f16 -> f32 wgmma encode", "data": "synthetic",
             "config": {"workload": workload(args.size, args.wtype, args.blocks),
-                       "parallelism": (f"tp{world}" if args.mode == "tp" else f"dp{world} (one independent stream per GPU, no data-path collective)") if world > 1 else "single-gpu", "l2": "inputs larger than L2 (4.1 GB of weights streamed per token vs 126 MB L2)",
+                       "parallelism": (f"tp{world}" if args.mode == "tp" else f"dp{world} (one independent stream per GPU, no data-path collective)") if world > 1 else "single-gpu", "l2": "inputs larger than L2 (4.1 GB of weights streamed per token vs 50 MB L2)",
                        "value_region": "CUDA-event time of the 128-step device-chained greedy decode loop", "n_ctx": 2048},
             "encode_ms": enc_dev, "encode_e2e_ms": enc_wall, "prefix_ms": prefix_ms,
             "e2e": {"value": e2e, "unit": "tokens/s", "h2d_bytes_per_step": int(img.nbytes + 32 * st.n_embd * 4 + 4 * 256), "d2h_bytes_per_step": int(32 * st.n_embd * 4 + 4 * N_GEN),
@@ -414,7 +418,7 @@ def main():
     tp_env = os.environ.get("MINIGPT4_BENCH_TP")
     tp_leg = world > 1 and (tp_env == "1" or (tp_env != "0" and world in (2, 4)) or args.mode == "tp")
     if world > 1 and not tp_leg and tp_env != "0":
-        line["tp"] = {"world": world, "skipped": "tensor parallelism over %d GPUs has not run on hardware yet (2 and 4 have: profiles/r2_bench_*gpu_dp_and_tp.json); "
+        line["tp"] = {"world": world, "skipped": "tensor parallelism over %d GPUs is off by default (2 and 4 run it); "
                                                 "MINIGPT4_BENCH_TP=1 measures it" % world}
     if tp_leg:
         # the tensor-parallel LLaMA step of north_star on the same GPUs (strong scaling: ONE stream over all ranks), measured next to the

@@ -1,5 +1,5 @@
 /*
- * minigpt4.h — C ABI of the B200-native MiniGPT-4 engine (libminigpt4.so).
+ * minigpt4.h — C ABI of the H100-native MiniGPT-4 engine (libminigpt4.so).
  *
  * This header re-declares, symbol for symbol and field for field, the drop-in
  * boundary of Maknee/minigpt4.cpp so that the unmodified ctypes binding

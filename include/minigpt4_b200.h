@@ -1,5 +1,5 @@
 /*
- * minigpt4_b200.h — EXTRA entry points of the B200-native libminigpt4.so.
+ * minigpt4_b200.h — EXTRA entry points of the H100-native libminigpt4.so.
  *
  * The 18 symbols of minigpt4.h are untouched.  These additions exist because the reference ABI cannot express
  * (a) a tensor-parallel degree / device choice (SURVEY §8b "Extension needed by configs"),
@@ -60,7 +60,7 @@ struct MiniGPT4B200Stats {
     unsigned long long kernel_launches; /* kernels of this library launched so far (both graphs) */
     int n_layer, n_embd, n_ff, n_vocab, n_ctx, tp_rank, tp_world, sm_count;
     int decode_megakernel;              /* > 0: decode step = one persistent kernel per token (value = kernel generation); 0: one launch per op (graph) */
-    int prefill_gemm;                   /* 1: prompt / prefix rows (N >= 2) run through the tcgen05 kind::i8 prefill GEMM; 0: per-op matvec path */
+    int prefill_gemm;                   /* 1: prompt / prefix rows (N >= 2) run through the wgmma s8 prefill GEMM; 0: per-op matvec path */
 };
 MINIGPT4_API int minigpt4_b200_stats(struct MiniGPT4Context *ctx, struct MiniGPT4B200Stats *out);
 

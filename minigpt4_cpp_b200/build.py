@@ -1,4 +1,4 @@
-"""Build libminigpt4.so for sm_100a with nvcc (in-tree; output build/libminigpt4.so, where the reference's
+"""Build libminigpt4.so for sm_90a with nvcc (in-tree; output build/libminigpt4.so, where the reference's
 ctypes loader looks: reference minigpt4/minigpt4_library.py:539-566)."""
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ SOURCES = ["llama.cu", "vision.cu", "api.cpp", "engine.cpp", "formats.cpp", "tex
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false / -ffp-contract=off: no implicit FMA contraction — float expressions evaluate exactly as written so the
 # language path is bit-identical to the CPU oracle's canonical reduction order (see oracle/oracle.cpp header)
-FLAGS = ["-ccbin", "/usr/bin/g++", "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-fmad=false",
+FLAGS = ["-ccbin", "/usr/bin/g++", "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",
          "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function,-Wno-class-memaccess,-ffp-contract=off", "-I", str(ROOT / "include")]
 
 
@@ -60,7 +60,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         if failed:
             raise RuntimeError("libminigpt4.so: compilation failed")
         tmp = OUT.with_suffix(f".so.tmp{os.getpid()}")
-        link = [NVCC, "-ccbin", "/usr/bin/g++", "-shared", "-o", str(tmp), *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        link = [NVCC, "-ccbin", "/usr/bin/g++", "-shared", "-o", str(tmp), *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                 "-Xlinker", "--no-undefined", "-ldl", "-lpthread", "-cudart", "static"]
         r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:

@@ -1,5 +1,5 @@
 // api.cpp — the C ABI of libminigpt4.so: the reference's 18 entry points (include/minigpt4.h, mirroring reference
-// minigpt4.cpp:2543-2987) plus the B200 extensions (include/minigpt4_b200.h).
+// minigpt4.cpp:2543-2987) plus the extensions (include/minigpt4_b200.h).
 #include "../../include/minigpt4_b200.h"
 #include "engine.h"
 #include "image.h"

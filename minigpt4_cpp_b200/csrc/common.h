@@ -1,4 +1,4 @@
-// common.h — shared host-side declarations of the B200-native engine.
+// common.h — shared host-side declarations of the H100-native engine.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

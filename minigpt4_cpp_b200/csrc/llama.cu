@@ -788,7 +788,7 @@ float LlamaDevice::time_matvec(int kind, int reps, double *bytes_per_launch) {
     for (int r = 0; r < reps; ++r) {
         if (kind == 4) {
             for (int i = 0; i < 8; ++i) {
-                CUDA_CHECK(cudaMemsetAsync(flush, i, flush_bytes, stream_));  // evict the 126 MB L2
+                CUDA_CHECK(cudaMemsetAsync(flush, i, flush_bytes, stream_));  // evict the 50 MB L2
                 CUDA_CHECK(cudaEventRecord(ev0_, stream_)); one(0); CUDA_CHECK(cudaEventRecord(ev1_, stream_));
                 CUDA_CHECK(cudaStreamSynchronize(stream_));
                 float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, ev0_, ev1_)); total_ms += ms; ++launches;

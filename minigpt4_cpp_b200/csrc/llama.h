@@ -123,7 +123,7 @@ private:
     int mega_gen_ = 6; void *mega6_params_ = nullptr; int mega6_nbl_ = 0;  // generation 6 (llama_mega6.cuh)
     bool h_state_busy_ = false;
     bool mega_ = false; unsigned *mega_barrier_ = nullptr; size_t mega_smem_ = 0; int mega_type_ = -1;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
 };
 
 }  // namespace mg4

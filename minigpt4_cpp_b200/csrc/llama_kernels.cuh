@@ -1,4 +1,4 @@
-// llama_kernels.cuh — sm_100a kernels of the LLaMA step (decode matvec family, attention, embedding gather).
+// llama_kernels.cuh — sm_90a kernels of the LLaMA step (decode matvec family, attention, embedding gather).
 //
 // Numerics mirror ggml@master-31cfbb1 (SURVEY.md §A.3): activations are quantised to the weight type's
 // vec_dot type (Q8_0 / Q8_1 / Q8_K / F16) and the block dot products are integer (dp4a) with F32 scaling —

@@ -1,24 +1,23 @@
 // llama_mega6.cuh — the persistent decode megakernel, generation 6: ONE launch per generated token.
 //
-// A 7B Q4_1 token streams 4.13 GB of weights through ~160 dependent matvecs of 1.6-12 us each.  Weights do not depend on activations, so the
+// A 7B Q4_1 token streams 4.13 GB of weights through ~160 dependent, short matvecs.  Weights do not depend on activations, so the
 // weight stream is kept running ACROSS op boundaries:
 //   * grid = one CTA per SM (cooperative launch), 16 warps; warps 0..W-1 (W <= 15) are STREAM warps, every warp of 0..14 also takes part in
 //     activation staging, warps 0-7 run the attention op
 //   * SELF-REFILLED PER-WARP STREAMS.  Every stream warp owns TWO shared-memory slots and a private cursor over the token's op program.  It
 //     walks "its" row pairs of every weight matrix (pairs lo + w, lo + w + W, ... of the CTA's contiguous share) and keeps the next two
 //     slot-loads in flight with cp.async.bulk (1-D TMA) + mbarrier complete_tx; right after it has read a slot it re-arms the slot ITSELF.
-//     No producer warp and no "empty" barriers: the measured ceiling of a single producer thread (~4.4 TB/s of 5 KB copies, try_wait +
-//     expect_tx + issue per copy) was the limit of generations 2-5, while 15 independent issuers per SM stream at 7.0-7.3 TB/s with the full
-//     Q4_1 dot product in the loop (tools/ubench_stream.cu, profiles/r2_ubench_stream.log).  The cursor runs straight through grid barriers,
-//     staging and the attention op: 2 x W slots (207 KB per SM, 30 MB chip-wide) are always requested ahead of the consumers.
+//     No producer warp and no "empty" barriers: a single producer thread is issue-bound on 5 KB copies (try_wait + expect_tx + issue per
+//     copy), which was the limit of generations 2-5; 15 independent issuers per SM are not (tools/ubench_stream.cu measures the primitive
+//     with the full Q4_1 dot product in the loop).  The cursor runs straight through grid barriers,
+//     staging and the attention op: 2 x W slots (207 KB per SM) are always requested ahead of the consumers.
 //   * REGISTER-RESIDENT ACTIVATIONS for n_embd-wide inputs (qkv, wo, gate/up, output): lane l keeps the Q8 blocks l, l+32, ... of the staged
 //     vector in registers, so a row pair costs shared-memory reads of the WEIGHTS only (TMA write + one read = 2 x the HBM rate of smem traffic)
 //   * per op: [grid barrier -> stage activations (RMSNorm + Q8 quantise) -> per owned row pair: wait slot, dp4a dots, re-arm slot,
 //     warp-shuffle reductions, fused epilogue].  Ops exchange x / q / att / act through L2 (ld.global.cg); a grid barrier (atomic counter)
 //     separates dependent ops.
 //   * NO deeper prefetch than the slots.  A look-ahead warp that asked L2 for the stream beyond the slots while the stream warps were stalled
-//     (cp.async.bulk.prefetch.L2, or cp.async into a scratch line) was measured and removed: 192 KB per CTA changed nothing, 384 KB cost 20 %
-//     (profiles/r2_v6_lookahead_ab.log) - the barrier / staging / attention phases between two matvecs are chains of L2 round trips, and every
+//     (cp.async.bulk.prefetch.L2, or cp.async into a scratch line) was tried and removed (no gain at 192 KB per CTA, a loss at 384 KB) - the barrier / staging / attention phases between two matvecs are chains of L2 round trips, and every
 //     byte of weight traffic in flight during them lengthens those round trips.
 // Reduction orders are the canonical ones of llama_kernels.cuh / oracle.cpp: logits are bit-identical to the per-op kernels and the CPU oracle.
 #pragma once

@@ -2,10 +2,11 @@
 // the weights (reference call sites minigpt4.cpp:2365-2382 add_tokens in n_batch chunks, :2399-2415 add_embedding = 32 rows at once).
 //
 // Semantics are ggml's quantised mul_mat, exactly as the decode matvec (llama_kernels.cuh): activations quantised to Q8_0 / Q8_1 per 32,
-// INTEGER block dot products, F32 scaling.  Here the integer dots run on the 5th-generation tensor cores:
-//   * one tcgen05.mma kind::i8 (M = 128 weight rows, N = 32 tokens, K = 32 = ONE quant block, accumulate = 0) per quant block puts the
-//     128 x 32 exact int32 block dots into TMEM; the per-block scales cannot be folded into the MMA, so
-//   * sixteen epilogue warps (32 rows x 8 tokens each) read each block's dots back (tcgen05.ld), apply  d_w * d_a * isum  and  m_w * s_a  on the CUDA cores and
+// INTEGER block dot products, F32 scaling.  Here the integer dots run on the Hopper tensor cores:
+//   * a CTA owns 128 weight rows x 32 tokens; each of its four consumer warpgroups owns a 64-row x 16-token quarter and issues one
+//     wgmma.mma_async m64n16k32 s8 x s8 -> s32 (K = 32 = ONE quant block, no accumulation) per quant block, which leaves the exact int32
+//     block dots in its registers (a thread holds 2 rows x 4 tokens); the per-block scales cannot be folded into the MMA, so
+//   * the same sixteen warps apply  d_w * d_a * isum  and  m_w * s_a  on the CUDA cores and
 //     accumulate in the CANONICAL FLOAT ORDER of oracle.cpp / k::dot2_q4: "lane" class l = b mod 32 accumulates its blocks l, l+32, ...
 //     in increasing order; the 32 class sums are then combined by the xor-butterfly tree (16, 8, 4, 2, 1).  The K loop therefore walks
 //     the classes in bit-reversed order (0, 16, 8, 24, ...), which turns the butterfly into a post-order tree walk with a 5-deep stack
@@ -13,9 +14,10 @@
 //   * operands come from a load-time "prefill operand cache": the nibbles expanded to int8 (Q4_0: q - 8, so the "-8 * sum(a)" term is
 //     inside the integer dot) in CLASS-MAJOR order — row r = [class l][slot i][32 bytes] — so that one 128-byte TMA box row holds four
 //     consecutive blocks of one class (SWIZZLE_128B, the layout the tensor core reads); the staged activations use the same order.
-//     (Trade: +1 byte per weight of HBM for the cache on a 180 GB device; the decode path keeps streaming the 4-bit original.)
+//     (Trade: +1 byte per weight of HBM for the cache, 6.5 GB for a 7B model; the decode path keeps streaming the 4-bit original.)
 // The kernel is epilogue-bound by construction (5 CUDA-core instructions per (row, token, block) against 32 int8 MACs on the tensor core):
 // exact Q8 semantics cost that; what the tensor core removes is the 8 dp4a + nibble unpacking per (row, token, block) of the matvec path.
+// Inside a warp nothing overlaps its MMAs (issue, commit, wait, scale); whether the other warps of a scheduler hide that wait is not measured.
 #pragma once
 #include "llama_kernels.cuh"
 #include <cuda.h>
@@ -24,16 +26,15 @@ namespace mg4 {
 namespace pf {
 using namespace k;
 
-constexpr int kTok = 32;          // tokens per CTA (UMMA N)
-constexpr int kRows = 128;        // weight rows per CTA (UMMA M)
+constexpr int kTok = 32;          // tokens per CTA
+constexpr int kRows = 128;        // weight rows per CTA
 constexpr int kStages = 4;        // shared-memory pipeline depth (tiles of 4 blocks)
 constexpr int kStageBytes = 16384 + 4096 + 1024;  // A 128 x 128 B | B 32 x 128 B | activation scales 32 x 4 x {d, s}
-constexpr int kGroups = 4;        // TMEM tile groups (4 x 32-column block regions each) -> 512 columns
-constexpr int kEpiWarps = 16;       // 4 per TMEM lane quarter: a warp owns 32 rows x kTpw tokens (twice the warps of the first cut: the epilogue is a latency chain)
-constexpr int kTpw = kTok * 4 / kEpiWarps;   // tokens per epilogue warp (8)
-constexpr int kThreads = 64 + 32 * kEpiWarps;     // warp 0 = TMA producer, warp 1 = MMA issuer, warps 2-17 = epilogue
-static_assert(kTpw == 8, "tmem_ld8i");
-constexpr int kStackBytes = 4 * kTok * kRows * 8; // stack levels 1-4: [level][token][row] {d-tree, m-tree}
+constexpr int kConsWarps = 16;    // four warpgroups: (row half, token half) of the tile, wgmma M = 64, N = 16
+constexpr int kOut = 8;           // outputs per consumer thread: 2 rows x 4 tokens, in wgmma accumulator order
+constexpr int kThreads = 32 * kConsWarps + 32;    // warps 0-15 = MMA + epilogue, warp 16 = TMA producer
+constexpr int kStackBytes = 4 * kTok * kRows * 8; // stack levels 1-4: [level][output of the thread][thread] {d-tree, m-tree}
+static_assert(kOut * 32 * kConsWarps == kTok * kRows, "one stack slot per output of the tile");
 
 struct PrefillArgs {
     int rows;            // valid weight rows (the operand cache is padded to a multiple of 128 rows)
@@ -67,25 +68,20 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-// D[tmem] = A[smem] . B[smem], int8 x int8 -> int32, no accumulation (every quant block gets its own TMEM columns)
-__device__ __forceinline__ void tc_mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 16] = A[64 x 32] . B[16 x 32]^T from shared memory, int8 x int8 -> int32, no accumulation (every quant block gets its own registers):
+// thread (warp w, lane) of the warpgroup holds d[4 j + 2 h + e] = D[16 w + lane / 4 + 8 h][8 j + 2 (lane % 4) + e]
+__device__ __forceinline__ void wgmma_i8_n16(int (&d)[kOut], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc) : "memory");
+        "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]) : "l"(adesc), "l"(bdesc));
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (as vision_kernels.cuh: version 1, layout type 2, SBO = 8 rows * 128 B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor, kind::i8: D = S32 (c_format 2), A = B = signed 8-bit (format 1), both K-major, M = 128, N = n
-__device__ __forceinline__ uint32_t umma_idesc_i8(int n) { return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24); }
-__device__ __forceinline__ void tmem_ld8i(uint32_t taddr, int (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (as vision_kernels.cuh: layout type 1 in bits 62-63, SBO = 8 rows * 128 B)
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 __device__ __forceinline__ uint4 ldg_nc16(const void *p) {
     uint4 r;
@@ -123,7 +119,7 @@ __device__ __forceinline__ void prefill_epilogue(const PrefillArgs &g, int r, in
     }
 }
 
-// grid (rows_pad / 128, ceil(n_tok / 32)); block 320; dynamic smem = 1024 (alignment) + 4 stages + stack + barriers
+// grid (rows_pad / 128, ceil(n_tok / 32)); block 544; dynamic smem = 1024 (alignment) + 4 stages + stack + barriers
 template <bool Q41>
 __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_q4(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                                                                   const __grid_constant__ CUtensorMap tmS, const PrefillArgs g) {
@@ -132,32 +128,21 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_q4(const __grid_cons
     float2 *stack = (float2 *)(smem + (size_t)kStages * kStageBytes);
     uint64_t *full = (uint64_t *)((unsigned char *)stack + kStackBytes);
     uint64_t *empty = full + kStages;
-    uint64_t *rfull = empty + kStages;
-    uint64_t *rempty = rfull + kGroups;
-    uint32_t *tmem_slot = (uint32_t *)(rempty + kGroups);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m_tile = blockIdx.x, t_tile = blockIdx.y;
     const int tpc = g.S >> 2;  // tiles per class
     const int jr0 = (int)blockIdx.z * g.jr_per_z, jr1 = jr0 + g.jr_per_z;   // leaves (classes in bit-reversed order) of this CTA's subtree
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmS) : "memory");
-        for (int i = 0; i < kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1 + kEpiWarps); }
-        for (int i = 0; i < kGroups; ++i) { mbar_init(&rfull[i], 1); mbar_init(&rempty[i], kEpiWarps); }
+        for (int i = 0; i < kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kConsWarps) {
         // ---------------- TMA producer ----------------
         if (lane == 0) {
             unsigned cnt = 0;
@@ -176,109 +161,87 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_q4(const __grid_cons
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        const uint32_t idesc = umma_idesc_i8(kTok);
-        unsigned cnt = 0;
-        for (int jr = jr0; jr < jr1; ++jr) {
-            const int l = bitrev5(jr);
-            for (int j = 0; j < tpc; ++j) {
-                const int v = tile_blocks(g.nb, l, j);
-                if (v == 0) continue;
-                const int s = (int)(cnt % kStages); const uint32_t ph = (cnt / kStages) & 1u;
-                const int gq = (int)(cnt % kGroups); const uint32_t gph = (cnt / kGroups) & 1u; ++cnt;
-                mbar_wait(&full[s], ph);
-                mbar_wait(&rempty[gq], gph ^ 1u);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t sa = smem_u32(smem + (size_t)s * kStageBytes), sb = sa + 16384u;
-                    for (int i = 0; i < v; ++i)
-                        tc_mma_i8(tmem_base + (uint32_t)(gq * 128 + i * 32), umma_desc_sw128(sa + i * 32), umma_desc_sw128(sb + i * 32), idesc);
-                    tc_commit(&rfull[gq]);   // block dots of this tile are in TMEM
-                    tc_commit(&empty[s]);    // ... and the tensor core is done reading the stage's A / B
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ---------------- epilogue: scale, accumulate in canonical order, butterfly tree, fused output ----------------
-        const int ew = warp - 2, quarter = warp & 3, tq = ew >> 2;   // TMEM lanes 32 * (warp % 4) .. + 31; tokens kTpw * tq .. + kTpw - 1
-        const int row_in = quarter * 32 + lane, r = m_tile * kRows + row_in, c0 = tq * kTpw;
-        const uint32_t tlane = (uint32_t)(quarter * 32) << 16;
-        const __half2 *wrow = g.wsc + (size_t)r * (32 * g.S);
-        float accd[kTpw], accm[kTpw], l0d[kTpw], l0m[kTpw];
+        return;
+    }
+    // ---------------- consumers: block dots, scale, accumulate in canonical order, butterfly tree, fused output ----------------
+    // output o = 4 j + 2 h + e of this thread: row row_in + 8 h, token tok0 + 8 j + e (the wgmma accumulator layout)
+    const int wg = warp >> 2, rh = wg & 1, th = wg >> 1;
+    const int row_in = rh * 64 + (warp & 3) * 16 + (lane >> 2), r = m_tile * kRows + row_in, tok0 = th * 16 + 2 * (lane & 3);
+    const __half2 *wrow = g.wsc + (size_t)r * (32 * g.S);
+    const size_t wrow8 = (size_t)8 * (32 * g.S);
+    float2 *mystack = stack + threadIdx.x;   // level lev, output o: mystack[((lev - 1) * kOut + o) * 32 * kConsWarps]
+    float accd[kOut], accm[kOut], l0d[kOut], l0m[kOut];
 #pragma unroll
-        for (int c = 0; c < kTpw; ++c) { accd[c] = 0.f; accm[c] = 0.f; l0d[c] = 0.f; l0m[c] = 0.f; }
-        unsigned cnt = 0;
-        for (int jr = jr0; jr < jr1; ++jr) {
-            const int l = bitrev5(jr);
-            for (int j = 0; j < tpc; ++j) {
-                const int v = tile_blocks(g.nb, l, j);
-                if (v == 0) continue;
-                const int s = (int)(cnt % kStages); const uint32_t ph = (cnt / kStages) & 1u;
-                const int gq = (int)(cnt % kGroups); const uint32_t gph = (cnt / kGroups) & 1u; ++cnt;
-                const uint4 w4 = ldg_nc16(wrow + l * g.S + 4 * j);   // {d, m} of this row's four blocks (issued before the waits)
-                mbar_wait(&full[s], ph);       // activation scales of the tile are in shared memory
-                mbar_wait(&rfull[gq], gph);    // block dots are in TMEM
-                tc_fence_after();
-                const float2 *asc = (const float2 *)(smem + (size_t)s * kStageBytes + 16384 + 4096);  // [token][4] {d, s}
-                const unsigned wv[4] = {w4.x, w4.y, w4.z, w4.w};
+    for (int o = 0; o < kOut; ++o) { accd[o] = 0.f; accm[o] = 0.f; l0d[o] = 0.f; l0m[o] = 0.f; }
+    unsigned cnt = 0;
+    for (int jr = jr0; jr < jr1; ++jr) {
+        const int l = bitrev5(jr);
+        for (int j = 0; j < tpc; ++j) {
+            const int v = tile_blocks(g.nb, l, j);
+            if (v == 0) continue;
+            const int s = (int)(cnt % kStages); const uint32_t ph = (cnt / kStages) & 1u; ++cnt;
+            const uint4 w4[2] = {ldg_nc16(wrow + l * g.S + 4 * j), ldg_nc16(wrow + wrow8 + l * g.S + 4 * j)};   // {d, m} of the four blocks of both rows (issued before the wait)
+            mbar_wait(&full[s], ph);       // operands and activation scales of the tile are in shared memory
+            const uint32_t sa = smem_u32(smem + (size_t)s * kStageBytes) + (uint32_t)rh * 8192u, sb = sa - (uint32_t)rh * 8192u + 16384u + (uint32_t)th * 2048u;
+            int isum[4][kOut];
+            wgmma_fence();
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    if (i < v) {
-                        int isum[kTpw];
-                        tmem_ld8i(tmem_base + tlane + (uint32_t)(gq * 128 + i * 32 + c0), isum);
-                        const float2 f = __half22float2(*(const __half2 *)&wv[i]);
+            for (int i = 0; i < 4; ++i)   // all four: the slots past the last block of a class are zero padding, and an unconditional issue keeps the MMAs asynchronous
+                wgmma_i8_n16(isum[i], wgmma_desc_sw128(sa + i * 32), wgmma_desc_sw128(sb + i * 32));
+            wgmma_commit();
+            wgmma_wait_all();
+            const float2 *asc = (const float2 *)(smem + (size_t)s * kStageBytes + 16384 + 4096);  // [token][4] {d, s}
+            const unsigned wv[2][4] = {{w4[0].x, w4[0].y, w4[0].z, w4[0].w}, {w4[1].x, w4[1].y, w4[1].z, w4[1].w}};
 #pragma unroll
-                        for (int c = 0; c < kTpw; ++c) {
-                            const float2 ds = asc[(c0 + c) * 4 + i];
-                            if (Q41) { accd[c] = fmaf(f.x * ds.x, (float)isum[c], accd[c]); accm[c] = fmaf(f.y, ds.y, accm[c]); }
-                            else accd[c] += ((float)isum[c] * f.x) * ds.x;
-                        }
+            for (int i = 0; i < 4; ++i) {
+                if (i < v) {
+                    const float2 f[2] = {__half22float2(*(const __half2 *)&wv[0][i]), __half22float2(*(const __half2 *)&wv[1][i])};
+#pragma unroll
+                    for (int o = 0; o < kOut; ++o) {
+                        const int h = (o >> 1) & 1;
+                        const float2 ds = asc[(tok0 + 8 * (o >> 2) + (o & 1)) * 4 + i];
+                        if (Q41) { accd[o] = fmaf(f[h].x * ds.x, (float)isum[i][o], accd[o]); accm[o] = fmaf(f[h].y, ds.y, accm[o]); }
+                        else accd[o] += ((float)isum[i][o] * f[h].x) * ds.x;
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { mbar_arrive(&rempty[gq]); mbar_arrive(&empty[s]); }
             }
-            // class l is complete: fold it into the butterfly tree (post-order walk, jr = leaf number in bit-reversed class order)
-            const int jl = jr - jr0;   // leaf number inside this CTA's subtree (jr0 is a multiple of the subtree size)
-            if ((jl & 1) == 0) {
-#pragma unroll
-                for (int c = 0; c < kTpw; ++c) { l0d[c] = accd[c]; l0m[c] = accm[c]; accd[c] = 0.f; accm[c] = 0.f; }
-            } else {
-                int ones = 1; while (ones < 5 && ((jl >> ones) & 1)) ++ones;  // trailing ones of jl (>= 1)
-#pragma unroll
-                for (int c = 0; c < kTpw; ++c) {
-                    float vd = l0d[c] + accd[c], vm = l0m[c] + accm[c];
-                    accd[c] = 0.f; accm[c] = 0.f;
-                    for (int lev = 1; lev < ones; ++lev) {
-                        const float2 o = stack[((size_t)(lev - 1) * kTok + (c0 + c)) * kRows + row_in];
-                        vd = o.x + vd; vm = o.y + vm;
-                    }
-                    if (jr != jr1 - 1) stack[((size_t)(ones - 1) * kTok + (c0 + c)) * kRows + row_in] = make_float2(vd, vm);
-                    else { l0d[c] = vd; l0m[c] = vm; }
-                }
-            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-        // results: res[c] = d-tree + m-tree (k::dot2_q4: warp_sum(accd) + warp_sum(accm)); fused epilogues of k::matvec_kernel
-        const int n_past = g.state->n_past;
+        // class l is complete: fold it into the butterfly tree (post-order walk, jr = leaf number in bit-reversed class order)
+        const int jl = jr - jr0;   // leaf number inside this CTA's subtree (jr0 is a multiple of the subtree size)
+        if ((jl & 1) == 0) {
 #pragma unroll
-        for (int c = 0; c < kTpw; ++c) {
-            const int t = t_tile * kTok + c0 + c;
-            if (gridDim.z > 1) {   // K split: the root of this CTA's subtree; prefill_combine finishes the tree
-                if (t < g.n_tok && r < g.rows) g.partial[((size_t)blockIdx.z * g.part_tok + t) * g.part_rows + r] = make_float2(l0d[c], l0m[c]);
-                continue;
+            for (int o = 0; o < kOut; ++o) { l0d[o] = accd[o]; l0m[o] = accm[o]; accd[o] = 0.f; accm[o] = 0.f; }
+        } else {
+            int ones = 1; while (ones < 5 && ((jl >> ones) & 1)) ++ones;  // trailing ones of jl (>= 1)
+#pragma unroll
+            for (int o = 0; o < kOut; ++o) {
+                float vd = l0d[o] + accd[o], vm = l0m[o] + accm[o];
+                accd[o] = 0.f; accm[o] = 0.f;
+                for (int lev = 1; lev < ones; ++lev) {
+                    const float2 p = mystack[(size_t)((lev - 1) * kOut + o) * (32 * kConsWarps)];
+                    vd = p.x + vd; vm = p.y + vm;
+                }
+                if (jr != jr1 - 1) mystack[(size_t)((ones - 1) * kOut + o) * (32 * kConsWarps)] = make_float2(vd, vm);
+                else { l0d[o] = vd; l0m[o] = vm; }
             }
-            const float res = l0d[c] + l0m[c];
-            const float other = __shfl_xor_sync(0xffffffffu, res, 1);   // the pair row (RoPE / SwiGLU pair adjacent rows)
-            if (t >= g.n_tok || r >= g.rows) continue;
-            prefill_epilogue(g, r, t, n_past, res, other);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    // results: res[o] = d-tree + m-tree (k::dot2_q4: warp_sum(accd) + warp_sum(accm)); fused epilogues of k::matvec_kernel
+    const int n_past = g.state->n_past;
+#pragma unroll
+    for (int o = 0; o < kOut; ++o) {
+        const int t = t_tile * kTok + tok0 + 8 * (o >> 2) + (o & 1), ro = r + 8 * ((o >> 1) & 1);
+        if (gridDim.z > 1) {   // K split: the root of this CTA's subtree; prefill_combine finishes the tree
+            if (t < g.n_tok && ro < g.rows) g.partial[((size_t)blockIdx.z * g.part_tok + t) * g.part_rows + ro] = make_float2(l0d[o], l0m[o]);
+            continue;
+        }
+        const float res = l0d[o] + l0m[o];
+        const float other = __shfl_xor_sync(0xffffffffu, res, 4);   // the pair row (RoPE / SwiGLU pair adjacent rows) sits four lanes away
+        if (t >= g.n_tok || ro >= g.rows) continue;
+        prefill_epilogue(g, ro, t, n_past, res, other);
+    }
 }
 
 // K-split GEMMs: fold the subtree roots of the grid.z slices (pairwise, in leaf order = the upper levels of the butterfly tree), then the epilogue.

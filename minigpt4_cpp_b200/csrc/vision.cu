@@ -34,7 +34,8 @@ static void make_map_f16(CUtensorMap *m, const void *ptr, int rows, int cols, in
     if (r != CUDA_SUCCESS) MG4_PANIC("cuTensorMapEncodeTiled failed (%d) for [%d x %d] box %d", (int)r, rows, cols, box_rows);
 }
 
-static int next_pow2_cols(int c) { int p = 32; while (p < c) p <<= 1; return p; }
+static const int kTokTiles[] = {32, 80, 144, 256};   // instantiated token tiles (wgmma N) of gemm_f16_wgmma
+static int tok_tile(int t) { for (int nt : kTokTiles) if (t <= nt) return nt; return 256; }
 
 static GemmPlan *make_plan(const __half *W, int M, int K, const __half *X, int T, int epi, int ksplit = 1) {
     if (M % 128 || K % 64 || T < 1 || T > 272) MG4_PANIC("gemm plan: unsupported shape M=%d K=%d T=%d", M, K, T);
@@ -42,44 +43,45 @@ static GemmPlan *make_plan(const __half *W, int M, int K, const __half *X, int T
     memset(p, 0, sizeof(*p));
     GemmArgs &a = p->a;
     a.M_out = M; a.T = T; a.K = K; a.epi = epi;
-    a.t_pad = (T + 15) & ~15;
-    a.n1 = std::min(256, a.t_pad); a.n2 = a.t_pad - a.n1;
-    if (a.t_pad > 256) { a.box_rows = a.t_pad / 2; a.n_box = 2; } else { a.box_rows = a.t_pad; a.n_box = 1; }
-    a.stage_bytes = 16384 + a.t_pad * 128;
-    a.stages = std::min(8, (200 * 1024) / a.stage_bytes);
-    a.tmem_cols = next_pow2_cols(a.t_pad);
-    p->smem = (size_t)a.stages * a.stage_bytes + 1024 + 256;
     p->grid = M / 128;
-    p->grid_y = 1; p->grid_z = 1;
-    // split the tokens of the 257-token GEMMs over grid.y CTAs so that ~132-144 SMs work (MINIGPT4_B200_VISION_TSPLIT=0: one CTA per weight slab, for A/B runs)
+    p->grid_z = 1;
+    int splits = 1;
+    // split the tokens of the 257-token GEMMs over grid.y CTAs so that most of the 132 SMs work (MINIGPT4_B200_VISION_TSPLIT=0: as few CTAs per weight slab as fit, for A/B runs)
     const bool tsplit = !(getenv("MINIGPT4_B200_VISION_TSPLIT") && atoi(getenv("MINIGPT4_B200_VISION_TSPLIT")) == 0);  // (read per plan: a test loads both variants)
     if (tsplit && T > 128 && epi != GE_PATCH) {
-        const int splits = std::max(2, std::min(4, 148 / p->grid));            // 33 tiles -> 4, 48 -> 3, 11 / 12 -> 4
-        const int tt = (((T + splits - 1) / splits) + 15) & ~15;               // tokens per CTA, multiple of 16 (UMMA N)
-        a.t_tile = tt; a.t_pad = tt; a.n1 = tt; a.n2 = 0; a.box_rows = tt; a.n_box = 1;
-        a.stage_bytes = 16384 + tt * 128;                                      // stays a multiple of 1024 (128-byte-swizzle atoms)
-        a.stages = std::min(8, (200 * 1024) / a.stage_bytes);
-        a.tmem_cols = next_pow2_cols(tt);
-        p->smem = (size_t)a.stages * a.stage_bytes + 1024 + 256;
-        p->grid_y = (T + tt - 1) / tt;
+        splits = std::max(2, std::min(4, 132 / p->grid));                      // 33 tiles -> 4 (132 CTAs), 48 -> 2 (96), 11 / 12 -> 4 (x split-K)
         if (ksplit > 1 && ksplit <= K / 64) {                                  // split-K: grid.z slices of whole k-blocks, raw partials out (GE_PARTIAL)
             a.k_split_blocks = (K / 64 + ksplit - 1) / ksplit;
             p->grid_z = (K / 64 + a.k_split_blocks - 1) / a.k_split_blocks;
             if (p->grid_z > 1) a.epi = GE_PARTIAL; else { a.k_split_blocks = 0; p->grid_z = 1; }
         }
     }
+    a.nt = tok_tile((T + splits - 1) / splits);                                // tokens per CTA
+    p->grid_y = (T + a.nt - 1) / a.nt;
+    a.stage_bytes = 16384 + a.nt * 128;                                        // a multiple of 1024 (128-byte-swizzle atoms)
+    a.stages = std::min(8, (200 * 1024) / a.stage_bytes);
+    p->smem = (size_t)a.stages * a.stage_bytes + 1024 + 256;
     make_map_f16(&p->tmW, W, M, K, 128);
-    make_map_f16(&p->tmX, X, T, K, a.box_rows);
+    make_map_f16(&p->tmX, X, T, K, a.nt);
     return p;
 }
-static void launch_plan(const GemmPlan *p, cudaStream_t s) {
+template <int NT> static void launch_gemm(const GemmPlan *p, cudaStream_t s) {
     static bool configured[64] = {};   // per device
     int dev = 0; cudaGetDevice(&dev);
     if (!configured[dev & 63]) {
-        CUDA_CHECK(cudaFuncSetAttribute(gemm_f16_tcgen05, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024));
+        CUDA_CHECK(cudaFuncSetAttribute(gemm_f16_wgmma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024));
         configured[dev & 63] = true;
     }
-    gemm_f16_tcgen05<<<dim3((unsigned)p->grid, (unsigned)p->grid_y, (unsigned)p->grid_z), 192, p->smem, s>>>(p->tmW, p->tmX, p->a);
+    gemm_f16_wgmma<NT><<<dim3((unsigned)p->grid, (unsigned)p->grid_y, (unsigned)p->grid_z), kGemmThreads, p->smem, s>>>(p->tmW, p->tmX, p->a);
+}
+static void launch_plan(const GemmPlan *p, cudaStream_t s) {
+    switch (p->a.nt) {
+        case 32: launch_gemm<32>(p, s); break;
+        case 80: launch_gemm<80>(p, s); break;
+        case 144: launch_gemm<144>(p, s); break;
+        case 256: launch_gemm<256>(p, s); break;
+        default: MG4_PANIC("gemm plan: token tile %d is not instantiated", p->a.nt);
+    }
     CUDA_CHECK(cudaGetLastError());
 }
 

@@ -17,7 +17,7 @@ namespace mg4 {
 
 struct VisionDims { int D = 1408, T = 257, H = 16, dh = 88, FF = 6144, n_blocks = 0, n_q = 32, qh = 768, q_layers = 0, n_embd_llm = 4096; };
 
-struct GemmPlan;  // one planned tcgen05 GEMM launch (tensor maps + args)
+struct GemmPlan;  // one planned wgmma GEMM launch (tensor maps + args)
 
 class VisionDevice {
 public:
@@ -39,7 +39,7 @@ public:
     size_t weight_bytes() const { return weight_bytes_; }
     cudaStream_t stream() const { return stream_; }
 
-    // kernel-level test hook: out[T][M] = bias + X[T][K] . W[M][K]^T through the tcgen05 GEMM (F16 operands on host)
+    // kernel-level test hook: out[T][M] = bias + X[T][K] . W[M][K]^T through the wgmma GEMM (F16 operands on host)
     static void test_gemm(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, float *out_f32);
     static int test_dequant(int gg_type, const void *raw, long n, void *out_f16);
     static void test_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out);

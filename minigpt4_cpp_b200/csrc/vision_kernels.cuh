@@ -1,13 +1,13 @@
-// vision_kernels.cuh — sm_100a kernels of the vision graph (EVA ViT-g/14 + Q-Former + llama_proj), the path
+// vision_kernels.cuh — sm_90a kernels of the vision graph (EVA ViT-g/14 + Q-Former + llama_proj), the path
 // behind minigpt4_encode_image (reference minigpt4.cpp:2094-2363).
 //
-// Dense contractions run on the 5th-gen tensor cores: TMA (cp.async.bulk.tensor, 128B swizzle) stages F16 operand
-// tiles in shared memory, one elected thread issues tcgen05.mma kind::f16 with the F32 accumulator in TMEM, and four
-// epilogue warps read it back with tcgen05.ld and fuse bias / GELU / residual / positional-embedding work.
-// ggml numerics (SURVEY §A.3): F16 weights x activations rounded to F16, F32 accumulation — exactly kind::f16.
+// Dense contractions run on the Hopper tensor cores: a producer warp stages F16 operand tiles in shared memory with TMA
+// (cp.async.bulk.tensor, 128B swizzle), two consumer warpgroups issue wgmma.mma_async m64nNk16 (both operands read from
+// shared memory, F32 accumulator in registers) and then fuse bias / GELU / residual / positional-embedding work on it.
+// ggml numerics (SURVEY §A.3): F16 weights x activations rounded to F16, F32 accumulation — exactly f32.f16.f16.
 //
-// "Swap-AB" tiling: UMMA M (128) runs over OUTPUT FEATURES (always a multiple of 128 here), UMMA N over TOKENS
-// (257 = one N=256 MMA + one N=16 MMA into 272 TMEM columns), so each CTA streams its weight slab exactly once.
+// "Swap-AB" tiling: wgmma M (2 x 64) runs over OUTPUT FEATURES (always a multiple of 128 here), wgmma N over TOKENS
+// (one instruction shape per token tile: 32, 80, 144 or 256), so each CTA streams its weight slab exactly once.
 #pragma once
 #include "common.h"
 #include <cuda.h>
@@ -19,9 +19,8 @@ enum GemmEpi : int { GE_BIAS = 0, GE_QSCALE = 1, GE_GELU_F16 = 2, GE_RESID = 3, 
 
 struct GemmArgs {
     int M_out, T, K;          // output features (multiple of 128), valid tokens, contraction (multiple of 64)
-    int t_pad, n1, n2;        // t_pad = round16(T) <= 272; MMA N split
-    int box_rows, n_box;      // TMA copies per stage for the token operand
-    int stages, stage_bytes, tmem_cols;
+    int nt;                   // tokens per CTA = wgmma N (32, 80, 144 or 256); grid.y = ceil(T / nt)
+    int stages, stage_bytes;
     int epi;
     const float *bias;        // [M_out] or null
     float qscale; int qscale_rows;  // GE_QSCALE: rows < qscale_rows are multiplied by qscale after the bias
@@ -29,15 +28,17 @@ struct GemmArgs {
     const float *resid;       // GE_RESID: out = resid + (acc + bias)   (may alias out_f32)
     const float *pos;         // GE_PATCH: out[t+1] = acc + bias + pos[t+1]
     const __half *tab_gelu;
-    int t_tile;               // token split: tokens per CTA, grid.y = ceil(T / t_tile), t_pad == n1 == t_tile, n2 == 0 (0: one CTA takes all tokens)
     int k_split_blocks;       // split-K: 64-wide k-blocks per grid.z slice (0: no split)
     float *partial; long long partial_stride;  // GE_PARTIAL: slice z writes acc (+ bias if z == 0) to partial[z * partial_stride + t * ld_out + m]
 };
+
+constexpr int kGemmThreads = 288;   // warps 0-7 = two consumer warpgroups (64 features each), warp 8 = TMA producer
 
 // ---- raw PTX wrappers ---------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count)); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -51,155 +52,160 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 format: layout type 1 in bits 62-63, SBO = 8 rows * 128 B; LBO unused)
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 format: version 1, layout type 2, SBO = 8 rows * 128 B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, F16 operands from shared memory, F32 accumulator: thread (warp w, lane) of the warpgroup holds
+// d[4 j + 2 h + e] = D[16 w + lane / 4 + 8 h][8 j + 2 (lane % 4) + e]
+__device__ __forceinline__ void wgmma_f16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// instruction descriptor: D=F32, A=B=F16, both K-major, M=128
-__device__ __forceinline__ uint32_t umma_idesc_f16(int n) { return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24); }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                   "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void wgmma_f16(float (&d)[40], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-
+__device__ __forceinline__ void wgmma_f16(float (&d)[72], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n144k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71}, %72, %73, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_f16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 // ---------------------------------------------------------------------------------------------
 // out[t][m] = epi( sum_k W[m][k] * X[t][k] )      W: F16 [M_out][K] (TMA map tmW), X: F16 [T][K] (TMA map tmX)
-// grid = M_out/128 CTAs of 192 threads: warp0 = TMA producer, warp1 = TMEM alloc + MMA issuer, warps 2-5 = epilogue
+// grid.x = M_out/128 CTAs of 288 threads: warps 0-7 = two consumer warpgroups (wgmma + epilogue, 64 features each), warp 8 = TMA producer
 // ---------------------------------------------------------------------------------------------
-// TOKEN SPLIT (grid.y): the CTAs of one 128-feature weight slab take t_tile tokens each, so the T = 257 GEMMs run on 44-144 SMs instead of 11-48
-// (r1_v3 ncu: an 11-CTA GEMM is bound by what ONE SM can pull through TMA, 70 GB/s); rows past T come back from TMA as zeros and are masked in
-// the epilogue.  t_tile == 0: one CTA takes all tokens.
+// TOKEN SPLIT (grid.y): the CTAs of one 128-feature weight slab take NT tokens each, so the T = 257 GEMMs spread over most of the SMs instead
+// of 11-48 of them; rows past T come back from TMA as zeros and are masked in the epilogue.
 // SPLIT-K (grid.z, the two residual GEMMs proj / fc2 whose M is only 1408): a CTA covers the k-blocks [z * k_split_blocks, ...) of its tile and
 // writes raw partial sums (GE_PARTIAL, bias on slice 0); layernorm_fold_kernel folds the slices into the residual stream in slice order
-// (deterministic).  Measured on the 39-block ViT-g + Q-Former encode: 8.69 ms (one CTA per slab) -> 6.57 ms (token split) -> 5.72 ms (+ split-K 3).
-__global__ void __launch_bounds__(192, 1) gemm_f16_tcgen05(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const GemmArgs g) {
+// (deterministic).
+template <int NT>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_f16_wgmma(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const GemmArgs g) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + (size_t)g.stages * g.stage_bytes);
     uint64_t *empty = full + 8;
-    uint64_t *tmem_full = empty + 8;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m_tile = blockIdx.x;
-    const int t0 = (int)blockIdx.y * g.t_tile;  // first token of this CTA
+    const int t0 = (int)blockIdx.y * NT;  // first token of this CTA
     const int num_k_all = g.K / 64;
     const int kb0 = (g.k_split_blocks != 0) ? (int)blockIdx.z * g.k_split_blocks : 0;          // first k-block of this CTA (split-K)
     const int num_k = (g.k_split_blocks != 0) ? min(g.k_split_blocks, num_k_all - kb0) : num_k_all;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
-        for (int i = 0; i < g.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(tmem_full, 1);
+        for (int i = 0; i < g.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }   // a stage is free when the 8 consumer warps have released it
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(g.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
-            const uint32_t tx = 16384u + (uint32_t)g.t_pad * 128u;
+            const uint32_t tx = 16384u + (uint32_t)NT * 128u;
             for (int kb = 0; kb < num_k; ++kb) {
                 const int s = kb % g.stages; const uint32_t ph = (uint32_t)(kb / g.stages) & 1u;
                 mbar_wait(&empty[s], ph ^ 1u);
                 unsigned char *sa = smem + (size_t)s * g.stage_bytes, *sb = sa + 16384;
                 mbar_expect_tx(&full[s], tx);
                 tma_load_2d(sa, &tmW, (kb0 + kb) * 64, m_tile * 128, &full[s]);
-                for (int b = 0; b < g.n_box; ++b) tma_load_2d(sb + (size_t)b * g.box_rows * 128, &tmX, (kb0 + kb) * 64, t0 + b * g.box_rows, &full[s]);
+                tma_load_2d(sb, &tmX, (kb0 + kb) * 64, t0, &full[s]);
             }
         }
-    } else if (warp == 1) {
-        const uint32_t id1 = umma_idesc_f16(g.n1), id2 = umma_idesc_f16(g.n2 ? g.n2 : 16);
-        for (int kb = 0; kb < num_k; ++kb) {
-            const int s = kb % g.stages; const uint32_t ph = (uint32_t)(kb / g.stages) & 1u;
-            mbar_wait(&full[s], ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sa = smem_u32(smem + (size_t)s * g.stage_bytes), sb = sa + 16384u;
+        return;
+    }
+    const int wg = warp >> 2;
+    float acc[NT / 2];
+    for (int kb = 0; kb < num_k; ++kb) {
+        const int s = kb % g.stages; const uint32_t ph = (uint32_t)(kb / g.stages) & 1u;
+        mbar_wait(&full[s], ph);
+        const uint32_t sa = smem_u32(smem + (size_t)s * g.stage_bytes) + (uint32_t)wg * 8192u, sb = sa - (uint32_t)wg * 8192u + 16384u;
+        wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t ad = umma_desc_sw128(sa + k * 32), bd = umma_desc_sw128(sb + k * 32);
-                    tc_mma_f16(tmem_base, ad, bd, id1, (uint32_t)((kb | k) != 0));
-                    if (g.n2) tc_mma_f16(tmem_base + 256u, ad, umma_desc_sw128(sb + 256u * 128u + k * 32), id2, (uint32_t)((kb | k) != 0));
-                }
-                tc_commit(&empty[s]);
-                if (kb == num_k - 1) tc_commit(tmem_full);
-            }
-            __syncwarp();
+        for (int k = 0; k < 4; ++k) wgmma_f16(acc, wgmma_desc_sw128(sa + k * 32), wgmma_desc_sw128(sb + k * 32), (uint32_t)((kb | k) != 0));
+        wgmma_commit();
+        if (kb > 0) {   // one k-block stays in flight: the tensor core has finished reading the previous stage
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(&empty[(kb - 1) % g.stages]);
         }
-    } else {
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const int quarter = warp & 3;
-        const int m = m_tile * 128 + quarter * 32 + lane;
-        const float bias = g.bias ? g.bias[m] : 0.f;
-        const float qs = (g.epi == GE_QSCALE && m < g.qscale_rows) ? g.qscale : 1.0f;
-        for (int c0 = 0; c0 < g.t_pad; c0 += 16) {
-            float v[16];
-            tmem_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0, v);
-            if (g.epi == GE_PARTIAL) {  // split-K slice: raw partial sums (bias rides on slice 0); the following LayerNorm folds the slices into x
-                float *dst = g.partial + (size_t)blockIdx.z * (size_t)g.partial_stride;
-                const float b0 = blockIdx.z == 0 ? bias : 0.f;
+    }
+    wgmma_wait<0>();
+
+    const int m0 = m_tile * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's features: m0 and m0 + 8
+    const int tl = t0 + 2 * (lane & 3);                                      // ... and tokens: tl + 8 j + {0, 1}
+    float bias[2], qs[2];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) { const int t = t0 + c0 + j; if (t < g.T) dst[(size_t)t * g.ld_out + m] = b0 + v[j]; }
-                continue;
+    for (int h = 0; h < 2; ++h) {
+        bias[h] = g.bias ? g.bias[m0 + 8 * h] : 0.f;
+        qs[h] = (g.epi == GE_QSCALE && m0 + 8 * h < g.qscale_rows) ? g.qscale : 1.0f;
+    }
+    // batches of 16 accumulators (four 8-token chunks): value q of a batch is chunk q / 4, feature half (q / 2) % 2, token q % 2
+#pragma unroll
+    for (int jb = 0; jb < NT / 8; jb += 4) {
+        if (g.epi == GE_PARTIAL) {  // split-K slice: raw partial sums (bias rides on slice 0); the following LayerNorm folds the slices into x
+            float *dst = g.partial + (size_t)blockIdx.z * (size_t)g.partial_stride;
+#pragma unroll
+            for (int q = 0; q < 16; ++q) {
+                const int j = jb + (q >> 2), h = (q >> 1) & 1, t = tl + 8 * j + (q & 1);
+                if (j < NT / 8 && t < g.T) dst[(size_t)t * g.ld_out + m0 + 8 * h] = (blockIdx.z == 0 ? bias[h] : 0.f) + acc[(j < NT / 8 ? j : 0) * 4 + (q & 3)];
             }
-            // No early exit inside the 16-token batch: every load of the batch (residual / positional embedding) is issued
-            // before its first use, so the epilogue pays one L2 round trip per batch instead of one per token.
-            float aux[16];
-            if (g.epi == GE_RESID || g.epi == GE_PATCH) {
-                const float *src = g.epi == GE_RESID ? g.resid : g.pos;
-                const int off = g.epi == GE_PATCH ? 1 : 0;
+            continue;
+        }
+        // No early exit inside the batch: every load of the batch (residual / positional embedding) is issued
+        // before its first use, so the epilogue pays one L2 round trip per batch instead of one per token.
+        float aux[16];
+        if (g.epi == GE_RESID || g.epi == GE_PATCH) {
+            const float *src = g.epi == GE_RESID ? g.resid : g.pos;
+            const int off = g.epi == GE_PATCH ? 1 : 0;
 #pragma unroll
-                for (int j = 0; j < 16; ++j) { const int t = t0 + c0 + j; aux[j] = t < g.T ? src[(size_t)(t + off) * g.ld_out + m] : 0.f; }
+            for (int q = 0; q < 16; ++q) {
+                const int j = jb + (q >> 2), h = (q >> 1) & 1, t = tl + 8 * j + (q & 1);
+                aux[q] = (j < NT / 8 && t < g.T) ? src[(size_t)(t + off) * g.ld_out + m0 + 8 * h] : 0.f;
             }
-            if (g.epi == GE_GELU_F16) {
-                __half hv[16];
+        }
+        if (g.epi == GE_GELU_F16) {
+            __half hv[16];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) hv[j] = g.tab_gelu[__half_as_ushort(__float2half_rn(bias + v[j]))];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) { const int t = t0 + c0 + j; if (t < g.T) g.out_f16[(size_t)t * g.ld_out + m] = hv[j]; }
-                continue;
+            for (int q = 0; q < 16; ++q) {
+                const int j = jb + (q >> 2), h = (q >> 1) & 1;
+                hv[q] = g.tab_gelu[__half_as_ushort(__float2half_rn(bias[h] + acc[(j < NT / 8 ? j : 0) * 4 + (q & 3)]))];
             }
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const int t = t0 + c0 + j;
-                if (t < g.T) {
-                    float r = bias + v[j];
-                    switch (g.epi) {
-                        case GE_QSCALE: r *= qs; g.out_f32[(size_t)t * g.ld_out + m] = r; break;
-                        case GE_RESID: g.out_f32[(size_t)t * g.ld_out + m] = aux[j] + r; break;
-                        case GE_PATCH: g.out_f32[(size_t)(t + 1) * g.ld_out + m] = (0.0f + r) + aux[j]; break;
-                        default: g.out_f32[(size_t)t * g.ld_out + m] = r; if (g.out_f16) g.out_f16[(size_t)t * g.ld_out + m] = __float2half_rn(r); break;
-                    }
+            for (int q = 0; q < 16; ++q) {
+                const int j = jb + (q >> 2), h = (q >> 1) & 1, t = tl + 8 * j + (q & 1);
+                if (j < NT / 8 && t < g.T) g.out_f16[(size_t)t * g.ld_out + m0 + 8 * h] = hv[q];
+            }
+            continue;
+        }
+#pragma unroll
+        for (int q = 0; q < 16; ++q) {
+            const int j = jb + (q >> 2), h = (q >> 1) & 1, t = tl + 8 * j + (q & 1), m = m0 + 8 * h;
+            if (j < NT / 8 && t < g.T) {
+                float r = bias[h] + acc[(j < NT / 8 ? j : 0) * 4 + (q & 3)];
+                switch (g.epi) {
+                    case GE_QSCALE: r *= qs[h]; g.out_f32[(size_t)t * g.ld_out + m] = r; break;
+                    case GE_RESID: g.out_f32[(size_t)t * g.ld_out + m] = aux[q] + r; break;
+                    case GE_PATCH: g.out_f32[(size_t)(t + 1) * g.ld_out + m] = (0.0f + r) + aux[q]; break;
+                    default: g.out_f32[(size_t)t * g.ld_out + m] = r; if (g.out_f16) g.out_f16[(size_t)t * g.ld_out + m] = __float2half_rn(r); break;
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(g.tmem_cols) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -217,7 +223,7 @@ __device__ __forceinline__ float warp_max_f(float v) {
     return v;
 }
 // one CTA of 128 threads per row (n <= 1536: 12 values per thread, in registers, one global pass).  A single warp per row made the
-// kernel a ~1900-instruction dependent chain with one warp per scheduler (24 us for 257 x 1408 under ncu, r1_v3); four warps per row
+// kernel a ~1900-instruction dependent chain with one warp per scheduler; four warps per row
 // cut the chain by 4 and give every scheduler of every SM something to overlap.
 __global__ void __launch_bounds__(128) layernorm_kernel(const float *__restrict__ x, int rows, int n, const float *__restrict__ w, const float *__restrict__ b,
                                                         __half *__restrict__ out16, float *__restrict__ out32, const float *__restrict__ add_in /* optional: x + add_in before the norm */) {
@@ -310,7 +316,7 @@ __global__ void __launch_bounds__(128) layernorm_fold_kernel(float *__restrict__
 // q: [nq][ldq] (+ head*DH), k,v: [nk][ldkv] (+ head*DH).  grid (heads, ceil(nq / q_per_cta)), block 256.
 // K ([nk][DH+4], float4 rows, odd float4 pitch -> conflict-free 128-bit reads) and V ([nk][DH]) of the head live in shared
 // memory.  The kernel is shared-memory-bandwidth bound, so each warp processes NQ = 4 queries at a time: every K / V value read from
-// shared memory feeds 4 FMAs (r1_v3 ncu: the two-query version ran at 6 % of the FP32 peak, 79 us per ViT block).  The per-warp
+// shared memory feeds 4 FMAs.  The per-warp
 // scratch holds the warp's q rows while the scores are formed and is then reused for its probability rows.  Per element the
 // arithmetic (FMA order over d and over keys, LUT exp, double sum) is unchanged.  out: F16 [nq][ld_out] (operand of the next GEMM).
 // ---------------------------------------------------------------------------------------------

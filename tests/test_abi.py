@@ -71,21 +71,7 @@ def test_model_load_missing_path_returns_null(lib):
 
 def test_quantize_missing_input(lib):
     with pytest.raises(RuntimeError, match="PathDoesNotExist"):
-        lib.minigpt4_quantize_model("/nonexistent/in.bin", "/tmp/out.bin", 5)
-
-
-def test_reference_binding_binds_unmodified(lib):
-    """The reference's own ctypes file (when mounted) must bind to the new .so without edits."""
-    ref = Path("/root/reference/minigpt4/minigpt4_library.py")
-    if not ref.exists():
-        pytest.skip("reference tree not mounted on this box")
-    import importlib.util
-    from minigpt4_cpp_b200.build import OUT
-    spec = importlib.util.spec_from_file_location("ref_minigpt4_library", ref)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    rlib = mod.MiniGPT4SharedLibrary(str(OUT))
-    assert rlib.minigpt4_is_eos("x###") and rlib.minigpt4_contains_eos_token("##")
+        lib.minigpt4_quantize_model("/nonexistent/in.bin", "/nonexistent/out.bin", 5)
 
 
 def test_null_arguments_are_harmless(lib):
@@ -108,7 +94,7 @@ def test_model_load_without_a_device_is_an_error_code_not_an_abort(lib, tmp_path
     from minigpt4_cpp_b200 import modelgen as mg
     ext = m.B200(lib)
     if ext.L.minigpt4_b200_device_count() > 0:
-        pytest.skip("this box has a CUDA device")
+        pytest.skip("a CUDA device is present")
     p = str(tmp_path / "llama.bin")
     mg.write_llama_ggjt(p, mg.LlamaSpec(n_vocab=1024, n_embd=128, n_head=1, n_layer=1, wtype="q4_1"))
     assert ext.L.minigpt4_b200_llm_load(p.encode(), 32, 1, 0) is None

@@ -1,5 +1,5 @@
 """Device paths of the remaining ggjt block types - Q4_K (dot2_q4k) and Q5_0 / Q5_1 / Q8_0 (dot2_b32), their repack and token-embedding kernels:
-bit-identical to the CPU oracle (first run on hardware in round 2: 68 cases green, profiles/r2_call_block_types.txt)."""
+bit-identical to the CPU oracle."""
 import os
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""Tensor-core prefill (csrc/llama_prefill.cuh, tcgen05 kind::i8): prompt / prefix rows must be BIT-IDENTICAL to the per-op matvec path and
+"""Tensor-core prefill (csrc/llama_prefill.cuh, wgmma s8): prompt / prefix rows must be BIT-IDENTICAL to the per-op matvec path and
 to the CPU oracle for any number of rows - the epilogue keeps the canonical float order (per-class sequential sums + xor-butterfly tree).
 Reference behaviour: llama_eval_embd with N = 32 in one batch (minigpt4.cpp:2405-2412), llama_eval in n_batch chunks (:2369-2379)."""
 import numpy as np

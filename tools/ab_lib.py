@@ -1,4 +1,4 @@
-"""A/B timing of several builds of libminigpt4.so on the SAME box (bisection of a decode regression): 7B-wide 4-layer Q4_1 model, 32-row prefix,
+"""A/B timing of several builds of libminigpt4.so on the SAME GPU in one process (bisection of a decode regression): 7B-wide 4-layer Q4_1 model, 32-row prefix,
 128 device-chained greedy tokens, best of 3.  Only the oldest C entry points are used.   python tools/ab_lib.py build/ab/libA.so build/ab/libB.so ..."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

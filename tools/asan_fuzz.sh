@@ -1,7 +1,6 @@
 #!/bin/bash
 # Host-side robustness run (no GPU): the file readers, the container quantiser, the tokenizer / samplers and the image decoders are compiled
 # stand-alone with AddressSanitizer + UndefinedBehaviorSanitizer and fed damaged inputs.     bash tools/asan_fuzz.sh [iterations-scale]
-# Last run: profiles/r2_host_asan_fuzz.txt
 set -e
 cd "$(dirname "$0")/.."
 S=${1:-1}; W=/tmp/mg4fuzz; mkdir -p $W

@@ -1,4 +1,4 @@
-"""Round-2 cross-check (GPU box only; NOT part of the test suite, never on the product path): pin the oracle's restatement of ggml's
+"""Cross-check (needs a GPU and vLLM; NOT part of the test suite, never on the product path): pin the oracle's restatement of ggml's
 quantised mul_mat against kernels that DESCEND from ggml itself.  vLLM (library code in this image) ships llama.cpp's CUDA MMVQ /
 dequantise kernels as `torch.ops._C.ggml_mul_mat_vec_a8` / `ggml_dequantize`: activations quantised to q8_1, integer block dots,
 the block layouts of ggml — i.e. the arithmetic this repo could only restate from memory ("parity unpinned", DESIGN.md §2).
@@ -7,7 +7,7 @@ Prints, per block type, (a) dequantiser: vLLM vs oracle, expected exact after ro
 CUDA kernel.  ggml-cuda's q8_1 keeps d and s as halves and reduces in another order, so (b) agrees to ~1e-3 relative, not bit for bit;
 a layout or formula error (nibble order, the `- 8`, the m * s term, the K-quant scale packing) would show up as O(1).
 
-    python tools/crosscheck_vllm_gguf.py            # on a B200 box:  gpurun -- 'python tools/crosscheck_vllm_gguf.py'
+    python tools/crosscheck_vllm_gguf.py            # on a machine with an H100 and vLLM installed
 """
 import os
 import sys

@@ -1,15 +1,17 @@
 #!/bin/bash
-# Full 1-GPU check-out: canary, GPU suite, bench (both arms), ncu captures.   gpurun --timeout 2400 -- 'bash tools/gpu_full.sh'
-mkdir -p gpurun_out
-TAG=${TAG:-r2_final}
-run() { name=$1; shift; t=$1; shift; echo "=== $name"; timeout -k 5 $t "$@" > gpurun_out/$name.log 2>&1; rc=$?; echo "exit $rc"; tail -n ${TAILN:-12} gpurun_out/$name.log; return $rc; }
+# Full 1-GPU check-out on an H100: canary, GPU suite, prefill timing, bench (both arms), torch.profiler kernel tables, per-op trace, smoke.
+# Logs go to $OUT (default: a fresh temporary directory, printed at the end).
+OUT=${OUT:-$(mktemp -d)}
+mkdir -p "$OUT"
+run() { name=$1; shift; t=$1; shift; echo "=== $name"; timeout -k 5 $t "$@" > "$OUT/$name.log" 2>&1; rc=$?; echo "exit $rc"; tail -n ${TAILN:-12} "$OUT/$name.log"; return $rc; }
+nvidia-smi --query-gpu=name,power.limit,clocks.max.sm --format=csv > "$OUT/gpu.csv"
 TAILN=6 run canary6 300 python tools/canary.py || exit 1
 TAILN=8 run pytest_gpu 900 python -m pytest tests -m gpu -q -p no:cacheprovider
 TAILN=3 run prefill_plain 300 python tools/prof_prefill.py
 TAILN=3 run bench 600 python bench.py
 TAILN=3 run bench_reference 600 python bench.py --impl reference --steps 2 --warmup 1
-TAILN=2 run ncu_mega 420 ncu --set full --clock-control none --import-source on -k regex:decode_megakernel -s 10 -c 2 -o gpurun_out/${TAG}_mega -f python tools/prof_decode.py
-TAILN=2 run ncu_turn 900 ncu --metrics gpu__time_duration.sum --clock-control none -k 'regex:decode_megakernel|prefill|stage_rows|attn_kernel|gemm_f16|attention_f32|layernorm|im2col|cls_row|matvec_kernel|embed_rows|finalize' -c 1200 --csv --log-file gpurun_out/${TAG}_turn_launches.csv python tools/prof_turn.py
+TAILN=40 run prof_decode 420 python tools/torch_prof.py tools/prof_decode.py
+TAILN=40 run prof_turn 900 python tools/torch_prof.py tools/prof_turn.py
 TAILN=30 run trace6 200 python tools/mega_trace.py
-python -c "import ctypes; l=ctypes.CDLL('build/libminigpt4.so'); print('smoke via __graft_entry__')"; timeout 300 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/smoke.log 2>&1; tail -2 gpurun_out/smoke.log
-echo done
+TAILN=2 run smoke 300 python -c "import __graft_entry__ as g; g.smoke()"
+echo "done: logs in $OUT"

@@ -1,5 +1,5 @@
 """Lean profiling target: Vicuna-7B-shaped Q4_1 model (synthetic), 32-row prefix, then N chained decode steps.
-Run under ncu with -k regex:decode_megakernel (see tools/gpu_full.sh)."""
+Run under a profiler (python tools/torch_prof.py tools/prof_decode.py prints the kernel table)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

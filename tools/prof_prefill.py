@@ -1,5 +1,5 @@
 """Profiling target for the prompt path: Vicuna-7B-shaped Q4_1 model (synthetic), a 32-row embedding prefix and a 45-row mixed prompt.
-Run under ncu with a -k regex that excludes the load-time kernels (see tools/gpu_full.sh)."""
+Run under a profiler (python tools/torch_prof.py tools/prof_prefill.py prints the kernel table)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

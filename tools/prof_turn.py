@@ -1,5 +1,5 @@
 """Profiling target: ONE chat turn through the reference ABI (7B q4_1 + ViT-g f16, synthetic): encode, system prompt + begin_chat_image (one merged
-prefill pass), N greedy tokens.  Run under ncu with a -k regex that excludes the load-time kernels (tools/gpu_full.sh) for the launch list of a step."""
+prefill pass), N greedy tokens.  Run under a profiler (python tools/torch_prof.py tools/prof_turn.py) for the kernel table of a step."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

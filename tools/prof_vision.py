@@ -1,5 +1,5 @@
 """Lean profiling target for the vision graph: full-size ViT-g + Q-Former (synthetic F16 weights), two encodes.
-Run under ncu with -k regex:gemm_f16|attention_f32|layernorm (see tools/gpu_full.sh)."""
+Run under a profiler (python tools/torch_prof.py tools/prof_vision.py prints the kernel table)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -1,10 +1,10 @@
 """What the kernels are made of: per kernel of build/llama.cu.o, build/vision.cu.o and build/tp.cpp.o the counts of the SASS mnemonics that prove
-the Blackwell paths (B200_PROFILING.md): UTCHMMA / UTCIMMA (tcgen05.mma f16 / i8), LDTM (tcgen05.ld), UTMALDG (TMA tensor load), UBLKCP
-(cp.async.bulk), SYNCS (mbarrier), IDP.4A (dp4a).   python tools/sass_census.py > profiles/r2_sass_census.txt"""
+the Hopper paths: HGMMA / IGMMA (wgmma f16 / s8), WARPGROUP (wgmma fences and waits), UTMALDG (TMA tensor load), UBLKCP
+(cp.async.bulk), SYNCS (mbarrier), IDP.4A (dp4a).   python tools/sass_census.py   (after a build; prints to stdout)"""
 import re, subprocess, sys, collections
 from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
-PAT = ["UTCHMMA", "UTCIMMA", "UTCQMMA", "LDTM", "UTMALDG", "UBLKCP", "UBLKPF", "SYNCS", "IDP.4A", "HMMA", "IMMA", "LDG", "LDS", "SHFL", "BAR.SYNC", "ATOMG", "REDG"]
+PAT = ["HGMMA", "IGMMA", "WARPGROUP", "UTMALDG", "UBLKCP", "UBLKPF", "SYNCS", "IDP.4A", "HMMA", "IMMA", "LDG", "LDS", "SHFL", "BAR.SYNC", "ATOMG", "REDG"]
 for obj in ("llama.cu.o", "vision.cu.o", "tp.cpp.o"):
     out = subprocess.run(["cuobjdump", "-sass", str(ROOT / "build" / obj)], capture_output=True, text=True).stdout
     cur, counts = None, collections.OrderedDict()

@@ -1,11 +1,11 @@
 """Guard against unintended code-generation changes in kernels that have been measured: md5 of each kernel's SASS (addresses and encodings
-stripped) in build/llama.cu.o and build/vision.cu.o against profiles/sass_hashes.json.
+stripped) in build/llama.cu.o and build/vision.cu.o against build/sass_hashes.json (a local record, not committed).
 
     python tools/sass_guard.py            # compare; lists changed / new / vanished kernels
     python tools/sass_guard.py --write    # record the current build as the baseline (do this right after a measured GPU run)
 
-Used at the end of round 1 to add experimental variants (llama_mega_ll.cuh, token-split / split-K GEMMs, extra block types) while proving
-that every kernel behind the published numbers stayed byte-identical (ptxas output is sensitive even to a kernel-parameter struct growing)."""
+Use: record after a measured run, then add experimental variants while proving that every measured kernel stayed byte-identical
+(ptxas output is sensitive even to a kernel-parameter struct growing)."""
 import hashlib
 import json
 import re
@@ -14,7 +14,7 @@ import sys
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-BASE = ROOT / "profiles" / "sass_hashes.json"
+BASE = ROOT / "build" / "sass_hashes.json"
 
 
 def hashes() -> dict[str, str]:
@@ -41,6 +41,8 @@ if __name__ == "__main__":
         BASE.write_text(json.dumps(cur, indent=0, sort_keys=True))
         print(f"recorded {len(cur)} kernels in {BASE}")
         sys.exit(0)
+    if not BASE.exists():
+        sys.exit(f"no baseline recorded: run with --write after a measured run ({BASE})")
     base = json.loads(BASE.read_text())
     changed = sorted(k for k in base if k in cur and base[k] != cur[k])
     gone = sorted(k for k in base if k not in cur)

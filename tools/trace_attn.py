@@ -1,6 +1,6 @@
 import os, sys
 os.environ["MINIGPT4_B200_MEGA_TRACE"] = "1"
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, os.getcwd())
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import minigpt4_cpp_b200 as m, bench
 from minigpt4_cpp_b200 import modelgen as mg

@@ -1,11 +1,11 @@
-// ubench_stream.cu — primitive measurements behind the decode megakernel design (stand-alone; nvcc -arch=sm_100a).
+// ubench_stream.cu — primitive measurements behind the decode megakernel design (stand-alone; nvcc -arch=sm_90a).
 //   T1  per-warp self-refilled TMA stream: every consumer warp owns two shared-memory slots and re-arms a slot itself right after
 //       consuming it (no producer warp, no "empty" barriers).  work = 0 (wait only), 1 (read the slot), 2 (Q4_1 dot, register activations)
 //   T2  T1 + a warp that asks L2 for the CTA's stream `window` bytes ahead (cp.async.bulk.prefetch.L2)
 //   T4  grid barrier round trip, variants
 //   T5  grid barrier + every CTA gathers a 16 KB vector from L2 (the activation exchange of one op)
 //   T6  direct global->register streaming (ld.global.nc.v4, 8 in flight per lane)
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o build/ubench_stream tools/ubench_stream.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o build/ubench_stream tools/ubench_stream.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
