@@ -1,6 +1,7 @@
 """Fast GPU canary for the decode megakernel: bit-exact against the CPU oracle on seeded tiny models, at short AND long positions
-(the in-kernel attention has a one-pass regime below 192 keys and a multi-pass regime above), Q4_1 and Q4_0, plus a 7B-wide
-2-layer model (the production row widths).  ~20 s; run before spending GPU minutes on anything else."""
+(the in-kernel attention has a one-pass regime below 192 keys and a multi-pass regime above), Q4_1 and Q4_0, plus 7B- and 13B-wide
+2-layer models (the production row widths; 13B: five register-resident blocks per lane, fewer stream warps).  ~30 s; run before spending
+GPU minutes on anything else."""
 import os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -16,7 +17,9 @@ with tempfile.TemporaryDirectory() as d:
              ("q4_0", dict(n_vocab=1024, n_embd=512, n_head=4, n_layer=2), 40, 12),
              ("q4_1", dict(n_vocab=2048, n_embd=4096, n_head=32, n_layer=2), 180, 20),
              ("q5_k", dict(n_vocab=1024, n_embd=512, n_head=4, n_layer=2), 200, 12),
-             ("q5_k", dict(n_vocab=2048, n_embd=4096, n_head=32, n_layer=2), 60, 12)]
+             ("q5_k", dict(n_vocab=2048, n_embd=4096, n_head=32, n_layer=2), 60, 12),
+             ("q4_1", dict(n_vocab=2048, n_embd=5120, n_head=40, n_layer=2), 230, 12),
+             ("q5_k", dict(n_vocab=2048, n_embd=5120, n_head=40, n_layer=2), 60, 12)]
     for wt, dims, n_prompt, n_gen in cases:
         p = f"{d}/llama-{wt}-{dims['n_embd']}.bin"
         mg.write_llama_ggjt(p, mg.LlamaSpec(wtype=wt, **dims))
