@@ -49,6 +49,31 @@ MINIGPT4_API const char *minigpt4_b200_token_text(struct MiniGPT4Context *ctx, i
  * fed; *ms_out the CUDA-event time of the loop.  The bench's device-resident `value` leg. */
 MINIGPT4_API int minigpt4_b200_decode_chain(struct MiniGPT4Context *ctx, int steps, int32_t *ids_out, float *ms_out);
 
+/* multi-session serving: several conversations over one loaded model ------------------------------------------------
+ * A session is a MiniGPT4Context that shares the model of `ctx` (language and vision weights, the prefill operand cache and
+ * scratch, encode lanes, tokenizer) and owns a conversation: its KV cache of ctx's n_ctx positions, n_past, prompt queue,
+ * logits, device state, decode graph / megakernel and a sampler seeded with `seed`.  All 18 entry points of minigpt4.h work
+ * on it.  ctx and its sessions form a group; they may be freed in any order and the weights go with the last of them.
+ * The contexts of one group must not be called from two threads at once (the reference's contract for one context).
+ * Returns NULL on failure (device memory exhausted, a tensor-parallel ctx, ctx NULL). */
+MINIGPT4_API struct MiniGPT4Context *minigpt4_b200_session_create(struct MiniGPT4Context *ctx, int seed);
+/* live contexts of ctx's group; device bytes ctx owns (KV cache 2 * n_layer * n_ctx * n_embd * 2 B plus its activations of
+ * 512 prompt rows and a few small buffers); device bytes it shares with its group (weights, operand cache, tables, prefill
+ * scratch, the batched step's workspace once built).  Any pointer may be NULL. */
+MINIGPT4_API int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_contexts, double *owned_bytes, double *shared_bytes);
+/* One decode step of n (1..8) distinct contexts of one group: the weights stream once for all of them.  Context i is fed ids[i]
+ * (ids[i] < 0: its current on-device greedy id, as in minigpt4_b200_decode_chain) at its own n_past; queued prompt pieces of
+ * each context are evaluated first.  Afterwards each context has new logits, n_past + 1, and ids_out[i] = its new greedy id;
+ * its logits are the bits a step on its own gives.  Synchronous.  NULL or duplicate contexts, contexts of different groups,
+ * n outside 1..8, a full context or an id >= n_vocab return the FailedToAddString error code (8) and change no context. */
+MINIGPT4_API int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, int32_t *ids_out);
+/* minigpt4_end_chat on each context in turn (each samples from its own logits with its own sampler; greedy uses the device
+ * arg-max; tokens[i] = the sampled token's text), then the n sampled ids are fed in one minigpt4_b200_decode_batch step.
+ * The batch is validated before any sampling. */
+MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p,
+                                              float tfs_z, float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
+                                              float alpha_frequency, int mirostat, float mirostat_tau, float mirostat_eta, int penalize_nl);
+
 /* batch encode (config 5): n images -> n embeddings, same semantics per image as minigpt4_encode_image */
 MINIGPT4_API int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, IN struct MiniGPT4Images *images, OUT struct MiniGPT4Embeddings *embeddings);
 

@@ -197,6 +197,29 @@ int minigpt4_b200_decode_chain(struct MiniGPT4Context *ctx, int steps, int32_t *
     if (ms_out) *ms_out = ms;
     return 0;
 }
+struct MiniGPT4Context *minigpt4_b200_session_create(struct MiniGPT4Context *ctx, int seed) {
+    if (!ctx) return nullptr;
+    Engine *e = new Engine();
+    if (Error err = e->init_session(*E(ctx), seed)) { MG4_ERR("Failed to create a session: %s", error_name(err)); delete e; return nullptr; }
+    return reinterpret_cast<struct MiniGPT4Context *>(e);
+}
+int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_contexts, double *owned_bytes, double *shared_bytes) {
+    if (!ctx) return ErrLoadLanguageModel;
+    const LlamaDevice &l = E(ctx)->llm();
+    if (n_contexts) *n_contexts = l.group_size();
+    if (owned_bytes) *owned_bytes = (double)l.owned_bytes();
+    if (shared_bytes) *shared_bytes = (double)l.shared_bytes();
+    return 0;
+}
+int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, int32_t *ids_out) {
+    return Engine::decode_batch(reinterpret_cast<Engine *const *>(ctxs), n, ids, ids_out);
+}
+int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p, float tfs_z,
+                                 float typical_p, int32_t /*repeat_last_n*/, float /*repeat_penalty*/, float /*alpha_presence*/,
+                                 float /*alpha_frequency*/, int mirostat, float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {
+    SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    return Engine::end_chat_batch(reinterpret_cast<Engine *const *>(ctxs), n, tokens, sp);
+}
 int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, struct MiniGPT4Images *images, struct MiniGPT4Embeddings *embeddings) {
     if (embeddings->n_embeddings < images->n_images) return ErrImageSize;
     return E(ctx)->encode_images(images->images, images->n_images, embeddings->embeddings, nullptr);

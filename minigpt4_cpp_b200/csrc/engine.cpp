@@ -11,7 +11,7 @@ TPConfig g_tp_config;
 
 Engine::~Engine() {
     llm_.reset();
-    vis_lanes_.clear();   // (lanes borrow the first lane's weights)
+    vis_lanes_.reset();   // (lanes borrow the first lane's weights)
     vis_.reset();
     tp.destroy();
 }
@@ -34,7 +34,7 @@ Error Engine::init(const std::string &path, const std::string &llm_path, int ver
             const double t0 = now_ms();
             LlamaFile lf;
             if (!lf.load(llm_path)) { MG4_ERR("failed to read language model %s", llm_path.c_str()); return ErrLoadLanguageModel; }
-            tok_.init(lf.vocab);
+            tok_->init(lf.vocab);
             llm_.reset(new LlamaDevice());
             if (!llm_->load(lf, n_ctx > 0 ? n_ctx : 2048, tp.world > 1 ? &tp : nullptr)) return ErrLoadLanguageModel;
             MG4_INFO("Load language model took %.0f ms", now_ms() - t0);
@@ -63,6 +63,61 @@ Error Engine::init(const std::string &path, const std::string &llm_path, int ver
     return ErrNone;
 }
 
+Error Engine::init_session(const Engine &parent, int seed) {
+    if (parent.tp.world > 1) { MG4_ERR("sessions of a tensor-parallel context are not supported"); return ErrLoadLanguageModel; }
+    vfile_ = parent.vfile_; vis_ = parent.vis_; vis_lanes_ = parent.vis_lanes_; tok_ = parent.tok_;
+    n_batch_ = parent.n_batch_;
+    try {
+        LoadScope loading;   // device memory exhausted -> an error code, not an abort
+        llm_.reset(new LlamaDevice());
+        if (!llm_->load_session(*parent.llm_)) return ErrLoadLanguageModel;
+    } catch (const LoadFailure &f) {
+        fprintf(stderr, "[minigpt4-b200][error] session: %s\n", f.msg);
+        return ErrLoadLanguageModel;
+    } catch (const std::exception &e) {
+        fprintf(stderr, "[minigpt4-b200][error] session: %s\n", e.what());
+        return ErrLoadLanguageModel;
+    }
+    sampler_.reset(new Sampler(seed));
+    logits_.resize((size_t)llm_->dims().n_vocab);
+    return ErrNone;
+}
+
+// Batched decode (extension): every check happens before anything runs, so a refused batch leaves every context as it was.
+bool Engine::batch_valid(Engine *const *e, int n, const int32_t *ids) {
+    if (!e || n < 1 || n > 8) { MG4_ERR("decode_batch: %d contexts (1 .. 8)", n); return false; }
+    for (int i = 0; i < n; ++i) {
+        if (!e[i]) { MG4_ERR("decode_batch: context %d is NULL", i); return false; }
+        for (int j = 0; j < i; ++j) if (e[j] == e[i]) { MG4_ERR("decode_batch: context %d appears twice", i); return false; }
+        if (e[i]->llm_->group() != e[0]->llm_->group()) { MG4_ERR("decode_batch: context %d serves another model", i); return false; }
+        const LlamaDims &d = e[i]->llm_->dims();
+        if (e[i]->n_past_ + 1 > d.n_ctx) { MG4_ERR("decode_batch: context %d is full (n_ctx %d)", i, d.n_ctx); return false; }
+        if (ids && ids[i] >= d.n_vocab) { MG4_ERR("decode_batch: token id %d out of range", ids[i]); return false; }
+    }
+    return true;
+}
+Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out) {
+    if (!ids || !ids_out || !batch_valid(e, n, ids)) return ErrFailedToAddString;
+    for (int i = 0; i < n; ++i) if (!e[i]->flush()) return ErrFailedToAddString;   // queued prompt rows: each context's own prefill pass
+    if (n == 1) {   // one context: its own decode graph or megakernel, exactly as add_tokens' single-token step
+        Engine &c = *e[0];
+        if (!c.llm_->decode_step(ids[0], c.n_past_)) return ErrFailedToAddString;
+        ids_out[0] = c.llm_->argmax();
+    } else {
+        LlamaDevice *L[8]; int np[8];
+        for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; }
+        LlamaDevice::decode_batch(L, n, ids, np, ids_out);
+    }
+    for (int i = 0; i < n; ++i) e[i]->n_past_ += 1;
+    return ErrNone;
+}
+Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p) {
+    if (!tokens || !batch_valid(e, n, nullptr)) return ErrFailedToAddString;   // (before any sampler draws)
+    int32_t ids[8], out[8];
+    for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
+    return decode_batch(e, n, ids, out);
+}
+
 // input validation = reference minigpt4.cpp:2130-2138
 Error Engine::encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out) {
     if (!vis_) MG4_PANIC("encode_image on a context loaded without a vision model");
@@ -87,18 +142,18 @@ Error Engine::encode_images(const ::MiniGPT4Image *images, size_t n, ::MiniGPT4E
         if (images[i].format != MINIGPT4_IMAGE_FORMAT_F32) return ErrImageNotF32;
     }
     const size_t lanes = std::min<size_t>(n, (size_t)kEncodeLanes);
-    while (vis_lanes_.size() + 1 < lanes) {
+    while (vis_lanes_->size() + 1 < lanes) {
         std::unique_ptr<VisionDevice> l(new VisionDevice());
         try {
             LoadScope loading;   // (a lane that does not fit in device memory is an error code, not an abort)
             if (Error e = l->load(*vfile_, vis_.get())) return e;
         } catch (const LoadFailure &f) {
-            fprintf(stderr, "[minigpt4-b200][error] encode lane %zu: %s\n", vis_lanes_.size() + 1, f.msg);
+            fprintf(stderr, "[minigpt4-b200][error] encode lane %zu: %s\n", vis_lanes_->size() + 1, f.msg);
             return ErrLoadModelFileHeader;
         }
-        vis_lanes_.push_back(std::move(l));
+        vis_lanes_->push_back(std::move(l));
     }
-    auto lane = [&](size_t k) { return k == 0 ? vis_.get() : vis_lanes_[k - 1].get(); };
+    auto lane = [&](size_t k) { return k == 0 ? vis_.get() : (*vis_lanes_)[k - 1].get(); };
     const size_t ne = (size_t)32 * vis_->dims().n_embd_llm;
     const double t0 = now_ms();
     for (size_t base = 0; base < n; base += lanes) {
@@ -142,7 +197,7 @@ Error Engine::add_tokens(const std::vector<int32_t> &tokens) {
     return ErrNone;
 }
 // add_strings (minigpt4.cpp:2384-2397): add_bos is ALWAYS true
-Error Engine::add_strings(const char *s) { return add_tokens(tok_.encode(s ? s : "", true)); }
+Error Engine::add_strings(const char *s) { return add_tokens(tok_->encode(s ? s : "", true)); }
 
 Error Engine::add_embedding(const float *rows, int n_rows) {
     if (n_rows <= 0) return ErrNone;
@@ -181,7 +236,7 @@ int32_t Engine::sample_token(const SamplingParams &p) {
 }
 const char *Engine::id_to_token(int32_t id) const {  // minigpt4.cpp:2485-2497
     if (id == 2) return "</s>";
-    return tok_.piece(id);
+    return tok_->piece(id);
 }
 
 }  // namespace mg4

@@ -21,6 +21,13 @@ public:
     ~Engine();
     // path may be empty (language model only, extension entry point)
     Error init(const std::string &path, const std::string &llm_path, int verbosity, int seed, int n_ctx, int n_batch, bool numa);
+    // a session: a new conversation over the model of `parent` (language and vision weights, encode lanes, tokenizer shared; own KV
+    // cache, prompt queue, logits, state and a sampler seeded with `seed`)
+    Error init_session(const Engine &parent, int seed);
+    // one decode step of n (1..8) distinct contexts of one group, weights streamed once (see minigpt4_b200_decode_batch); all or nothing
+    static Error decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out);
+    // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
+    static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
     static constexpr int kEncodeLanes = 8;
     Error encode_images(const ::MiniGPT4Image *images, size_t n, ::MiniGPT4Embedding *out, float *total_ms);   // batched: concurrent lanes
@@ -36,7 +43,7 @@ public:
     bool has_vision() const { return (bool)vis_; }
     VisionDevice *vision() { return vis_.get(); }
     LlamaDevice &llm() { return *llm_; }
-    Tokenizer &tokenizer() { return tok_; }
+    Tokenizer &tokenizer() { return *tok_; }
     int n_past() const { return n_past_; }
     void advance(int n) { n_past_ += n; }
     int n_embd_llm() const { return llm_->dims().n_embd; }
@@ -44,11 +51,13 @@ public:
     TPLink tp;
 
 private:
-    std::unique_ptr<VisionFile> vfile_;
-    std::unique_ptr<VisionDevice> vis_;
-    std::vector<std::unique_ptr<VisionDevice>> vis_lanes_;   // lanes 1.. of the batched encode (lane 0 = vis_)
+    static bool batch_valid(Engine *const *e, int n, const int32_t *ids);
+    // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)
+    std::shared_ptr<VisionFile> vfile_;
+    std::shared_ptr<VisionDevice> vis_;
+    std::shared_ptr<std::vector<std::unique_ptr<VisionDevice>>> vis_lanes_ = std::make_shared<std::vector<std::unique_ptr<VisionDevice>>>();   // lanes 1.. of the batched encode (lane 0 = vis_)
+    std::shared_ptr<Tokenizer> tok_ = std::make_shared<Tokenizer>();
     std::unique_ptr<LlamaDevice> llm_;
-    Tokenizer tok_;
     std::unique_ptr<Sampler> sampler_;
     std::vector<float> logits_;
     int n_past_ = 0;

@@ -2,6 +2,7 @@
 #include "llama_kernels.cuh"
 #include "llama_mega6.cuh"
 #include "llama_prefill.cuh"
+#include "llama_sessions.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -12,6 +13,32 @@ namespace mg4 {
 using namespace k;
 
 static size_t g_max_dyn_smem = 0;
+
+// device bytes allocated by this thread through dmalloc: the owned / shared split that minigpt4_b200_session_info reports
+static thread_local size_t t_dev_bytes = 0;
+template <class T> static void dmalloc(T **p, size_t n) { CUDA_CHECK(cudaMalloc((void **)p, n)); t_dev_bytes += n; }
+
+// what the contexts of one model share besides the weight pointers each of them holds: the batched decode step's workspace,
+// stream and graphs (built by the group's first decode_batch of each size)
+struct LlamaGroup {
+    size_t weight_bytes = 0;       // the parent's load minus its own context: weights, operand cache, tables, prefill scratch
+    size_t batch_bytes = 0;
+    cudaStream_t stream = nullptr;
+    float *x = nullptr, *q = nullptr, *att = nullptr, *act = nullptr;   // [8] rows
+    unsigned char *qact = nullptr;
+    DeviceState *state = nullptr;  // the batch's tokens (embed_* gather column t from tokens[t])
+    SessionSlot *slots = nullptr, *h_slots = nullptr;
+    int *ids = nullptr, *h_ids = nullptr;
+    cudaGraphExec_t graph[9] = {};
+    int graph_kernels[9] = {};
+    ~LlamaGroup() {
+        for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
+        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)qact, (void *)state, (void *)slots, (void *)ids}) if (p) cudaFree(p);
+        if (h_slots) cudaFreeHost(h_slots);
+        if (h_ids) cudaFreeHost(h_ids);
+        if (stream) cudaStreamDestroy(stream);
+    }
+};
 
 template <int WT, int NT>
 static void launch_mv(const MatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
@@ -73,6 +100,54 @@ static void launch_matvec(MatvecArgs a, int nt, int sm_count, cudaStream_t s, un
     if (counter) ++*counter;
 }
 
+// the batched decode step's QKV and logits matrices (llama_sessions.cuh): same grid and staging as launch_matvec
+template <int WT, int NT>
+static void launch_mvs(const SessionMatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
+    static bool configured[64] = {};
+    int dev = 0; cudaGetDevice(&dev);
+    if (!configured[dev & 63]) {
+        CUDA_CHECK(cudaFuncSetAttribute(matvec_sessions_kernel<WT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g_max_dyn_smem));
+        configured[dev & 63] = true;
+    }
+    matvec_sessions_kernel<WT, NT><<<grid, kThreads, smem, s>>>(a);
+}
+template <int WT>
+static void launch_mvs_nt(int nt, const SessionMatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
+    switch (nt) {
+        case 1: launch_mvs<WT, 1>(a, grid, smem, s); break;
+        case 2: launch_mvs<WT, 2>(a, grid, smem, s); break;
+        case 4: launch_mvs<WT, 4>(a, grid, smem, s); break;
+        default: launch_mvs<WT, 8>(a, grid, smem, s); break;
+    }
+}
+static void launch_matvec_sessions(const MatvecArgs &m, const SessionSlot *slots, size_t kv_off, int nt, int sm_count, cudaStream_t s, unsigned long long *counter,
+                                   bool restage = true) {
+    if (restage) launch_stage(m, s, counter);
+    SessionMatvecArgs a{m, slots, kv_off};
+    const int rows = m.w.rows;
+    const int target = 2 * sm_count * kWarps;
+    int rpw = (rows + target - 1) / target;
+    rpw = std::max(2, (rpw + 1) & ~1);
+    a.m.rows_per_warp = rpw;
+    const int grid = (rows + kWarps * rpw - 1) / (kWarps * rpw);
+    const size_t smem = (size_t)nt * act_bytes(act_of(m.w.type), m.w.cols);
+    if (smem > g_max_dyn_smem) MG4_PANIC("activation staging needs %zu B of shared memory (> %zu)", smem, g_max_dyn_smem);
+    switch (m.w.type) {
+        case GG_Q4_0: launch_mvs_nt<GG_Q4_0>(nt, a, grid, smem, s); break;
+        case GG_Q4_1: launch_mvs_nt<GG_Q4_1>(nt, a, grid, smem, s); break;
+        case GG_Q5_K: launch_mvs_nt<GG_Q5_K>(nt, a, grid, smem, s); break;
+        case GG_Q4_K: launch_mvs_nt<GG_Q4_K>(nt, a, grid, smem, s); break;
+        case GG_Q5_0: launch_mvs_nt<GG_Q5_0>(nt, a, grid, smem, s); break;
+        case GG_Q5_1: launch_mvs_nt<GG_Q5_1>(nt, a, grid, smem, s); break;
+        case GG_Q8_0: launch_mvs_nt<GG_Q8_0>(nt, a, grid, smem, s); break;
+        case GG_Q6_K: launch_mvs_nt<GG_Q6_K>(nt, a, grid, smem, s); break;
+        case GG_F16: launch_mvs_nt<GG_F16>(nt, a, grid, smem, s); break;
+        default: MG4_PANIC("no matvec kernel for ggml type %d", m.w.type);
+    }
+    CUDA_CHECK(cudaGetLastError());
+    if (counter) ++*counter;
+}
+
 // ------------------------------------------------------------------------------------------------
 // weight upload + repack
 // ------------------------------------------------------------------------------------------------
@@ -83,7 +158,7 @@ static bool type_supported(int t) {  // (Q4_K, Q5_0, Q5_1, Q8_0: tests/test_bloc
 static void qmat_alloc(QMat &m, int type, int rows, int cols) {
     m.type = type; m.rows = (rows + 1) & ~1; m.cols = cols;
     const size_t R = (size_t)m.rows;
-    auto zalloc = [](void **p, size_t n) { CUDA_CHECK(cudaMalloc(p, n)); CUDA_CHECK(cudaMemset(*p, 0, n)); };
+    auto zalloc = [](void **p, size_t n) { dmalloc(p, n); CUDA_CHECK(cudaMemset(*p, 0, n)); };
     switch (type) {
         case GG_Q4_0: m.row_bytes = (cols / 32 * 18 + 15) & ~15; zalloc(&m.p0, R * m.row_bytes + 256); break;
         case GG_Q4_1: m.row_bytes = (cols / 32 * 20 + 15) & ~15; zalloc(&m.p0, R * m.row_bytes + 256); break;
@@ -138,7 +213,7 @@ static void repack_into(QMat &dst, const HostTensor &src, Stager &st, int row0, 
 
 static float *upload_f32(const HostTensor &t) {
     if (t.gg != GG_F32) MG4_PANIC("tensor %s must be F32", t.name.c_str());
-    float *d; CUDA_CHECK(cudaMalloc((void **)&d, t.nbytes)); CUDA_CHECK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
+    float *d; dmalloc(&d, t.nbytes); CUDA_CHECK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
     return d;
 }
 
@@ -146,12 +221,9 @@ static float *upload_f32(const HostTensor &t) {
 LlamaDevice::LlamaDevice() {}
 LlamaDevice::~LlamaDevice() {
     if (graph_) cudaGraphExecDestroy(graph_);
-    for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
-    qmat_free(output_);
-    for (void *p : {(void *)final_norm_, tok_raw_, (void *)kcache_, (void *)vcache_, (void *)rope_, (void *)tab_exp_, (void *)tab_silu_, (void *)x_, (void *)q_, (void *)att_,
-                    (void *)act_, (void *)logits_, (void *)partial_, (void *)qact_, (void *)embd_in_, (void *)state_}) if (p) cudaFree(p);
-    for (auto &L : layers_) for (PQMat *m : {&L.pqkv, &L.pwo, &L.pw13, &L.pw2}) { if (m->q) cudaFree(m->q); if (m->sc) cudaFree(m->sc); }
-    for (void *p : {(void *)pf_q8_, pf_sc_, (void *)tok_ids_, pf_part_}) if (p) cudaFree(p);
+    for (void *p : {(void *)kcache_, (void *)vcache_, (void *)x_, (void *)q_, (void *)att_, (void *)act_, (void *)logits_, (void *)partial_, (void *)qact_, (void *)state_})
+        if (p) cudaFree(p);
+    if (!group_ || group_.use_count() == 1) free_weights();   // (a failed load frees what it got to)
     if (mega_barrier_) cudaFree(mega_barrier_);
     if (mega_trace_) cudaFree(mega_trace_);
     delete (mk6::Params6 *)mega6_params_;
@@ -160,6 +232,13 @@ LlamaDevice::~LlamaDevice() {
     if (ev0_) cudaEventDestroy(ev0_);
     if (ev1_) cudaEventDestroy(ev1_);
     if (stream_) cudaStreamDestroy(stream_);
+}
+void LlamaDevice::free_weights() {
+    for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
+    qmat_free(output_);
+    for (void *p : {(void *)final_norm_, tok_raw_, (void *)rope_, (void *)tab_exp_, (void *)tab_silu_, (void *)embd_in_}) if (p) cudaFree(p);
+    for (auto &L : layers_) for (PQMat *m : {&L.pqkv, &L.pwo, &L.pw13, &L.pw2}) { if (m->q) cudaFree(m->q); if (m->sc) cudaFree(m->sc); }
+    for (void *p : {(void *)pf_q8_, pf_sc_, (void *)tok_ids_, pf_part_}) if (p) cudaFree(p);
 }
 
 static inline unsigned short f2h_bits(float f) { __half h = __float2half_rn(f); unsigned short u; memcpy(&u, &h, 2); return u; }
@@ -180,8 +259,8 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     cudaDeviceProp prop; CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
     sm_count_ = prop.multiProcessorCount;
     g_max_dyn_smem = std::min<size_t>(prop.sharedMemPerBlockOptin, 220 * 1024) - 1024;
-    CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    CUDA_CHECK(cudaEventCreate(&ev0_)); CUDA_CHECK(cudaEventCreate(&ev1_));
+    group_ = std::make_shared<LlamaGroup>();
+    const size_t bytes0 = t_dev_bytes;
 
     Stager st;
     bytes_per_token_ = 0;
@@ -231,15 +310,15 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
         const HostTensor &tok = f.get("tok_embeddings.weight");
         tok_type_ = tok.gg;
         if (!(type_supported(tok.gg) || tok.gg == GG_F32)) { MG4_ERR("tok_embeddings has unsupported type %d", tok.gg); return false; }
-        CUDA_CHECK(cudaMalloc(&tok_raw_, tok.nbytes));
+        dmalloc(&tok_raw_, tok.nbytes);
         CUDA_CHECK(cudaMemcpy(tok_raw_, tok.data, tok.nbytes, cudaMemcpyHostToDevice));
     }
     // ggml's fp16 lookup tables (ggml_init): exp and silu, computed with the host libm exactly as ggml does
     {
         std::vector<unsigned short> te(65536), ts(65536);
         for (int i = 0; i < 65536; ++i) { const float x = h2f_bits((unsigned short)i); te[(size_t)i] = f2h_bits(expf(x)); ts[(size_t)i] = f2h_bits(x / (1.0f + expf(-x))); }
-        CUDA_CHECK(cudaMalloc((void **)&tab_exp_, 131072)); CUDA_CHECK(cudaMemcpy(tab_exp_, te.data(), 131072, cudaMemcpyHostToDevice));
-        CUDA_CHECK(cudaMalloc((void **)&tab_silu_, 131072)); CUDA_CHECK(cudaMemcpy(tab_silu_, ts.data(), 131072, cudaMemcpyHostToDevice));
+        dmalloc(&tab_exp_, 131072); CUDA_CHECK(cudaMemcpy(tab_exp_, te.data(), 131072, cudaMemcpyHostToDevice));
+        dmalloc(&tab_silu_, 131072); CUDA_CHECK(cudaMemcpy(tab_silu_, ts.data(), 131072, cudaMemcpyHostToDevice));
     }
     // RoPE table, mode 0: theta_i = pos * 10000^(-2i/n_rot) formed by repeated multiplication, cosf/sinf from libm (ggml_rope_f32)
     {
@@ -247,34 +326,63 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
         std::vector<float2> tab((size_t)n_ctx * hd2);
         const float theta_scale = powf(10000.0f, -2.0f / 128.0f);
         for (int p = 0; p < n_ctx; ++p) { float theta = (float)p; for (int i = 0; i < hd2; ++i) { tab[(size_t)p * hd2 + i] = make_float2(cosf(theta), sinf(theta)); theta *= theta_scale; } }
-        CUDA_CHECK(cudaMalloc((void **)&rope_, tab.size() * sizeof(float2)));
+        dmalloc(&rope_, tab.size() * sizeof(float2));
         CUDA_CHECK(cudaMemcpy(rope_, tab.data(), tab.size() * sizeof(float2), cudaMemcpyHostToDevice));
     }
-    const size_t kv = (size_t)d_.n_layer * n_ctx * El;
-    CUDA_CHECK(cudaMalloc((void **)&kcache_, kv * 2)); CUDA_CHECK(cudaMemset(kcache_, 0, kv * 2));
-    CUDA_CHECK(cudaMalloc((void **)&vcache_, kv * 2)); CUDA_CHECK(cudaMemset(vcache_, 0, kv * 2));
-    const size_t R = (size_t)kPrefillMax;  // rows of one prefill pass (the per-op path uses the first 8)
-    CUDA_CHECK(cudaMalloc((void **)&x_, R * E * 4));
-    CUDA_CHECK(cudaMalloc((void **)&q_, R * El * 4));
-    CUDA_CHECK(cudaMalloc((void **)&att_, R * El * 4));
-    CUDA_CHECK(cudaMalloc((void **)&act_, R * FFl * 4));
-    CUDA_CHECK(cudaMalloc((void **)&partial_, (size_t)8 * E * 4));
-    CUDA_CHECK(cudaMalloc((void **)&tok_ids_, R * 4));
-    CUDA_CHECK(cudaMalloc((void **)&qact_, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096)));
-    CUDA_CHECK(cudaMalloc((void **)&logits_, (size_t)(d_.n_vocab + 1) * 4));
-    CUDA_CHECK(cudaMalloc((void **)&embd_in_, (size_t)512 * E * 4));
-    CUDA_CHECK(cudaMalloc((void **)&state_, sizeof(DeviceState))); CUDA_CHECK(cudaMemset(state_, 0, sizeof(DeviceState)));
-    CUDA_CHECK(cudaHostAlloc((void **)&h_state_, sizeof(DeviceState), cudaHostAllocDefault)); memset(h_state_, 0, sizeof(DeviceState));
-    CUDA_CHECK(cudaHostAlloc((void **)&h_argmax_, 64, cudaHostAllocDefault)); *h_argmax_ = 0;
+    alloc_context();
+    // scratch of the synchronous prefill path (eval_rows ends with a stream sync), shared by the sessions of this model
+    const size_t R = (size_t)kPrefillMax;
+    dmalloc(&tok_ids_, R * 4);
+    dmalloc(&embd_in_, (size_t)512 * E * 4);
     CUDA_CHECK(cudaDeviceSynchronize());
     CUDA_CHECK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(49152, d_.n_ctx * 6)));
     if (tp_ && tp_->world > 1) tp_->setup_peers(E, stream_);
     pf_ready_ = build_prefill();
-    build_graph();
+    { const size_t b = t_dev_bytes; build_graph(); owned_bytes_ += t_dev_bytes - b; }
+    group_->weight_bytes = t_dev_bytes - bytes0 - owned_bytes_;
     MG4_INFO("LLaMA on device: %d layers, n_embd %d, n_ff %d, vocab %d, %.1f MB streamed per token, tp %d/%d", d_.n_layer, E, FF, d_.n_vocab,
              bytes_per_token_ / 1048576.0, rank, world);
     return true;
 }
+
+void LlamaDevice::alloc_context() {
+    const size_t b0 = t_dev_bytes;
+    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+    CUDA_CHECK(cudaEventCreate(&ev0_)); CUDA_CHECK(cudaEventCreate(&ev1_));
+    const size_t kv = (size_t)d_.n_layer * d_.n_ctx * El;
+    dmalloc(&kcache_, kv * 2); CUDA_CHECK(cudaMemset(kcache_, 0, kv * 2));
+    dmalloc(&vcache_, kv * 2); CUDA_CHECK(cudaMemset(vcache_, 0, kv * 2));
+    const size_t R = (size_t)kPrefillMax;  // rows of one prefill pass (the per-op path uses the first 8)
+    dmalloc(&x_, R * E * 4);
+    dmalloc(&q_, R * El * 4);
+    dmalloc(&att_, R * El * 4);
+    dmalloc(&act_, R * FFl * 4);
+    dmalloc(&partial_, (size_t)8 * E * 4);
+    dmalloc(&qact_, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
+    dmalloc(&logits_, (size_t)(d_.n_vocab + 1) * 4);
+    dmalloc(&state_, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(state_, 0, sizeof(DeviceState)));
+    CUDA_CHECK(cudaHostAlloc((void **)&h_state_, sizeof(DeviceState), cudaHostAllocDefault)); memset(h_state_, 0, sizeof(DeviceState));
+    CUDA_CHECK(cudaHostAlloc((void **)&h_argmax_, 64, cudaHostAllocDefault)); *h_argmax_ = 0;
+    owned_bytes_ += t_dev_bytes - b0;
+}
+
+bool LlamaDevice::load_session(const LlamaDevice &p) {
+    if (p.tp_ && p.tp_->world > 1) { MG4_ERR("sessions of a tensor-parallel context are not supported"); return false; }
+    group_ = p.group_;
+    d_ = p.d_; n_head_local_ = p.n_head_local_; n_embd_local_ = p.n_embd_local_; n_ff_local_ = p.n_ff_local_;
+    layers_ = p.layers_; output_ = p.output_; final_norm_ = p.final_norm_; tok_raw_ = p.tok_raw_; tok_type_ = p.tok_type_;
+    rope_ = p.rope_; tab_exp_ = p.tab_exp_; tab_silu_ = p.tab_silu_; embd_in_ = p.embd_in_; tok_ids_ = p.tok_ids_;
+    pf_ready_ = p.pf_ready_; pf_S_e_ = p.pf_S_e_; pf_S_ff_ = p.pf_S_ff_; pf_q8_ = p.pf_q8_; pf_sc_ = p.pf_sc_; pf_part_ = p.pf_part_; pf_part_bytes_ = p.pf_part_bytes_;
+    memcpy(pf_tmB_e_, p.pf_tmB_e_, 128); memcpy(pf_tmS_e_, p.pf_tmS_e_, 128); memcpy(pf_tmB_ff_, p.pf_tmB_ff_, 128); memcpy(pf_tmS_ff_, p.pf_tmS_ff_, 128);
+    bytes_per_token_ = p.bytes_per_token_; sm_count_ = p.sm_count_;
+    alloc_context();
+    CUDA_CHECK(cudaDeviceSynchronize());
+    { const size_t b = t_dev_bytes; build_graph(); owned_bytes_ += t_dev_bytes - b; }
+    MG4_INFO("LLaMA session: %d contexts share %.1f MB of weights, %.1f MB of its own", group_size(), group_->weight_bytes / 1048576.0, owned_bytes_ / 1048576.0);
+    return true;
+}
+size_t LlamaDevice::shared_bytes() const { return group_ ? group_->weight_bytes + group_->batch_bytes : 0; }
 
 // ------------------------------------------------------------------------------------------------
 // one pass of all layers over `ntok` (<= nt) rows that sit in x_; positions/tokens come from *state_
@@ -462,8 +570,8 @@ static int pf_slots(int cols) { const int nbl = (cols / 32 + 31) / 32; return 4 
 static void pq_build(PQMat &p, const QMat &m) {
     p.rows = m.rows; p.rows_pad = (m.rows + 127) & ~127; p.cols = m.cols; p.nb = m.cols / 32; p.S = pf_slots(m.cols); p.q41 = m.type == GG_Q4_1;
     const size_t pitch = (size_t)32 * p.S * 32;
-    CUDA_CHECK(cudaMalloc((void **)&p.q, (size_t)p.rows_pad * pitch)); CUDA_CHECK(cudaMemset(p.q, 0, (size_t)p.rows_pad * pitch));
-    CUDA_CHECK(cudaMalloc(&p.sc, (size_t)p.rows_pad * 32 * p.S * 4)); CUDA_CHECK(cudaMemset(p.sc, 0, (size_t)p.rows_pad * 32 * p.S * 4));
+    dmalloc(&p.q, (size_t)p.rows_pad * pitch); CUDA_CHECK(cudaMemset(p.q, 0, (size_t)p.rows_pad * pitch));
+    dmalloc(&p.sc, (size_t)p.rows_pad * 32 * p.S * 4); CUDA_CHECK(cudaMemset(p.sc, 0, (size_t)p.rows_pad * 32 * p.S * 4));
     const size_t n = (size_t)m.rows * p.nb;
     pf::expand_q4_classmajor<<<(unsigned)((n + 255) / 256), 256>>>((const unsigned char *)m.p0, m.row_bytes, m.rows, p.nb, p.q41 ? 1 : 0, p.S, p.q, (__half2 *)p.sc);
     CUDA_CHECK(cudaGetLastError());
@@ -486,14 +594,14 @@ bool LlamaDevice::build_prefill() {
     for (auto &L : layers_) { pq_build(L.pqkv, L.qkv); pq_build(L.pwo, L.wo); pq_build(L.pw13, L.w13); pq_build(L.pw2, L.w2); }
     pf_S_e_ = pf_slots(E); pf_S_ff_ = pf_slots(FF);
     const size_t pitch_e = (size_t)32 * pf_S_e_ * 32, pitch_ff = (size_t)32 * pf_S_ff_ * 32, R = (size_t)kPrefillMax;
-    CUDA_CHECK(cudaMalloc((void **)&pf_q8_, R * std::max(pitch_e, pitch_ff))); CUDA_CHECK(cudaMemset(pf_q8_, 0, R * std::max(pitch_e, pitch_ff)));
-    CUDA_CHECK(cudaMalloc(&pf_sc_, R * std::max(pitch_e, pitch_ff) / 4)); CUDA_CHECK(cudaMemset(pf_sc_, 0, R * std::max(pitch_e, pitch_ff) / 4));
+    dmalloc(&pf_q8_, R * std::max(pitch_e, pitch_ff)); CUDA_CHECK(cudaMemset(pf_q8_, 0, R * std::max(pitch_e, pitch_ff)));
+    dmalloc(&pf_sc_, R * std::max(pitch_e, pitch_ff) / 4); CUDA_CHECK(cudaMemset(pf_sc_, 0, R * std::max(pitch_e, pitch_ff) / 4));
     make_map_u8(pf_tmB_e_, pf_q8_, R, pitch_e, 128, pf::kTok, true);
     make_map_u8(pf_tmS_e_, pf_sc_, R, pitch_e / 4, 32, pf::kTok, false);
     make_map_u8(pf_tmB_ff_, pf_q8_, R, pitch_ff, 128, pf::kTok, true);
     make_map_u8(pf_tmS_ff_, pf_sc_, R, pitch_ff / 4, 32, pf::kTok, false);
     pf_part_bytes_ = (size_t)96 << 20;   // roots of K-split slices: [slice][token][row] {d-tree, m-tree}
-    CUDA_CHECK(cudaMalloc(&pf_part_, pf_part_bytes_));
+    dmalloc(&pf_part_, pf_part_bytes_);
     const size_t smem = 1024 + (size_t)pf::kStages * pf::kStageBytes + pf::kStackBytes + 256;
     CUDA_CHECK(cudaFuncSetAttribute(pf::prefill_gemm_q4<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_CHECK(cudaFuncSetAttribute(pf::prefill_gemm_q4<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -584,9 +692,9 @@ bool LlamaDevice::build_mega() {
     CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
     if (!coop) return false;
     mega_type_ = wt;
-    CUDA_CHECK(cudaMalloc((void **)&mega_barrier_, 64)); CUDA_CHECK(cudaMemset(mega_barrier_, 0, 64));
+    dmalloc(&mega_barrier_, 64); CUDA_CHECK(cudaMemset(mega_barrier_, 0, 64));
     mega_n_ops_ = (tp ? 7 : 5) * d_.n_layer + 3;
-    if (getenv("MINIGPT4_B200_MEGA_TRACE")) { CUDA_CHECK(cudaMalloc((void **)&mega_trace_, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long))); CUDA_CHECK(cudaMemset(mega_trace_, 0, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long))); }
+    if (getenv("MINIGPT4_B200_MEGA_TRACE")) { dmalloc(&mega_trace_, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long)); CUDA_CHECK(cudaMemset(mega_trace_, 0, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long))); }
     mega_gen_ = 6;
     if (!build_mega6()) return false;
     const void *fn = mega_fn();
@@ -732,6 +840,104 @@ float LlamaDevice::decode_chain(int steps, int n_past, int32_t *ids_out) {
     if (ids_out) CUDA_CHECK(cudaMemcpy(ids_out, ids_dev, (size_t)steps * 4, cudaMemcpyDeviceToHost));
     cudaFree(ids_dev);
     return ms;
+}
+
+// ------------------------------------------------------------------------------------------------
+// batched decode step over B contexts of one group (llama_sessions.cuh): prepare (tokens) -> embed B rows -> layers (QKV and attention
+// per column through the slot table; wo / gate-up / down through matvec_kernel at ntok = B) -> logits of every column into its own
+// context -> finalize every context's DeviceState -> the B ids to pinned memory.  Captured once per B on the group stream.
+// ------------------------------------------------------------------------------------------------
+void LlamaDevice::build_batch_graph(int B) {
+    LlamaGroup &G = *group_;
+    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_, C = d_.n_ctx, nt = nt_for(B);
+    if (!G.stream) {
+        const size_t b0 = t_dev_bytes;
+        CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
+        dmalloc(&G.x, (size_t)8 * E * 4);
+        dmalloc(&G.q, (size_t)8 * El * 4);
+        dmalloc(&G.att, (size_t)8 * El * 4);
+        dmalloc(&G.act, (size_t)8 * FFl * 4);
+        dmalloc(&G.qact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
+        dmalloc(&G.state, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.state, 0, sizeof(DeviceState)));
+        dmalloc(&G.slots, 8 * sizeof(SessionSlot));
+        dmalloc(&G.ids, 8 * sizeof(int));
+        CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, 8 * sizeof(int), cudaHostAllocDefault));
+        CUDA_CHECK(cudaDeviceSynchronize());
+        G.batch_bytes = t_dev_bytes - b0;
+    }
+    {   // attention scratch = n_ctx * 6 bytes; the attribute only grows (groups of one process may differ in n_ctx)
+        static int attn_smem[64] = {};
+        int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
+        const int need = std::max(49152, C * 6);
+        if (need > attn_smem[dev & 63]) { CUDA_CHECK(cudaFuncSetAttribute(attn_sessions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, need)); attn_smem[dev & 63] = need; }
+    }
+    const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
+    cudaStream_t s = G.stream;
+    unsigned long long n = 0;
+    cudaGraph_t g = nullptr;
+    CUDA_CHECK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.state); ++n;
+    const size_t trb = gg_row_bytes(tok_type_, (size_t)E);
+    if (tok_type_ == GG_Q4_K) embed_q4k_kernel<<<B, 256, 0, s>>>((const unsigned char *)tok_raw_, trb, E, G.state, G.x);
+    else if (tok_type_ == GG_Q5_0 || tok_type_ == GG_Q5_1 || tok_type_ == GG_Q8_0) embed_b32_kernel<<<B, 256, 0, s>>>(tok_type_, (const unsigned char *)tok_raw_, trb, E, G.state, G.x);
+    else embed_kernel<<<B, 256, 0, s>>>(tok_type_, (const unsigned char *)tok_raw_, trb, E, G.state, G.x);
+    ++n;
+    for (int il = 0; il < d_.n_layer; ++il) {
+        Layer &L = layers_[(size_t)il];
+        const size_t kv_off = (size_t)il * C * El;
+        MatvecArgs a{};
+        a.x = G.x; a.x_stride = E; a.norm_w = L.attn_norm; a.ntok = B; a.epi = EPI_QKV; a.staged = G.qact;
+        a.q_out = G.q; a.rope = rope_; a.e_local = El; a.half_dim = 64; a.state = G.state; a.tab_silu = tab_silu_;
+        if (L.fused_qkv) { a.w = L.qkv; a.part = -1; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.slots, kv_off, nt, sm_count_, s, &n); }
+        else {
+            const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
+            for (int part = 0; part < 3; ++part) {
+                const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
+                a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.slots, kv_off, nt, sm_count_, s, &n, !same);
+            }
+        }
+        attn_sessions_kernel<<<dim3((unsigned)n_head_local_, (unsigned)B), 256, (size_t)C * 6, s>>>(G.q, G.slots, kv_off, G.att, El, C, kq_scale, tab_exp_);
+        CUDA_CHECK(cudaGetLastError()); ++n;
+        MatvecArgs b{};
+        b.w = L.wo; b.x = G.att; b.x_stride = El; b.ntok = B; b.n_valid = b.w.rows; b.state = G.state; b.tab_silu = tab_silu_; b.staged = G.qact;
+        b.epi = EPI_RESID; b.out = G.x; b.out_stride = E; b.resid = G.x;
+        launch_matvec(b, nt, sm_count_, s, &n);
+        MatvecArgs c{};
+        c.w = L.w13; c.x = G.x; c.x_stride = E; c.norm_w = L.ffn_norm; c.ntok = B; c.epi = EPI_SWIGLU; c.out = G.act; c.out_stride = FFl; c.n_valid = c.w.rows;
+        c.state = G.state; c.tab_silu = tab_silu_; c.staged = G.qact;
+        launch_matvec(c, nt, sm_count_, s, &n);
+        MatvecArgs e{};
+        e.w = L.w2; e.x = G.act; e.x_stride = FFl; e.ntok = B; e.n_valid = e.w.rows; e.state = G.state; e.tab_silu = tab_silu_; e.staged = G.qact;
+        e.epi = EPI_RESID; e.out = G.x; e.out_stride = E; e.resid = G.x;
+        launch_matvec(e, nt, sm_count_, s, &n);
+    }
+    MatvecArgs o{};
+    o.w = output_; o.x = G.x; o.x_stride = E; o.norm_w = final_norm_; o.ntok = B; o.epi = EPI_LOGITS; o.n_valid = d_.n_vocab;
+    o.state = G.state; o.tab_silu = tab_silu_; o.staged = G.qact;
+    launch_matvec_sessions(o, G.slots, 0, nt, sm_count_, s, &n);
+    finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.ids); ++n;
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(G.h_ids, G.ids, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamEndCapture(s, &g));
+    CUDA_CHECK(cudaGraphInstantiate(&G.graph[B], g, 0));
+    CUDA_CHECK(cudaGraphDestroy(g));
+    G.graph_kernels[B] = (int)n;
+}
+
+void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids, const int *n_past, int32_t *ids_out) {
+    LlamaDevice &L0 = *c[0];
+    LlamaGroup &G = *L0.group_;
+    // a context's own decode step may still be running on its stream (decode_step returns before it finishes): it has to be done
+    // before the group stream reads and writes that context's cache, logits and state
+    for (int i = 0; i < n; ++i) c[i]->sync();
+    if (!G.graph[n]) L0.build_batch_graph(n);
+    for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], ids[i], c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
+    CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, G.stream));
+    CUDA_CHECK(cudaGraphLaunch(G.graph[n], G.stream));
+    CUDA_CHECK(cudaStreamSynchronize(G.stream));   // (h_slots / h_ids are reused by the next step)
+    L0.launches_ += (unsigned long long)G.graph_kernels[n];
+    for (int i = 0; i < n; ++i) { ids_out[i] = G.h_ids[i]; *c[i]->h_argmax_ = G.h_ids[i]; }
 }
 
 // measurement seam: average CUDA-event duration (us) of one all-reduce of a [1, n_embd] partial on the tensor-parallel path in use

@@ -11,6 +11,7 @@
 //     vec_dot type (Q8_0/Q8_1/Q8_K/F16) in its prologue — the integer-dot formulation ggml uses (SURVEY §A.3)
 #pragma once
 #include "formats.h"
+#include <memory>
 
 namespace mg4 {
 
@@ -41,11 +42,33 @@ struct DeviceState {   // lives in device memory; kernels read positions/tokens 
     int pad[3];
 };
 
+struct SessionSlot {   // one column of a batched decode step (device table of the group, refreshed by one copy per step)
+    int n_past;        // the context's position: its token is evaluated there
+    int id;            // token to feed; < 0: the context's on-device greedy id (DeviceState::tokens[0])
+    __half *kcache, *vcache;   // the context's caches (layer 0)
+    float *logits;
+    DeviceState *state;
+};
+
+struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
+
 class LlamaDevice {
 public:
     LlamaDevice();
     ~LlamaDevice();
     bool load(const LlamaFile &f, int n_ctx, TPLink *tp);
+    // A new context over the weights of `parent` (the repacked matrices, the prefill operand cache, token embeddings, RoPE table,
+    // LUTs and the prefill scratch, which is only used synchronously): own KV cache of the parent's n_ctx, activations, state,
+    // stream and decode graph / megakernel.  The weights go with the last context of the group.  Single GPU only.
+    bool load_session(const LlamaDevice &parent);
+    const LlamaGroup *group() const { return group_.get(); }
+    int group_size() const { return (int)group_.use_count(); }
+    size_t owned_bytes() const { return owned_bytes_; }   // device bytes of this context: KV cache + per-context scratch
+    size_t shared_bytes() const;                          // device bytes shared by the group: weights, operand cache, tables, prefill scratch, batch workspace
+    // One decode step of n (2..8) distinct contexts of one group; the weights stream once.  Column i is fed ids[i] (< 0: the context's
+    // on-device greedy id) at position n_past[i]; afterwards each context holds what its own decode_step would have left (logits,
+    // arg-max, DeviceState) and ids_out[i] = its new arg-max.  Synchronous.  The caller validates (distinct, one group, ranges).
+    static void decode_batch(LlamaDevice *const *ctx, int n, const int32_t *ids, const int *n_past, int32_t *ids_out);
     const LlamaDims &dims() const { return d_; }
     // Evaluate `n` tokens / embedding rows starting at position n_past. Afterwards logits of the last row are
     // on device and the arg-max id is known.  Returns false if the context would overflow.
@@ -124,6 +147,12 @@ private:
     bool h_state_busy_ = false;
     bool mega_ = false; unsigned *mega_barrier_ = nullptr; size_t mega_smem_ = 0; int mega_type_ = -1;
     int sm_count_ = 132;
+    // sessions: every context of a group holds the same weight pointers above; group_ counts the contexts
+    std::shared_ptr<LlamaGroup> group_;
+    size_t owned_bytes_ = 0;
+    void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
+    void free_weights();             // by the last context of the group
+    void build_batch_graph(int B);   // decode_batch's graph for B columns, captured on the group stream
 };
 
 }  // namespace mg4

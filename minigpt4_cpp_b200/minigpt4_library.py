@@ -216,6 +216,10 @@ _EXT = {
     "minigpt4_b200_get_hidden": ([_CTX, _VP, _I], _I),
     "minigpt4_b200_token_text": ([_CTX, _I], _S),
     "minigpt4_b200_decode_chain": ([_CTX, _I, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_session_create": ([_CTX, _I], _CTX),
+    "minigpt4_b200_session_info": ([_CTX, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
+    "minigpt4_b200_decode_batch": ([_VP, _I, _VP, _VP], _I),
+    "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
@@ -301,6 +305,43 @@ class B200:
         ms = C.c_float(0)
         self._chk(self.L.minigpt4_b200_decode_chain(ctx.ptr, steps, _ptr(ids), C.byref(ms)))
         return ids, ms.value
+
+    # multi-session serving: contexts that share one loaded model, stepped together
+    def session_create(self, ctx, seed: int = 1337) -> MiniGPT4Context:
+        """a new conversation over ctx's model (weights shared, own KV cache / state / sampler seeded with `seed`)"""
+        ptr = self.L.minigpt4_b200_session_create(ctx.ptr, seed)
+        assert ptr is not None, "minigpt4_b200_session_create failed"
+        return MiniGPT4Context(ptr)
+
+    def session_info(self, ctx) -> tuple[int, float, float]:
+        """(live contexts of the group, device bytes ctx owns, device bytes it shares)"""
+        n, owned, shared = C.c_int(0), C.c_double(0), C.c_double(0)
+        self._chk(self.L.minigpt4_b200_session_info(ctx.ptr, C.byref(n), C.byref(owned), C.byref(shared)))
+        return n.value, owned.value, shared.value
+
+    @staticmethod
+    def _ctx_array(ctxs):
+        return (C.c_void_p * max(1, len(ctxs)))(*[c.ptr for c in ctxs])
+
+    def decode_batch(self, ctxs, ids=None) -> np.ndarray:
+        """one decode step of every context in `ctxs` (1..8 of one group; weights streamed once); ids[i] < 0 or ids None: each context's
+        own greedy id.  Returns the new greedy ids."""
+        n = len(ctxs)
+        a = np.full(n, -1, np.int32) if ids is None else np.ascontiguousarray(ids, np.int32)
+        out = np.zeros(max(1, n), np.int32)
+        self._chk(self.L.minigpt4_b200_decode_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), n, _ptr(a), _ptr(out)))
+        return out[:n]
+
+    def end_chat_batch(self, ctxs, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
+                       repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 1.0, alpha_frequency: float = 1.0,
+                       mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0, penalize_nl: int = 1) -> list[str]:
+        """minigpt4_end_chat on each context (own logits, own sampler), the sampled tokens fed in one batched step; returns their texts"""
+        n = len(ctxs)
+        toks = (C.c_char_p * max(1, n))()
+        self._chk(self.L.minigpt4_b200_end_chat_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), n, C.cast(toks, C.c_void_p), temp, top_k, top_p,
+                                                      tfs_z, typical_p, repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, mirostat,
+                                                      mirostat_tau, mirostat_eta, penalize_nl))
+        return [toks[i].decode("utf-8", errors="ignore") for i in range(n)]
 
     def time_matvec(self, ctx, kind: int, reps: int = 3) -> tuple[float, float]:
         ms, nb = C.c_float(0), C.c_double(0)
