@@ -67,6 +67,16 @@ MINIGPT4_API int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_
  * its logits are the bits a step on its own gives.  Synchronous.  NULL or duplicate contexts, contexts of different groups,
  * n outside 1..8, a full context or an id >= n_vocab return the FailedToAddString error code (8) and change no context. */
 MINIGPT4_API int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, int32_t *ids_out);
+/* Evaluate the queued prompt rows (add_tokens / add_embedding pieces not yet evaluated) of n (1..8) distinct contexts of one group
+ * in shared passes over the weights, at most 512 rows per pass; a context's rows may be split across two passes.  Afterwards each
+ * context is exactly as minigpt4_b200_flush would have left it: n_past, KV cache, logits (bit for bit), greedy id and the device
+ * state the next decode step continues from.  Contexts with an empty queue are left untouched; n = 1 is that context's own flush.
+ * minigpt4_b200_get_hidden(ctx, out, k), with k the number of its rows in the pass that evaluated its last row, returns the residual
+ * stream of those rows, i.e. of its last k rows (an own flush leaves the rows of its own last pass the same way).
+ * minigpt4_b200_decode_batch and end_chat_batch flush their contexts this way.
+ * Synchronous.  NULL or duplicate contexts, contexts of different groups or n outside 1..8 return the FailedToAddString error
+ * code (8) and change no context. */
+MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n);
 /* minigpt4_end_chat on each context in turn (each samples from its own logits with its own sampler; greedy uses the device
  * arg-max; tokens[i] = the sampled token's text), then the n sampled ids are fed in one minigpt4_b200_decode_batch step.
  * The batch is validated before any sampling. */

@@ -84,12 +84,18 @@ Error Engine::init_session(const Engine &parent, int seed) {
 }
 
 // Batched decode (extension): every check happens before anything runs, so a refused batch leaves every context as it was.
-bool Engine::batch_valid(Engine *const *e, int n, const int32_t *ids) {
-    if (!e || n < 1 || n > 8) { MG4_ERR("decode_batch: %d contexts (1 .. 8)", n); return false; }
+bool Engine::group_valid(Engine *const *e, int n, const char *what) {
+    if (!e || n < 1 || n > 8) { MG4_ERR("%s: %d contexts (1 .. 8)", what, n); return false; }
     for (int i = 0; i < n; ++i) {
-        if (!e[i]) { MG4_ERR("decode_batch: context %d is NULL", i); return false; }
-        for (int j = 0; j < i; ++j) if (e[j] == e[i]) { MG4_ERR("decode_batch: context %d appears twice", i); return false; }
-        if (e[i]->llm_->group() != e[0]->llm_->group()) { MG4_ERR("decode_batch: context %d serves another model", i); return false; }
+        if (!e[i]) { MG4_ERR("%s: context %d is NULL", what, i); return false; }
+        for (int j = 0; j < i; ++j) if (e[j] == e[i]) { MG4_ERR("%s: context %d appears twice", what, i); return false; }
+        if (e[i]->llm_->group() != e[0]->llm_->group()) { MG4_ERR("%s: context %d serves another model", what, i); return false; }
+    }
+    return true;
+}
+bool Engine::batch_valid(Engine *const *e, int n, const int32_t *ids) {
+    if (!group_valid(e, n, "decode_batch")) return false;
+    for (int i = 0; i < n; ++i) {
         const LlamaDims &d = e[i]->llm_->dims();
         if (e[i]->n_past_ + 1 > d.n_ctx) { MG4_ERR("decode_batch: context %d is full (n_ctx %d)", i, d.n_ctx); return false; }
         if (ids && ids[i] >= d.n_vocab) { MG4_ERR("decode_batch: token id %d out of range", ids[i]); return false; }
@@ -98,7 +104,7 @@ bool Engine::batch_valid(Engine *const *e, int n, const int32_t *ids) {
 }
 Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out) {
     if (!ids || !ids_out || !batch_valid(e, n, ids)) return ErrFailedToAddString;
-    for (int i = 0; i < n; ++i) if (!e[i]->flush()) return ErrFailedToAddString;   // queued prompt rows: each context's own prefill pass
+    if (!flush_group(e, n)) return ErrFailedToAddString;   // queued prompt rows of all n contexts in shared passes
     if (n == 1) {   // one context: its own decode graph or megakernel, exactly as add_tokens' single-token step
         Engine &c = *e[0];
         if (!c.llm_->decode_step(ids[0], c.n_past_)) return ErrFailedToAddString;
@@ -113,9 +119,28 @@ Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t 
 }
 Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p) {
     if (!tokens || !batch_valid(e, n, nullptr)) return ErrFailedToAddString;   // (before any sampler draws)
+    if (!flush_group(e, n)) return ErrFailedToAddString;   // so that each sample_token finds its queue empty
     int32_t ids[8], out[8];
     for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
     return decode_batch(e, n, ids, out);
+}
+Error Engine::flush_batch(Engine *const *e, int n) {
+    if (!group_valid(e, n, "flush_batch")) return ErrFailedToAddString;
+    return flush_group(e, n) ? ErrNone : ErrFailedToAddString;
+}
+// the queues of a validated batch: one context with queued rows is its own flush(), several share the passes of eval_rows_batch
+bool Engine::flush_group(Engine *const *e, int n) {
+    Engine *q[8]; int m = 0;
+    for (int i = 0; i < n; ++i) if (!e[i]->pend_ids_.empty()) q[m++] = e[i];
+    if (m <= 1) return m == 0 || q[0]->flush();
+    LlamaDevice *L[8]; const int32_t *ids[8]; const float *emb[8]; int rows[8], base[8];
+    for (int i = 0; i < m; ++i) {
+        L[i] = q[i]->llm_.get(); ids[i] = q[i]->pend_ids_.data(); emb[i] = q[i]->pend_emb_.data();
+        rows[i] = (int)q[i]->pend_ids_.size(); base[i] = q[i]->pend_base_;
+    }
+    LlamaDevice::eval_rows_batch(L, m, ids, rows, emb, base);
+    for (int i = 0; i < m; ++i) { q[i]->pend_ids_.clear(); q[i]->pend_emb_.clear(); }
+    return true;
 }
 
 // input validation = reference minigpt4.cpp:2130-2138

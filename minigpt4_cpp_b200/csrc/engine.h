@@ -28,6 +28,8 @@ public:
     static Error decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out);
     // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
     static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
+    // the queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
+    static Error flush_batch(Engine *const *e, int n);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
     static constexpr int kEncodeLanes = 8;
     Error encode_images(const ::MiniGPT4Image *images, size_t n, ::MiniGPT4Embedding *out, float *total_ms);   // batched: concurrent lanes
@@ -51,7 +53,9 @@ public:
     TPLink tp;
 
 private:
+    static bool group_valid(Engine *const *e, int n, const char *what);   // 1..8 distinct non-NULL contexts of one group
     static bool batch_valid(Engine *const *e, int n, const int32_t *ids);
+    static bool flush_group(Engine *const *e, int n);
     // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)
     std::shared_ptr<VisionFile> vfile_;
     std::shared_ptr<VisionDevice> vis_;

@@ -19,7 +19,7 @@ static thread_local size_t t_dev_bytes = 0;
 template <class T> static void dmalloc(T **p, size_t n) { CUDA_CHECK(cudaMalloc((void **)p, n)); t_dev_bytes += n; }
 
 // what the contexts of one model share besides the weight pointers each of them holds: the batched decode step's workspace,
-// stream and graphs (built by the group's first decode_batch of each size)
+// stream and graphs (built by the group's first decode_batch of each size) and the batched prompt pass's workspace
 struct LlamaGroup {
     size_t weight_bytes = 0;       // the parent's load minus its own context: weights, operand cache, tables, prefill scratch
     size_t batch_bytes = 0;
@@ -31,11 +31,19 @@ struct LlamaGroup {
     int *ids = nullptr, *h_ids = nullptr;
     cudaGraphExec_t graph[9] = {};
     int graph_kernels[9] = {};
+    // the batched prompt pass (eval_rows_batch, built by the group's first batched flush): kPrefillMax rows of activations (pact also
+    // holds the qkv GEMM's [rows][3 n_embd] output), the last rows of the contexts that end in a pass, a slot per row and per context
+    float *px = nullptr, *pq = nullptr, *patt = nullptr, *pact = nullptr, *plast = nullptr;
+    unsigned char *pqact = nullptr;
+    DeviceState *pstate = nullptr;
+    SessionSlot *rslots = nullptr, *h_rslots = nullptr, *cslots = nullptr, *h_cslots = nullptr;
+    int *pids = nullptr, *h_pids = nullptr;
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
         for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)qact, (void *)state, (void *)slots, (void *)ids}) if (p) cudaFree(p);
-        if (h_slots) cudaFreeHost(h_slots);
-        if (h_ids) cudaFreeHost(h_ids);
+        for (void *p : {(void *)px, (void *)pq, (void *)patt, (void *)pact, (void *)plast, (void *)pqact, (void *)pstate, (void *)rslots, (void *)cslots, (void *)pids})
+            if (p) cudaFree(p);
+        for (void *p : {(void *)h_slots, (void *)h_ids, (void *)h_rslots, (void *)h_cslots, (void *)h_pids}) if (p) cudaFreeHost(p);
         if (stream) cudaStreamDestroy(stream);
     }
 };
@@ -611,41 +619,45 @@ bool LlamaDevice::build_prefill() {
     return true;
 }
 
+void LlamaDevice::pf_stage(const QMat &w, const float *x, int x_stride, const float *nw, int S, int n, cudaStream_t s) {
+    const int act = act_of(w.type);
+    const size_t sm = act_bytes(act, w.cols);
+    if (act == ACT_Q8_1) pf::stage_rows_classmajor<ACT_Q8_1><<<n, 256, sm, s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
+    else pf::stage_rows_classmajor<ACT_Q8_0><<<n, 256, sm, s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
+    ++launches_;
+}
+void LlamaDevice::pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, int n, const DeviceState *state, cudaStream_t s) {
+    const size_t smem = 1024 + (size_t)pf::kStages * pf::kStageBytes + pf::kStackBytes + 256;
+    const unsigned ty = (unsigned)((n + pf::kTok - 1) / pf::kTok);
+    pf::PrefillArgs a = epi;
+    a.rows = p.rows; a.n_tok = n; a.nb = p.nb; a.S = p.S; a.wsc = (const __half2 *)p.sc; a.state = state; a.tab_silu = tab_silu_;
+    const CUtensorMap *tb = (const CUtensorMap *)(ff_wide ? pf_tmB_ff_ : pf_tmB_e_), *ts = (const CUtensorMap *)(ff_wide ? pf_tmS_ff_ : pf_tmS_e_);
+    // K split over subtrees of the class butterfly so that matrices with few 128-row tiles (wo / down: 32) still fill the machine
+    const int tiles = p.rows_pad / pf::kRows;
+    int nz = 1;
+    if (!getenv("MINIGPT4_B200_PREFILL_NO_KSPLIT")) {   // waves of CTAs x work per CTA (+ a little per-CTA overhead), smallest wins
+        double best = 1e30;
+        for (int c = 1; c <= 8; c *= 2) {
+            if ((size_t)c * n * p.rows_pad * sizeof(float2) > pf_part_bytes_ && c > 1) break;
+            const int ctas = tiles * (int)ty * c;
+            const double cost = (double)((ctas + sm_count_ - 1) / sm_count_) / c + 0.02 * c;
+            if (cost < best - 1e-9) { best = cost; nz = c; }
+        }
+    }
+    a.jr_per_z = 32 / nz; a.partial = (float2 *)pf_part_; a.part_tok = n; a.part_rows = p.rows_pad;
+    const dim3 grid((unsigned)tiles, ty, (unsigned)nz);
+    if (p.q41) pf::prefill_gemm_q4<true><<<grid, pf::kThreads, smem, s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
+    else pf::prefill_gemm_q4<false><<<grid, pf::kThreads, smem, s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
+    ++launches_;
+    if (nz > 1) { const size_t work = (size_t)n * (p.rows / 2); pf::prefill_combine<<<(unsigned)((work + 255) / 256), 256, 0, s>>>(a, nz); ++launches_; }
+}
+
 // one pass of all layers over n (<= kPrefillMax) rows in x_; positions from *state_ (n_past), KV rows appended, logits of the last row
 void LlamaDevice::prefill_chunk(int n, bool want_logits) {
     const int E = d_.n_embd, El = n_embd_local_, FFl = n_ff_local_, C = d_.n_ctx;
     const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
-    const size_t smem = 1024 + (size_t)pf::kStages * pf::kStageBytes + pf::kStackBytes + 256;
-    const unsigned ty = (unsigned)((n + pf::kTok - 1) / pf::kTok);
-    auto stage = [&](const QMat &w, const float *x, int x_stride, const float *nw, int S) {
-        const int act = act_of(w.type);
-        const size_t sm = act_bytes(act, w.cols);
-        if (act == ACT_Q8_1) pf::stage_rows_classmajor<ACT_Q8_1><<<n, 256, sm, stream_>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
-        else pf::stage_rows_classmajor<ACT_Q8_0><<<n, 256, sm, stream_>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
-        ++launches_;
-    };
-    auto gemm = [&](const PQMat &p, bool ff_wide, pf::PrefillArgs a) {
-        a.rows = p.rows; a.n_tok = n; a.nb = p.nb; a.S = p.S; a.wsc = (const __half2 *)p.sc; a.state = state_; a.tab_silu = tab_silu_;
-        const CUtensorMap *tb = (const CUtensorMap *)(ff_wide ? pf_tmB_ff_ : pf_tmB_e_), *ts = (const CUtensorMap *)(ff_wide ? pf_tmS_ff_ : pf_tmS_e_);
-        // K split over subtrees of the class butterfly so that matrices with few 128-row tiles (wo / down: 32) still fill the machine
-        const int tiles = p.rows_pad / pf::kRows;
-        int nz = 1;
-        if (!getenv("MINIGPT4_B200_PREFILL_NO_KSPLIT")) {   // waves of CTAs x work per CTA (+ a little per-CTA overhead), smallest wins
-            double best = 1e30;
-            for (int c = 1; c <= 8; c *= 2) {
-                if ((size_t)c * n * p.rows_pad * sizeof(float2) > pf_part_bytes_ && c > 1) break;
-                const int ctas = tiles * (int)ty * c;
-                const double cost = (double)((ctas + sm_count_ - 1) / sm_count_) / c + 0.02 * c;
-                if (cost < best - 1e-9) { best = cost; nz = c; }
-            }
-        }
-        a.jr_per_z = 32 / nz; a.partial = (float2 *)pf_part_; a.part_tok = n; a.part_rows = p.rows_pad;
-        const dim3 grid((unsigned)tiles, ty, (unsigned)nz);
-        if (p.q41) pf::prefill_gemm_q4<true><<<grid, pf::kThreads, smem, stream_>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
-        else pf::prefill_gemm_q4<false><<<grid, pf::kThreads, smem, stream_>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
-        ++launches_;
-        if (nz > 1) { const size_t work = (size_t)n * (p.rows / 2); pf::prefill_combine<<<(unsigned)((work + 255) / 256), 256, 0, stream_>>>(a, nz); ++launches_; }
-    };
+    auto stage = [&](const QMat &w, const float *x, int x_stride, const float *nw, int S) { pf_stage(w, x, x_stride, nw, S, n, stream_); };
+    auto gemm = [&](const PQMat &p, bool ff_wide, const pf::PrefillArgs &a) { pf_gemm(p, ff_wide, a, n, state_, stream_); };
     for (int il = 0; il < d_.n_layer; ++il) {
         Layer &L = layers_[(size_t)il];
         __half *kc = kcache_ + (size_t)il * C * El, *vc = vcache_ + (size_t)il * C * El;
@@ -847,12 +859,18 @@ float LlamaDevice::decode_chain(int steps, int n_past, int32_t *ids_out) {
 // per column through the slot table; wo / gate-up / down through matvec_kernel at ntok = B) -> logits of every column into its own
 // context -> finalize every context's DeviceState -> the B ids to pinned memory.  Captured once per B on the group stream.
 // ------------------------------------------------------------------------------------------------
+static void attn_sessions_smem(int n_ctx) {   // attention scratch = n_ctx * 6 bytes; the attribute only grows (groups of one process may differ in n_ctx)
+    static int attn_smem[64] = {};
+    int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
+    const int need = std::max(49152, n_ctx * 6);
+    if (need > attn_smem[dev & 63]) { CUDA_CHECK(cudaFuncSetAttribute(attn_sessions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, need)); attn_smem[dev & 63] = need; }
+}
 void LlamaDevice::build_batch_graph(int B) {
     LlamaGroup &G = *group_;
     const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_, C = d_.n_ctx, nt = nt_for(B);
-    if (!G.stream) {
+    if (!G.x) {
         const size_t b0 = t_dev_bytes;
-        CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
+        if (!G.stream) CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
         dmalloc(&G.x, (size_t)8 * E * 4);
         dmalloc(&G.q, (size_t)8 * El * 4);
         dmalloc(&G.att, (size_t)8 * El * 4);
@@ -864,14 +882,9 @@ void LlamaDevice::build_batch_graph(int B) {
         CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
         CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, 8 * sizeof(int), cudaHostAllocDefault));
         CUDA_CHECK(cudaDeviceSynchronize());
-        G.batch_bytes = t_dev_bytes - b0;
+        G.batch_bytes += t_dev_bytes - b0;
     }
-    {   // attention scratch = n_ctx * 6 bytes; the attribute only grows (groups of one process may differ in n_ctx)
-        static int attn_smem[64] = {};
-        int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
-        const int need = std::max(49152, C * 6);
-        if (need > attn_smem[dev & 63]) { CUDA_CHECK(cudaFuncSetAttribute(attn_sessions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, need)); attn_smem[dev & 63] = need; }
-    }
+    attn_sessions_smem(C);
     const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
     cudaStream_t s = G.stream;
     unsigned long long n = 0;
@@ -938,6 +951,161 @@ void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids,
     CUDA_CHECK(cudaStreamSynchronize(G.stream));   // (h_slots / h_ids are reused by the next step)
     L0.launches_ += (unsigned long long)G.graph_kernels[n];
     for (int i = 0; i < n; ++i) { ids_out[i] = G.h_ids[i]; *c[i]->h_argmax_ = G.h_ids[i]; }
+}
+
+// ------------------------------------------------------------------------------------------------
+// batched prompt pass over the queued rows of several contexts of one group (llama_sessions.cuh).  Each pass takes the next <=
+// kPrefillMax rows of the contexts in order; row t carries its own position and its context's caches in a row slot (rslots).  Per layer:
+// qkv with RoPE and KV append at each row's position into its context's cache (tensor-core GEMM + qkv_rows_kernel, or per-op
+// matvec_sessions_kernel over 8-row chunks), attn_sessions_kernel over all rows, then wo / gate-up / down exactly as a single context's
+// pass.  Contexts whose last row is in the pass get their logits, arg-max and DeviceState through the context slots (cslots), as the
+// batched decode step does.  Every row is quantised and reduced on its own, so each context gets the bits of its own eval_rows.
+// ------------------------------------------------------------------------------------------------
+void LlamaDevice::build_prompt_workspace() {
+    LlamaGroup &G = *group_;
+    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_;
+    const size_t R = (size_t)kPrefillMax, b0 = t_dev_bytes;
+    if (!G.stream) CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
+    dmalloc(&G.px, R * E * 4);
+    dmalloc(&G.pq, R * El * 4);
+    dmalloc(&G.patt, R * El * 4);
+    dmalloc(&G.pact, R * std::max(FFl, 3 * El) * 4);
+    dmalloc(&G.plast, (size_t)8 * E * 4);
+    dmalloc(&G.pqact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
+    dmalloc(&G.pstate, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.pstate, 0, sizeof(DeviceState)));
+    dmalloc(&G.rslots, R * sizeof(SessionSlot));
+    dmalloc(&G.cslots, 8 * sizeof(SessionSlot));
+    dmalloc(&G.pids, 8 * sizeof(int));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_rslots, R * sizeof(SessionSlot), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_cslots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_pids, 8 * sizeof(int), cudaHostAllocDefault));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    G.batch_bytes += t_dev_bytes - b0;
+    attn_sessions_smem(d_.n_ctx);
+}
+
+void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past) {
+    LlamaDevice &L0 = *c[0];
+    LlamaGroup &G = *L0.group_;
+    for (int i = 0; i < n; ++i) c[i]->sync();   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
+    if (!G.px) L0.build_prompt_workspace();
+    const int E = L0.d_.n_embd, El = L0.n_embd_local_, FFl = L0.n_ff_local_, C = L0.d_.n_ctx, S = kPrefillMax;
+    const float kq_scale = 1.0f / sqrtf((float)L0.d_.n_embd / (float)L0.d_.n_head);
+    cudaStream_t s = G.stream;
+    std::vector<int32_t> pid((size_t)S);
+    int ci = 0, cj = 0;   // next row: row cj of context ci
+    while (ci < n) {
+        // ---- the pass: rows, their slots and ids; embedding rows of each context are a contiguous run of its emb[] (queued in order)
+        int rows = 0, n_emb = 0, nf = 0;
+        RowList last{};
+        int fin_ctx[8], fin_first[8];
+        for (; ci < n && rows < S; ++ci, cj = 0) {
+            const int take = std::min(n_rows[ci] - cj, S - rows);
+            LlamaDevice &X = *c[ci];
+            int k0 = -1, k1 = -1;
+            for (int j = 0; j < take; ++j) {
+                const int id = ids[ci][cj + j], r = rows + j;
+                G.h_rslots[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+                if (id >= 0) pid[(size_t)r] = id;
+                else {
+                    const int k = -1 - id;
+                    if (k0 < 0) k0 = k;
+                    k1 = k;
+                    pid[(size_t)r] = -1 - (n_emb + k - k0);
+                }
+            }
+            if (k0 >= 0) {
+                CUDA_CHECK(cudaMemcpyAsync(L0.embd_in_ + (size_t)n_emb * E, emb[ci] + (size_t)k0 * E, (size_t)(k1 - k0 + 1) * E * 4, cudaMemcpyHostToDevice, s));
+                n_emb += k1 - k0 + 1;
+            }
+            rows += take; cj += take;
+            if (cj < n_rows[ci]) break;   // the context continues in the next pass
+            G.h_cslots[nf] = SessionSlot{n_past[ci] + n_rows[ci] - 1, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+            last.r[nf] = rows - 1; fin_ctx[nf] = ci; fin_first[nf] = rows - take;
+            ++nf;
+        }
+        CUDA_CHECK(cudaMemcpyAsync(G.rslots, G.h_rslots, (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(L0.tok_ids_, pid.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s));
+        if (nf) CUDA_CHECK(cudaMemcpyAsync(G.cslots, G.h_cslots, (size_t)nf * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+        embed_rows_kernel<<<rows, 256, 0, s>>>(L0.tok_type_, (const unsigned char *)L0.tok_raw_, gg_row_bytes(L0.tok_type_, (size_t)E), E, L0.tok_ids_, L0.embd_in_, G.px);
+        ++L0.launches_;
+
+        // ---- the layers
+        const bool gemm = L0.pf_ready_ && rows >= 2;
+        for (int il = 0; il < L0.d_.n_layer; ++il) {
+            Layer &L = L0.layers_[(size_t)il];
+            const size_t kv_off = (size_t)il * C * El;
+            if (gemm) {
+                L0.pf_stage(L.qkv, G.px, E, L.attn_norm, L0.pf_S_e_, rows, s);
+                { pf::PrefillArgs a{}; a.epi = EPI_PLAIN; a.out = G.pact; a.out_stride = 3 * El; L0.pf_gemm(L.pqkv, false, a, rows, G.pstate, s); }
+                qkv_rows_kernel<<<dim3((unsigned)((3 * El / 2 + 255) / 256), (unsigned)rows), 256, 0, s>>>(G.pact, G.rslots, kv_off, G.pq, L0.rope_, El, 64);
+                ++L0.launches_;
+            } else {
+                for (int t0 = 0; t0 < rows; t0 += 8) {
+                    const int m = std::min(8, rows - t0);
+                    MatvecArgs a{};
+                    a.x = G.px + (size_t)t0 * E; a.x_stride = E; a.norm_w = L.attn_norm; a.ntok = m; a.epi = EPI_QKV; a.staged = G.pqact;
+                    a.q_out = G.pq + (size_t)t0 * El; a.rope = L0.rope_; a.e_local = El; a.half_dim = 64; a.state = G.pstate; a.tab_silu = L0.tab_silu_;
+                    if (L.fused_qkv) { a.w = L.qkv; a.part = -1; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.rslots + t0, kv_off, nt_for(m), L0.sm_count_, s, &L0.launches_); }
+                    else {
+                        const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
+                        for (int part = 0; part < 3; ++part) {
+                            const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
+                            a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows;
+                            launch_matvec_sessions(a, G.rslots + t0, kv_off, nt_for(m), L0.sm_count_, s, &L0.launches_, !same);
+                        }
+                    }
+                }
+            }
+            attn_sessions_kernel<<<dim3((unsigned)L0.n_head_local_, (unsigned)rows), 256, (size_t)C * 6, s>>>(G.pq, G.rslots, kv_off, G.patt, El, C, kq_scale, L0.tab_exp_);
+            CUDA_CHECK(cudaGetLastError()); ++L0.launches_;
+            if (gemm) {
+                L0.pf_stage(L.wo, G.patt, El, nullptr, L0.pf_S_e_, rows, s);
+                { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = G.px; a.out_stride = E; a.resid = G.px; L0.pf_gemm(L.pwo, false, a, rows, G.pstate, s); }
+                L0.pf_stage(L.w13, G.px, E, L.ffn_norm, L0.pf_S_e_, rows, s);
+                { pf::PrefillArgs a{}; a.epi = EPI_SWIGLU; a.out = G.pact; a.out_stride = FFl; L0.pf_gemm(L.pw13, false, a, rows, G.pstate, s); }
+                L0.pf_stage(L.w2, G.pact, FFl, nullptr, L0.pf_S_ff_, rows, s);
+                { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = G.px; a.out_stride = E; a.resid = G.px; L0.pf_gemm(L.pw2, true, a, rows, G.pstate, s); }
+            } else {
+                for (int t0 = 0; t0 < rows; t0 += 8) {
+                    const int m = std::min(8, rows - t0), nt = nt_for(m);
+                    float *x = G.px + (size_t)t0 * E, *act = G.pact + (size_t)t0 * FFl;
+                    MatvecArgs b{};
+                    b.w = L.wo; b.x = G.patt + (size_t)t0 * El; b.x_stride = El; b.ntok = m; b.n_valid = b.w.rows; b.state = G.pstate; b.tab_silu = L0.tab_silu_;
+                    b.staged = G.pqact; b.epi = EPI_RESID; b.out = x; b.out_stride = E; b.resid = x;
+                    launch_matvec(b, nt, L0.sm_count_, s, &L0.launches_);
+                    MatvecArgs g{};
+                    g.w = L.w13; g.x = x; g.x_stride = E; g.norm_w = L.ffn_norm; g.ntok = m; g.epi = EPI_SWIGLU; g.out = act; g.out_stride = FFl; g.n_valid = g.w.rows;
+                    g.state = G.pstate; g.tab_silu = L0.tab_silu_; g.staged = G.pqact;
+                    launch_matvec(g, nt, L0.sm_count_, s, &L0.launches_);
+                    MatvecArgs e{};
+                    e.w = L.w2; e.x = act; e.x_stride = FFl; e.ntok = m; e.n_valid = e.w.rows; e.state = G.pstate; e.tab_silu = L0.tab_silu_; e.staged = G.pqact;
+                    e.epi = EPI_RESID; e.out = x; e.out_stride = E; e.resid = x;
+                    launch_matvec(e, nt, L0.sm_count_, s, &L0.launches_);
+                }
+            }
+        }
+        CUDA_CHECK(cudaGetLastError());
+
+        // ---- contexts that end in this pass: logits + arg-max of their last row, DeviceState, hidden rows, pinned arg-max
+        if (nf) {
+            gather_rows_kernel<<<nf, 256, 0, s>>>(G.px, last, E, G.plast);
+            prepare_sessions_kernel<<<1, 32, 0, s>>>(G.cslots, nf, G.pstate);
+            MatvecArgs o{};
+            o.w = L0.output_; o.x = G.plast; o.x_stride = E; o.norm_w = L0.final_norm_; o.ntok = nf; o.epi = EPI_LOGITS; o.n_valid = L0.d_.n_vocab;
+            o.state = G.pstate; o.tab_silu = L0.tab_silu_; o.staged = G.pqact;
+            launch_matvec_sessions(o, G.cslots, 0, nt_for(nf), L0.sm_count_, s, &L0.launches_);
+            finalize_sessions_kernel<<<1, 32, 0, s>>>(G.cslots, nf, G.pids);
+            CUDA_CHECK(cudaGetLastError()); L0.launches_ += 3;
+            CUDA_CHECK(cudaMemcpyAsync(G.h_pids, G.pids, (size_t)nf * 4, cudaMemcpyDeviceToHost, s));
+            for (int f = 0; f < nf; ++f) {
+                const int k = last.r[f] + 1 - fin_first[f];
+                CUDA_CHECK(cudaMemcpyAsync(c[fin_ctx[f]]->x_, G.px + (size_t)fin_first[f] * E, (size_t)k * E * 4, cudaMemcpyDeviceToDevice, s));
+            }
+        }
+        CUDA_CHECK(cudaStreamSynchronize(s));   // (the pinned tables and the shared prompt scratch are reused by the next pass)
+        for (int f = 0; f < nf; ++f) *c[fin_ctx[f]]->h_argmax_ = G.h_pids[f];
+    }
 }
 
 // measurement seam: average CUDA-event duration (us) of one all-reduce of a [1, n_embd] partial on the tensor-parallel path in use

@@ -16,6 +16,7 @@
 namespace mg4 {
 
 struct TPLink;  // tensor-parallel communicator (tp.h)
+namespace pf { struct PrefillArgs; }   // llama_prefill.cuh
 
 struct QMat {          // one repacked weight matrix (or a fused group of matrices of one type)
     int type = -1;     // GGType
@@ -69,6 +70,12 @@ public:
     // on-device greedy id) at position n_past[i]; afterwards each context holds what its own decode_step would have left (logits,
     // arg-max, DeviceState) and ids_out[i] = its new arg-max.  Synchronous.  The caller validates (distinct, one group, ranges).
     static void decode_batch(LlamaDevice *const *ctx, int n, const int32_t *ids, const int *n_past, int32_t *ids_out);
+    // The queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights, kPrefillMax rows per pass:
+    // context i has n_rows[i] (1..kPrefillMax) rows starting at position n_past[i], ids[i][j] >= 0 a token, < 0 row -1 - ids[i][j] of
+    // emb[i] (n_embd floats per row, in order of first use).  Afterwards each context holds what its own eval_rows would have left
+    // (KV cache, logits, arg-max, DeviceState) and the first rows of its hidden state are its rows of the pass that evaluated its
+    // last row.  Synchronous.  The caller validates (distinct, one group, rows checked when they were queued).
+    static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past);
     const LlamaDims &dims() const { return d_; }
     // Evaluate `n` tokens / embedding rows starting at position n_past. Afterwards logits of the last row are
     // on device and the arg-max id is known.  Returns false if the context would overflow.
@@ -110,6 +117,10 @@ private:
     struct Layer { QMat qkv, wq, wk, wv, wo, w13, w2; bool fused_qkv; float *attn_norm, *ffn_norm; PQMat pqkv, pwo, pw13, pw2; };
     bool build_prefill();            // tensor-core prefill (llama_prefill.cuh): homogeneous Q4_0 / Q4_1 layers, single GPU
     void prefill_chunk(int n, bool want_logits);   // n <= kPrefillMax rows that sit in x_
+    // one matrix of a prefill pass over n rows on stream s: stage the input rows into the shared operand scratch, then the GEMM
+    // (state: the n_past that EPI_QKV reads)
+    void pf_stage(const QMat &w, const float *x, int x_stride, const float *norm_w, int S, int n, cudaStream_t s);
+    void pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, int n, const DeviceState *state, cudaStream_t s);
     bool pf_ready_ = false; int pf_S_e_ = 0, pf_S_ff_ = 0;
     signed char *pf_q8_ = nullptr; void *pf_sc_ = nullptr; int32_t *tok_ids_ = nullptr; void *pf_part_ = nullptr; size_t pf_part_bytes_ = 0;
     alignas(64) unsigned char pf_tmB_e_[128], pf_tmS_e_[128], pf_tmB_ff_[128], pf_tmS_ff_[128];
@@ -153,6 +164,7 @@ private:
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group
     void build_batch_graph(int B);   // decode_batch's graph for B columns, captured on the group stream
+    void build_prompt_workspace();   // eval_rows_batch's rows, slot tables and stream (group-owned, at the first batched flush)
 };
 
 }  // namespace mg4

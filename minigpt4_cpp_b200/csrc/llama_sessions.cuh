@@ -1,5 +1,5 @@
-// llama_sessions.cuh — sm_90a kernels of the batched decode step over several contexts that share one model
-// (minigpt4_b200_decode_batch; host side LlamaDevice::decode_batch in llama.cu, design DESIGN.md §4.8).
+// llama_sessions.cuh — sm_90a kernels of the batched decode step and the batched prompt pass over several contexts that share one
+// model (minigpt4_b200_decode_batch / flush_batch; host side LlamaDevice::decode_batch / eval_rows_batch in llama.cu, DESIGN.md §4.8).
 //
 // Column t of a batch belongs to context t: its own position, KV cache, logits buffer and DeviceState come from a small
 // device table (SessionSlot[B]) that the host refreshes with one copy per step, so the captured graph of each batch size is
@@ -119,6 +119,40 @@ __global__ void finalize_sessions_kernel(const SessionSlot *slots, int B, int *i
         st->n_tok = 1;
         ids_out[t] = id;
     }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// batched prompt pass (minigpt4_b200_flush_batch; host side LlamaDevice::eval_rows_batch): the queued rows of several contexts
+// concatenated, row t at its own context's position slots[t].n_past with that context's caches.  The per-op path appends through
+// matvec_sessions_kernel's EPI_QKV one 8-row chunk at a time; the tensor-core path runs the fused qkv GEMM with EPI_PLAIN into
+// qkv[rows][3 E] and this kernel applies pf::prefill_epilogue's RoPE and F16 append per row (the same expressions, so the same bits).
+// grid (ceil(3 E / 2 / 256), rows), block 256: one thread per adjacent row pair (r0, r0 + 1) of row t
+// ---------------------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) qkv_rows_kernel(const float *__restrict__ qkv, const SessionSlot *slots, size_t kv_off, float *__restrict__ q_out,
+                                                       const float2 *__restrict__ rope, int E, int half_dim) {
+    const int t = blockIdx.y, p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= 3 * E / 2) return;
+    const int r0 = 2 * p, part = r0 / E, rr = r0 % E;
+    const float v0 = qkv[(size_t)t * 3 * E + r0], v1 = qkv[(size_t)t * 3 * E + r0 + 1];
+    const SessionSlot &s = slots[t];
+    const int pos = s.n_past;
+    if (part == 2) {
+        s.vcache[kv_off + (size_t)pos * E + rr] = __float2half_rn(v0);
+        s.vcache[kv_off + (size_t)pos * E + rr + 1] = __float2half_rn(v1);
+    } else {
+        const float2 cs = rope[(size_t)pos * half_dim + (rr % (2 * half_dim)) / 2];
+        const float o0 = v0 * cs.x - v1 * cs.y, o1 = v0 * cs.y + v1 * cs.x;
+        if (part == 0) { q_out[(size_t)t * E + rr] = o0; q_out[(size_t)t * E + rr + 1] = o1; }
+        else { s.kcache[kv_off + (size_t)pos * E + rr] = __float2half_rn(o0); s.kcache[kv_off + (size_t)pos * E + rr + 1] = __float2half_rn(o1); }
+    }
+}
+
+struct RowList { int r[8]; };   // rows of a pass, by value
+
+// the last row of each context that ends in this pass -> contiguous rows for the logits matvec; grid = n rows
+__global__ void gather_rows_kernel(const float *__restrict__ x, const RowList rows, int E, float *__restrict__ out) {
+    const float *src = x + (size_t)rows.r[blockIdx.x] * E;
+    for (int i = threadIdx.x; i < E; i += blockDim.x) out[(size_t)blockIdx.x * E + i] = src[i];
 }
 
 }  // namespace k

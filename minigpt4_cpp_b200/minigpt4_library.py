@@ -219,6 +219,7 @@ _EXT = {
     "minigpt4_b200_session_create": ([_CTX, _I], _CTX),
     "minigpt4_b200_session_info": ([_CTX, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "minigpt4_b200_decode_batch": ([_VP, _I, _VP, _VP], _I),
+    "minigpt4_b200_flush_batch": ([_VP, _I], _I),
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
@@ -331,6 +332,10 @@ class B200:
         out = np.zeros(max(1, n), np.int32)
         self._chk(self.L.minigpt4_b200_decode_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), n, _ptr(a), _ptr(out)))
         return out[:n]
+
+    def flush_batch(self, ctxs) -> None:
+        """evaluate the queued prompt rows of every context in `ctxs` (1..8 of one group) in shared passes over the weights"""
+        self._chk(self.L.minigpt4_b200_flush_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), len(ctxs)))
 
     def end_chat_batch(self, ctxs, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
                        repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 1.0, alpha_frequency: float = 1.0,
