@@ -59,7 +59,7 @@ MINIGPT4_API int minigpt4_b200_decode_chain(struct MiniGPT4Context *ctx, int ste
 MINIGPT4_API struct MiniGPT4Context *minigpt4_b200_session_create(struct MiniGPT4Context *ctx, int seed);
 /* live contexts of ctx's group; device bytes ctx owns (KV cache 2 * n_layer * n_ctx * n_embd * 2 B plus its activations of
  * 512 prompt rows and a few small buffers); device bytes it shares with its group (weights, operand cache, tables, prefill
- * scratch, the batched step's workspace once built).  Any pointer may be NULL. */
+ * scratch, the workspace of the batched calls once built).  Any pointer may be NULL. */
 MINIGPT4_API int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_contexts, double *owned_bytes, double *shared_bytes);
 /* One decode step of n (1..8) distinct contexts of one group: the weights stream once for all of them.  Context i is fed ids[i]
  * (ids[i] < 0: its current on-device greedy id, as in minigpt4_b200_decode_chain) at its own n_past; queued prompt pieces of

@@ -18,56 +18,60 @@ static size_t g_max_dyn_smem = 0;
 static thread_local size_t t_dev_bytes = 0;
 template <class T> static void dmalloc(T **p, size_t n) { CUDA_CHECK(cudaMalloc((void **)p, n)); t_dev_bytes += n; }
 
-// what the contexts of one model share besides the weight pointers each of them holds: the batched decode step's workspace,
-// stream and graphs (built by the group's first decode_batch of each size) and the batched prompt pass's workspace
+// what the contexts of one model share besides the weight pointers each of them holds: the workspace of the batched passes (built by
+// the group's first decode_batch or batched flush; decode_batch uses its first 8 rows), their stream and the batched decode step's graphs
 struct LlamaGroup {
     size_t weight_bytes = 0;       // the parent's load minus its own context: weights, operand cache, tables, prefill scratch
     size_t batch_bytes = 0;
     cudaStream_t stream = nullptr;
-    float *x = nullptr, *q = nullptr, *att = nullptr, *act = nullptr;   // [8] rows
+    float *x = nullptr, *q = nullptr, *att = nullptr, *act = nullptr;   // [kPrefillMax] rows (act also holds the qkv GEMM's [rows][3 n_embd] output)
+    float *last = nullptr;         // [8] the last rows of the contexts that end in a prompt pass
     unsigned char *qact = nullptr;
-    DeviceState *state = nullptr;  // the batch's tokens (embed_* gather column t from tokens[t])
-    SessionSlot *slots = nullptr, *h_slots = nullptr;
-    int *ids = nullptr, *h_ids = nullptr;
+    DeviceState *state = nullptr;  // the batch's tokens (the decode graph's embed gathers column t from tokens[t])
+    SessionSlot *rows = nullptr, *h_rows = nullptr;     // [kPrefillMax] a slot per row of a prompt pass
+    SessionSlot *slots = nullptr, *h_slots = nullptr;   // [8] a slot per context: the columns of a decode step, the contexts that end in a prompt pass
+    int *ids = nullptr, *h_ids = nullptr;               // [8] their new arg-max ids
     cudaGraphExec_t graph[9] = {};
     int graph_kernels[9] = {};
-    // the batched prompt pass (eval_rows_batch, built by the group's first batched flush): kPrefillMax rows of activations (pact also
-    // holds the qkv GEMM's [rows][3 n_embd] output), the last rows of the contexts that end in a pass, a slot per row and per context
-    float *px = nullptr, *pq = nullptr, *patt = nullptr, *pact = nullptr, *plast = nullptr;
-    unsigned char *pqact = nullptr;
-    DeviceState *pstate = nullptr;
-    SessionSlot *rslots = nullptr, *h_rslots = nullptr, *cslots = nullptr, *h_cslots = nullptr;
-    int *pids = nullptr, *h_pids = nullptr;
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
-        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)qact, (void *)state, (void *)slots, (void *)ids}) if (p) cudaFree(p);
-        for (void *p : {(void *)px, (void *)pq, (void *)patt, (void *)pact, (void *)plast, (void *)pqact, (void *)pstate, (void *)rslots, (void *)cslots, (void *)pids})
+        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)rows, (void *)slots, (void *)ids})
             if (p) cudaFree(p);
-        for (void *p : {(void *)h_slots, (void *)h_ids, (void *)h_rslots, (void *)h_cslots, (void *)h_pids}) if (p) cudaFreeHost(p);
+        for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids}) if (p) cudaFreeHost(p);
         if (stream) cudaStreamDestroy(stream);
     }
 };
 
+// matvec_kernel, or with a slot table matvec_sessions_kernel (per-context positions, caches and logits; llama_sessions.cuh)
 template <int WT, int NT>
-static void launch_mv(const MatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
-    static bool configured[64] = {};   // the attribute is per device (minigpt4_b200_set_device: several contexts of one process may sit on different GPUs)
+static void launch_mv(const MatvecArgs &a, const SessionSlot *slots, size_t kv_off, int grid, size_t smem, cudaStream_t s) {
+    static bool configured[2][64] = {};   // the attribute is per device (minigpt4_b200_set_device: several contexts of one process may sit on different GPUs)
     int dev = 0; cudaGetDevice(&dev);
-    if (!configured[dev & 63]) {
-        CUDA_CHECK(cudaFuncSetAttribute(matvec_kernel<WT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g_max_dyn_smem));
-        configured[dev & 63] = true;
+    bool &done = configured[slots != nullptr][dev & 63];
+    if (!done) {
+        const void *fn = slots ? (const void *)matvec_sessions_kernel<WT, NT> : (const void *)matvec_kernel<WT, NT>;
+        CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g_max_dyn_smem));
+        done = true;
     }
-    matvec_kernel<WT, NT><<<grid, kThreads, smem, s>>>(a);
+    if (slots) matvec_sessions_kernel<WT, NT><<<grid, kThreads, smem, s>>>(SessionMatvecArgs{a, slots, kv_off});
+    else matvec_kernel<WT, NT><<<grid, kThreads, smem, s>>>(a);
 }
 template <int WT>
-static void launch_mv_nt(int nt, const MatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
+static void launch_mv_nt(int nt, const MatvecArgs &a, const SessionSlot *slots, size_t kv_off, int grid, size_t smem, cudaStream_t s) {
     switch (nt) {
-        case 1: launch_mv<WT, 1>(a, grid, smem, s); break;
-        case 2: launch_mv<WT, 2>(a, grid, smem, s); break;
-        case 4: launch_mv<WT, 4>(a, grid, smem, s); break;
-        default: launch_mv<WT, 8>(a, grid, smem, s); break;
+        case 1: launch_mv<WT, 1>(a, slots, kv_off, grid, smem, s); break;
+        case 2: launch_mv<WT, 2>(a, slots, kv_off, grid, smem, s); break;
+        case 4: launch_mv<WT, 4>(a, slots, kv_off, grid, smem, s); break;
+        default: launch_mv<WT, 8>(a, slots, kv_off, grid, smem, s); break;
     }
 }
 static int nt_for(int ntok) { return ntok <= 1 ? 1 : ntok <= 2 ? 2 : ntok <= 4 ? 4 : 8; }
+// the fields every matvec of a pass shares
+static MatvecArgs mv_args(const QMat &w, int ntok, DeviceState *state, unsigned char *staged, const __half *tab_silu) {
+    MatvecArgs a{};
+    a.w = w; a.n_valid = w.rows; a.ntok = ntok; a.state = state; a.staged = staged; a.tab_silu = tab_silu;
+    return a;
+}
 
 static void launch_stage(const MatvecArgs &a, cudaStream_t s, unsigned long long *counter) {
     const int act = act_of(a.w.type);
@@ -81,10 +85,12 @@ static void launch_stage(const MatvecArgs &a, cudaStream_t s, unsigned long long
     CUDA_CHECK(cudaGetLastError());
     if (counter) ++*counter;
 }
+// a.ntok (<= 8) rows through one matrix; slots / kv_off: matvec_sessions_kernel (EPI_QKV / EPI_LOGITS into each row's own context).
 // restage = false when the previous launch staged the same input in the same format (unfused q/k/v of one type)
-static void launch_matvec(MatvecArgs a, int nt, int sm_count, cudaStream_t s, unsigned long long *counter, bool restage = true) {
+static void launch_matvec(MatvecArgs a, int sm_count, cudaStream_t s, unsigned long long *counter, const SessionSlot *slots = nullptr, size_t kv_off = 0,
+                          bool restage = true) {
     if (restage) launch_stage(a, s, counter);
-    const int rows = a.w.rows;
+    const int rows = a.w.rows, nt = nt_for(a.ntok);
     const int target = 2 * sm_count * kWarps;
     int rpw = (rows + target - 1) / target;
     rpw = std::max(2, (rpw + 1) & ~1);
@@ -93,67 +99,30 @@ static void launch_matvec(MatvecArgs a, int nt, int sm_count, cudaStream_t s, un
     const size_t smem = (size_t)nt * act_bytes(act_of(a.w.type), a.w.cols);
     if (smem > g_max_dyn_smem) MG4_PANIC("activation staging needs %zu B of shared memory (> %zu)", smem, g_max_dyn_smem);
     switch (a.w.type) {
-        case GG_Q4_0: launch_mv_nt<GG_Q4_0>(nt, a, grid, smem, s); break;
-        case GG_Q4_1: launch_mv_nt<GG_Q4_1>(nt, a, grid, smem, s); break;
-        case GG_Q5_K: launch_mv_nt<GG_Q5_K>(nt, a, grid, smem, s); break;
-        case GG_Q4_K: launch_mv_nt<GG_Q4_K>(nt, a, grid, smem, s); break;
-        case GG_Q5_0: launch_mv_nt<GG_Q5_0>(nt, a, grid, smem, s); break;
-        case GG_Q5_1: launch_mv_nt<GG_Q5_1>(nt, a, grid, smem, s); break;
-        case GG_Q8_0: launch_mv_nt<GG_Q8_0>(nt, a, grid, smem, s); break;
-        case GG_Q6_K: launch_mv_nt<GG_Q6_K>(nt, a, grid, smem, s); break;
-        case GG_F16: launch_mv_nt<GG_F16>(nt, a, grid, smem, s); break;
+        case GG_Q4_0: launch_mv_nt<GG_Q4_0>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q4_1: launch_mv_nt<GG_Q4_1>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q5_K: launch_mv_nt<GG_Q5_K>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q4_K: launch_mv_nt<GG_Q4_K>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q5_0: launch_mv_nt<GG_Q5_0>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q5_1: launch_mv_nt<GG_Q5_1>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q8_0: launch_mv_nt<GG_Q8_0>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_Q6_K: launch_mv_nt<GG_Q6_K>(nt, a, slots, kv_off, grid, smem, s); break;
+        case GG_F16: launch_mv_nt<GG_F16>(nt, a, slots, kv_off, grid, smem, s); break;
         default: MG4_PANIC("no matvec kernel for ggml type %d", a.w.type);
     }
     CUDA_CHECK(cudaGetLastError());
     if (counter) ++*counter;
 }
 
-// the batched decode step's QKV and logits matrices (llama_sessions.cuh): same grid and staging as launch_matvec
-template <int WT, int NT>
-static void launch_mvs(const SessionMatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
-    static bool configured[64] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!configured[dev & 63]) {
-        CUDA_CHECK(cudaFuncSetAttribute(matvec_sessions_kernel<WT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g_max_dyn_smem));
-        configured[dev & 63] = true;
-    }
-    matvec_sessions_kernel<WT, NT><<<grid, kThreads, smem, s>>>(a);
-}
-template <int WT>
-static void launch_mvs_nt(int nt, const SessionMatvecArgs &a, int grid, size_t smem, cudaStream_t s) {
-    switch (nt) {
-        case 1: launch_mvs<WT, 1>(a, grid, smem, s); break;
-        case 2: launch_mvs<WT, 2>(a, grid, smem, s); break;
-        case 4: launch_mvs<WT, 4>(a, grid, smem, s); break;
-        default: launch_mvs<WT, 8>(a, grid, smem, s); break;
-    }
-}
-static void launch_matvec_sessions(const MatvecArgs &m, const SessionSlot *slots, size_t kv_off, int nt, int sm_count, cudaStream_t s, unsigned long long *counter,
-                                   bool restage = true) {
-    if (restage) launch_stage(m, s, counter);
-    SessionMatvecArgs a{m, slots, kv_off};
-    const int rows = m.w.rows;
-    const int target = 2 * sm_count * kWarps;
-    int rpw = (rows + target - 1) / target;
-    rpw = std::max(2, (rpw + 1) & ~1);
-    a.m.rows_per_warp = rpw;
-    const int grid = (rows + kWarps * rpw - 1) / (kWarps * rpw);
-    const size_t smem = (size_t)nt * act_bytes(act_of(m.w.type), m.w.cols);
-    if (smem > g_max_dyn_smem) MG4_PANIC("activation staging needs %zu B of shared memory (> %zu)", smem, g_max_dyn_smem);
-    switch (m.w.type) {
-        case GG_Q4_0: launch_mvs_nt<GG_Q4_0>(nt, a, grid, smem, s); break;
-        case GG_Q4_1: launch_mvs_nt<GG_Q4_1>(nt, a, grid, smem, s); break;
-        case GG_Q5_K: launch_mvs_nt<GG_Q5_K>(nt, a, grid, smem, s); break;
-        case GG_Q4_K: launch_mvs_nt<GG_Q4_K>(nt, a, grid, smem, s); break;
-        case GG_Q5_0: launch_mvs_nt<GG_Q5_0>(nt, a, grid, smem, s); break;
-        case GG_Q5_1: launch_mvs_nt<GG_Q5_1>(nt, a, grid, smem, s); break;
-        case GG_Q8_0: launch_mvs_nt<GG_Q8_0>(nt, a, grid, smem, s); break;
-        case GG_Q6_K: launch_mvs_nt<GG_Q6_K>(nt, a, grid, smem, s); break;
-        case GG_F16: launch_mvs_nt<GG_F16>(nt, a, grid, smem, s); break;
-        default: MG4_PANIC("no matvec kernel for ggml type %d", m.w.type);
-    }
-    CUDA_CHECK(cudaGetLastError());
-    if (counter) ++*counter;
+// attention scratch = n_ctx * 6 bytes of dynamic shared memory.  The attribute is per device and kernel, and it only grows: contexts of one
+// process may differ in n_ctx, and lowering it would make every later attention launch of a context with a larger n_ctx fail.
+static void attn_smem(int n_ctx) {
+    static int set[2][64] = {};
+    int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
+    const int need = std::max(49152, n_ctx * 6);
+    const void *fn[2] = {(const void *)attn_kernel, (const void *)attn_sessions_kernel};
+    for (int k = 0; k < 2; ++k)
+        if (need > set[k][dev & 63]) { CUDA_CHECK(cudaFuncSetAttribute(fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize, need)); set[k][dev & 63] = need; }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -343,7 +312,6 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     dmalloc(&tok_ids_, R * 4);
     dmalloc(&embd_in_, (size_t)512 * E * 4);
     CUDA_CHECK(cudaDeviceSynchronize());
-    CUDA_CHECK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(49152, d_.n_ctx * 6)));
     if (tp_ && tp_->world > 1) tp_->setup_peers(E, stream_);
     pf_ready_ = build_prefill();
     { const size_t b = t_dev_bytes; build_graph(); owned_bytes_ += t_dev_bytes - b; }
@@ -358,6 +326,7 @@ void LlamaDevice::alloc_context() {
     const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_;
     CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     CUDA_CHECK(cudaEventCreate(&ev0_)); CUDA_CHECK(cudaEventCreate(&ev1_));
+    attn_smem(d_.n_ctx);
     const size_t kv = (size_t)d_.n_layer * d_.n_ctx * El;
     dmalloc(&kcache_, kv * 2); CUDA_CHECK(cudaMemset(kcache_, 0, kv * 2));
     dmalloc(&vcache_, kv * 2); CUDA_CHECK(cudaMemset(vcache_, 0, kv * 2));
@@ -393,89 +362,122 @@ bool LlamaDevice::load_session(const LlamaDevice &p) {
 size_t LlamaDevice::shared_bytes() const { return group_ ? group_->weight_bytes + group_->batch_bytes : 0; }
 
 // ------------------------------------------------------------------------------------------------
-// one pass of all layers over `ntok` (<= nt) rows that sit in x_; positions/tokens come from *state_
+// one pass of all layers over p.rows rows that sit in p.x: every caller (decode graph, prompt passes, the batched decode step and the
+// batched prompt pass) records its layers here
 // ------------------------------------------------------------------------------------------------
-void LlamaDevice::launch_layers(int nt, int ntok, bool want_logits) {
+void LlamaDevice::record_layers(const Pass &p) {
     const int E = d_.n_embd, El = n_embd_local_, FFl = n_ff_local_, C = d_.n_ctx;
-    const bool tp = tp_ && tp_->world > 1;
     const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
-    const size_t attn_smem = (size_t)C * 6;
+    if (!p.slots && !p.gemm && p.rows > 8) MG4_PANIC("a per-op pass without a slot table takes at most 8 rows (got %d)", p.rows);  // (positions n_past + t of one launch)
+    auto mv = [&](const QMat &w, int m) { return mv_args(w, m, p.state, p.qact, tab_silu_); };
     for (int il = 0; il < d_.n_layer; ++il) {
         Layer &L = layers_[(size_t)il];
-        __half *kc = kcache_ + (size_t)il * C * El, *vc = vcache_ + (size_t)il * C * El;
-        MatvecArgs a{};
-        a.x = x_; a.x_stride = E; a.norm_w = L.attn_norm; a.ntok = ntok; a.epi = EPI_QKV; a.staged = qact_;
-        a.q_out = q_; a.kcache = kc; a.vcache = vc; a.rope = rope_; a.e_local = El; a.half_dim = 64; a.state = state_; a.tab_silu = tab_silu_;
-        if (L.fused_qkv) { a.w = L.qkv; a.part = -1; a.n_valid = a.w.rows; launch_matvec(a, nt, sm_count_, stream_, &launches_); }
-        else {
-            const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
-            for (int part = 0; part < 3; ++part) {
-                const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
-                a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows; launch_matvec(a, nt, sm_count_, stream_, &launches_, !same);
+        const size_t kv_off = (size_t)il * C * El;
+        // qkv: RoPE, and the F16 K / V rows appended at each row's position
+        if (p.gemm) {
+            pf_stage(L.qkv, p.x, E, L.attn_norm, pf_S_e_, p);
+            pf::PrefillArgs a{};
+            if (p.slots) { a.epi = EPI_PLAIN; a.out = p.act; a.out_stride = 3 * El; }
+            else { a.epi = EPI_QKV; a.q_out = p.q; a.kcache = kcache_ + kv_off; a.vcache = vcache_ + kv_off; a.rope = rope_; a.e_local = El; a.half_dim = 64; }
+            pf_gemm(L.pqkv, false, a, p);
+            if (p.slots) {
+                qkv_rows_kernel<<<dim3((unsigned)((3 * El / 2 + 255) / 256), (unsigned)p.rows), 256, 0, p.s>>>(p.act, p.slots, kv_off, p.q, rope_, El, 64);
+                ++*p.counter;
+            }
+        } else {
+            for (int t0 = 0; t0 < p.rows; t0 += 8) {
+                MatvecArgs a = mv(L.qkv, std::min(8, p.rows - t0));
+                a.x = p.x + (size_t)t0 * E; a.x_stride = E; a.norm_w = L.attn_norm; a.epi = EPI_QKV;
+                a.q_out = p.q + (size_t)t0 * El; a.rope = rope_; a.e_local = El; a.half_dim = 64;
+                if (!p.slots) { a.kcache = kcache_ + kv_off; a.vcache = vcache_ + kv_off; }
+                const SessionSlot *sl = p.slots ? p.slots + t0 : nullptr;
+                if (L.fused_qkv) { a.part = -1; launch_matvec(a, sm_count_, p.s, p.counter, sl, kv_off); }
+                else {
+                    const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
+                    for (int part = 0; part < 3; ++part) {
+                        const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
+                        a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows;
+                        launch_matvec(a, sm_count_, p.s, p.counter, sl, kv_off, !same);
+                    }
+                }
             }
         }
-        attn_kernel<<<dim3((unsigned)n_head_local_, (unsigned)ntok), 256, attn_smem, stream_>>>(q_, kc, vc, att_, state_, El, C, kq_scale, tab_exp_);
-        CUDA_CHECK(cudaGetLastError()); ++launches_;
-
-        MatvecArgs b{};
-        b.w = L.wo; b.x = att_; b.x_stride = El; b.norm_w = nullptr; b.ntok = ntok; b.n_valid = b.w.rows; b.state = state_; b.tab_silu = tab_silu_; b.staged = qact_;
-        if (!tp) { b.epi = EPI_RESID; b.out = x_; b.out_stride = E; b.resid = x_; launch_matvec(b, nt, sm_count_, stream_, &launches_); }
-        else if (tp_->peers_ready()) {   // partial -> this rank's exchange buffer; ONE kernel: signal peers, wait, sum all partials + residual out of peer memory
-            b.epi = EPI_PLAIN; b.out = tp_->partial_out(); b.out_stride = E; launch_matvec(b, nt, sm_count_, stream_, &launches_);
-            tp_->all_reduce_resid(x_, x_, (size_t)ntok * E, stream_); ++launches_;
+        const dim3 ag((unsigned)n_head_local_, (unsigned)p.rows);
+        if (p.slots) attn_sessions_kernel<<<ag, 256, (size_t)C * 6, p.s>>>(p.q, p.slots, kv_off, p.att, El, C, kq_scale, tab_exp_);
+        else attn_kernel<<<ag, 256, (size_t)C * 6, p.s>>>(p.q, kcache_ + kv_off, vcache_ + kv_off, p.att, p.state, El, C, kq_scale, tab_exp_);
+        CUDA_CHECK(cudaGetLastError()); ++*p.counter;
+        // wo, gate/up, down
+        if (p.gemm) {
+            pf_stage(L.wo, p.att, El, nullptr, pf_S_e_, p);
+            { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = p.x; a.out_stride = E; a.resid = p.x; pf_gemm(L.pwo, false, a, p); }
+            pf_stage(L.w13, p.x, E, L.ffn_norm, pf_S_e_, p);
+            { pf::PrefillArgs a{}; a.epi = EPI_SWIGLU; a.out = p.act; a.out_stride = FFl; pf_gemm(L.pw13, false, a, p); }
+            pf_stage(L.w2, p.act, FFl, nullptr, pf_S_ff_, p);
+            { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = p.x; a.out_stride = E; a.resid = p.x; pf_gemm(L.pw2, true, a, p); }
         } else {
-            b.epi = EPI_PLAIN; b.out = partial_; b.out_stride = E; launch_matvec(b, nt, sm_count_, stream_, &launches_);
-            tp_->all_reduce_sum(partial_, (size_t)ntok * E, stream_);
-            add_kernel<<<(ntok * E + 255) / 256, 256, 0, stream_>>>(x_, partial_, ntok * E); ++launches_;
-        }
-        MatvecArgs c{};
-        c.w = L.w13; c.x = x_; c.x_stride = E; c.norm_w = L.ffn_norm; c.ntok = ntok; c.epi = EPI_SWIGLU; c.out = act_; c.out_stride = FFl; c.n_valid = c.w.rows;
-        c.state = state_; c.tab_silu = tab_silu_; c.staged = qact_;
-        launch_matvec(c, nt, sm_count_, stream_, &launches_);
-        MatvecArgs e{};
-        e.w = L.w2; e.x = act_; e.x_stride = FFl; e.norm_w = nullptr; e.ntok = ntok; e.n_valid = e.w.rows; e.state = state_; e.tab_silu = tab_silu_; e.staged = qact_;
-        if (!tp) { e.epi = EPI_RESID; e.out = x_; e.out_stride = E; e.resid = x_; launch_matvec(e, nt, sm_count_, stream_, &launches_); }
-        else if (tp_->peers_ready()) {   // partial -> this rank's exchange buffer; ONE kernel: signal peers, wait, sum all partials + residual out of peer memory
-            e.epi = EPI_PLAIN; e.out = tp_->partial_out(); e.out_stride = E; launch_matvec(e, nt, sm_count_, stream_, &launches_);
-            tp_->all_reduce_resid(x_, x_, (size_t)ntok * E, stream_); ++launches_;
-        } else {
-            e.epi = EPI_PLAIN; e.out = partial_; e.out_stride = E; launch_matvec(e, nt, sm_count_, stream_, &launches_);
-            tp_->all_reduce_sum(partial_, (size_t)ntok * E, stream_);
-            add_kernel<<<(ntok * E + 255) / 256, 256, 0, stream_>>>(x_, partial_, ntok * E); ++launches_;
+            for (int t0 = 0; t0 < p.rows; t0 += 8) {
+                const int m = std::min(8, p.rows - t0);
+                float *x = p.x + (size_t)t0 * E, *act = p.act + (size_t)t0 * FFl;
+                MatvecArgs b = mv(L.wo, m);
+                b.x = p.att + (size_t)t0 * El; b.x_stride = El;
+                add_matvec(b, x, p);
+                MatvecArgs g = mv(L.w13, m);
+                g.x = x; g.x_stride = E; g.norm_w = L.ffn_norm; g.epi = EPI_SWIGLU; g.out = act; g.out_stride = FFl;
+                launch_matvec(g, sm_count_, p.s, p.counter);
+                MatvecArgs e = mv(L.w2, m);
+                e.x = act; e.x_stride = FFl;
+                add_matvec(e, x, p);
+            }
         }
     }
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// wo / down: the product added into the residual rows x.  A tensor-parallel rank adds the sum of every rank's partial product: one kernel
+// over peer memory (signal, wait, sum, residual), or NCCL and an add.
+void LlamaDevice::add_matvec(MatvecArgs a, float *x, const Pass &p) {
+    const int E = d_.n_embd;
+    const size_t n = (size_t)a.ntok * E;
+    a.out_stride = E;
+    if (!tp_ || tp_->world <= 1) { a.epi = EPI_RESID; a.out = x; a.resid = x; launch_matvec(a, sm_count_, p.s, p.counter); }
+    else if (tp_->peers_ready()) {
+        a.epi = EPI_PLAIN; a.out = tp_->partial_out(); launch_matvec(a, sm_count_, p.s, p.counter);
+        tp_->all_reduce_resid(x, x, n, p.s); ++*p.counter;
+    } else {
+        a.epi = EPI_PLAIN; a.out = partial_; launch_matvec(a, sm_count_, p.s, p.counter);
+        tp_->all_reduce_sum(partial_, n, p.s);
+        add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, p.s>>>(x, partial_, (int)n); ++*p.counter;
+    }
+}
+
+// one pass of this context over n rows that sit in x_ at positions state_->n_past + t, then (want_logits) the logits and arg-max of the
+// last row, finalize (n_past += n) and the 4-byte arg-max to pinned memory (valid after the next stream sync)
+void LlamaDevice::record_pass(int n, bool want_logits) {
+    record_layers(Pass{n, x_, q_, att_, act_, qact_, state_, nullptr, pf_ready_ && n >= 2, stream_, &launches_});
     if (want_logits) {
-        MatvecArgs o{};
-        o.w = output_; o.x = x_ + (size_t)(ntok - 1) * E; o.x_stride = E; o.norm_w = final_norm_; o.ntok = 1; o.epi = EPI_LOGITS; o.out = logits_; o.n_valid = d_.n_vocab;
-        o.state = state_; o.tab_silu = tab_silu_; o.staged = qact_;
-        launch_matvec(o, 1, sm_count_, stream_, &launches_);
+        MatvecArgs o = mv_args(output_, 1, state_, qact_, tab_silu_);
+        o.x = x_ + (size_t)(n - 1) * d_.n_embd; o.x_stride = d_.n_embd; o.norm_w = final_norm_; o.epi = EPI_LOGITS; o.out = logits_; o.n_valid = d_.n_vocab;
+        launch_matvec(o, sm_count_, stream_, &launches_);
     }
     finalize_kernel<<<1, 32, 0, stream_>>>(state_, want_logits ? 1 : 0, nullptr); ++launches_;
     CUDA_CHECK(cudaGetLastError());
-    // 4-byte result of the step for the greedy fast path (pinned; valid after the next stream sync)
     if (want_logits) CUDA_CHECK(cudaMemcpyAsync(h_argmax_, &state_->argmax_id, 4, cudaMemcpyDeviceToHost, stream_));
 }
 
-void LlamaDevice::run_chunk(int n, bool want_logits, bool from_tokens) {
-    // h_state_ already holds n_past / n_tok / tokens for this chunk
-    CUDA_CHECK(cudaMemcpyAsync(state_, h_state_, offsetof(DeviceState, argmax_key), cudaMemcpyHostToDevice, stream_));
-    if (from_tokens) {
-        if (tok_type_ == GG_Q4_K) embed_q4k_kernel<<<n, 256, 0, stream_>>>((const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        else if (tok_type_ == GG_Q5_0 || tok_type_ == GG_Q5_1 || tok_type_ == GG_Q8_0) embed_b32_kernel<<<n, 256, 0, stream_>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        else embed_kernel<<<n, 256, 0, stream_>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        ++launches_;
-    }
-    launch_layers(nt_for(n), n, want_logits);
-    CUDA_CHECK(cudaStreamSynchronize(stream_));  // h_state_ is rewritten by the next chunk
+// the token-embedding rows of the decode graphs: row t gathers DeviceState::tokens[t]
+void LlamaDevice::launch_embed(int n, const DeviceState *st, float *x, cudaStream_t s, unsigned long long *counter) const {
+    const unsigned char *tok = (const unsigned char *)tok_raw_;
+    const size_t rb = gg_row_bytes(tok_type_, (size_t)d_.n_embd);
+    if (tok_type_ == GG_Q4_K) embed_q4k_kernel<<<n, 256, 0, s>>>(tok, rb, d_.n_embd, st, x);
+    else if (tok_type_ == GG_Q5_0 || tok_type_ == GG_Q5_1 || tok_type_ == GG_Q8_0) embed_b32_kernel<<<n, 256, 0, s>>>(tok_type_, tok, rb, d_.n_embd, st, x);
+    else embed_kernel<<<n, 256, 0, s>>>(tok_type_, tok, rb, d_.n_embd, st, x);
+    CUDA_CHECK(cudaGetLastError()); ++*counter;
 }
 
 // One or more passes over `n` mixed rows starting at position n_past: ids[i] >= 0 is a token, ids[i] < 0 is row -1 - ids[i] of emb_host
 // (n_emb rows of n_embd floats).  The engine collects consecutive add_tokens / add_embedding calls of a chat turn (reference call sites
 // minigpt4.cpp:2365-2382 and :2399-2415 evaluate each piece separately; results are batch invariant) and evaluates them together, so the
 // weights stream once per kPrefillMax rows instead of once per piece.
-bool LlamaDevice::rows_mergeable() const {
-    return tok_type_ == GG_F32 || tok_type_ == GG_F16 || tok_type_ == GG_Q4_0 || tok_type_ == GG_Q4_1 || tok_type_ == GG_Q5_K || tok_type_ == GG_Q6_K;
-}
 bool LlamaDevice::eval_rows(const int32_t *ids, int n, const float *emb_host, int n_emb, int n_past) {
     if (n <= 0) return true;
     if (n_past + n > d_.n_ctx) { MG4_ERR("context overflow: %d + %d > n_ctx %d", n_past, n, d_.n_ctx); return false; }
@@ -485,7 +487,6 @@ bool LlamaDevice::eval_rows(const int32_t *ids, int n, const float *emb_host, in
     const int step = pf_ready_ ? kPrefillMax : 8;
     for (int i = 0; i < n; i += step) {
         const int c = std::min(step, n - i);
-        const bool last = i + c == n;
         CUDA_CHECK(cudaStreamSynchronize(stream_));  // h_state_ (pinned) of the previous pass / decode step has been consumed
         h_state_->n_past = n_past + i; h_state_->n_tok = c;
         for (int j = 0; j < std::min(c, 8); ++j) h_state_->tokens[j] = ids[i + j] >= 0 ? ids[i + j] : 0;
@@ -493,41 +494,9 @@ bool LlamaDevice::eval_rows(const int32_t *ids, int n, const float *emb_host, in
         CUDA_CHECK(cudaMemcpyAsync(tok_ids_, ids + i, (size_t)c * 4, cudaMemcpyHostToDevice, stream_));
         embed_rows_kernel<<<c, 256, 0, stream_>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, tok_ids_, embd_in_, x_);
         ++launches_;
-        if (pf_ready_ && c >= 2) prefill_chunk(c, last);
-        else launch_layers(nt_for(c), c, last);
+        record_pass(c, i + c == n);
     }
     CUDA_CHECK(cudaStreamSynchronize(stream_));
-    return true;
-}
-bool LlamaDevice::eval_tokens(const int32_t *ids, int n, int n_past) {
-    if (n <= 0) return true;
-    if (rows_mergeable()) return eval_rows(ids, n, nullptr, 0, n_past);
-    if (n_past + n > d_.n_ctx) { MG4_ERR("context overflow: %d + %d > n_ctx %d", n_past, n, d_.n_ctx); return false; }
-    for (int i = 0; i < n; ++i) if (ids[i] < 0 || ids[i] >= d_.n_vocab) { MG4_ERR("token id %d out of range", ids[i]); return false; }
-    for (int i = 0; i < n; i += 8) {   // token-embedding types outside dequant_elem (experimental block types): per-op path, 8 rows per pass
-        const int c = std::min(8, n - i);
-        h_state_->n_past = n_past + i; h_state_->n_tok = c;
-        for (int j = 0; j < c; ++j) h_state_->tokens[j] = ids[i + j];
-        run_chunk(c, i + c == n, true);
-    }
-    return true;
-}
-bool LlamaDevice::eval_embd(const float *rows_host, int n, int n_past) {
-    if (n <= 0) return true;
-    if (n > 512) { MG4_ERR("eval_embd: at most 512 rows per call"); return false; }
-    if (n_past + n > d_.n_ctx) { MG4_ERR("context overflow: %d + %d > n_ctx %d", n_past, n, d_.n_ctx); return false; }
-    if (rows_mergeable()) {
-        std::vector<int32_t> ids((size_t)n);
-        for (int i = 0; i < n; ++i) ids[(size_t)i] = -1 - i;
-        return eval_rows(ids.data(), n, rows_host, n, n_past);
-    }
-    CUDA_CHECK(cudaMemcpyAsync(embd_in_, rows_host, (size_t)n * d_.n_embd * 4, cudaMemcpyHostToDevice, stream_));
-    for (int i = 0; i < n; i += 8) {
-        const int c = std::min(8, n - i);
-        h_state_->n_past = n_past + i; h_state_->n_tok = c;
-        CUDA_CHECK(cudaMemcpyAsync(x_, embd_in_ + (size_t)i * d_.n_embd, (size_t)c * d_.n_embd * 4, cudaMemcpyDeviceToDevice, stream_));
-        run_chunk(c, i + c == n, false);
-    }
     return true;
 }
 void LlamaDevice::logits_to_host(float *dst) {
@@ -589,11 +558,11 @@ static void pq_build(PQMat &p, const QMat &m) {
 bool LlamaDevice::build_prefill() {
     if (getenv("MINIGPT4_B200_NO_PREFILL_GEMM")) return false;
     if (tp_ && tp_->world > 1) return false;  // (tensor-parallel ranks keep the per-op prefill path for now)
+    // (Q4 layers with Q4_K / Q5_0 / Q5_1 / Q8_0 token embeddings keep the per-op prefill path: no test covers them on the GEMM path)
     if (!(tok_type_ == GG_F32 || tok_type_ == GG_F16 || tok_type_ == GG_Q4_0 || tok_type_ == GG_Q4_1 || tok_type_ == GG_Q5_K || tok_type_ == GG_Q6_K)) return false;
-    for (auto &L : layers_) {
+    for (auto &L : layers_) {   // (each matrix stages its own input: mixed Q4_0 / Q4_1 layers are fine)
         if (!L.fused_qkv) return false;
         for (const QMat *m : {&L.qkv, &L.wo, &L.w13, &L.w2}) if (m->type != GG_Q4_0 && m->type != GG_Q4_1) return false;
-        if (act_of(L.qkv.type) != act_of(L.w13.type)) {}  // (each matrix stages its own input: mixed Q4_0 / Q4_1 layers are fine)
     }
     const int E = d_.n_embd, FF = d_.n_ff;
     size_t free_b = 0, total_b = 0; CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
@@ -613,24 +582,24 @@ bool LlamaDevice::build_prefill() {
     const size_t smem = 1024 + (size_t)pf::kStages * pf::kStageBytes + pf::kStackBytes + 256;
     CUDA_CHECK(cudaFuncSetAttribute(pf::prefill_gemm_q4<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_CHECK(cudaFuncSetAttribute(pf::prefill_gemm_q4<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_CHECK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(49152, d_.n_ctx * 6)));
     CUDA_CHECK(cudaDeviceSynchronize());
     MG4_INFO("tensor-core prefill: int8 class-major operand cache built (%d / %d slots per class)", pf_S_e_, pf_S_ff_);
     return true;
 }
 
-void LlamaDevice::pf_stage(const QMat &w, const float *x, int x_stride, const float *nw, int S, int n, cudaStream_t s) {
-    const int act = act_of(w.type);
+void LlamaDevice::pf_stage(const QMat &w, const float *x, int x_stride, const float *nw, int S, const Pass &ps) {
+    const int act = act_of(w.type), n = ps.rows;
     const size_t sm = act_bytes(act, w.cols);
-    if (act == ACT_Q8_1) pf::stage_rows_classmajor<ACT_Q8_1><<<n, 256, sm, s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
-    else pf::stage_rows_classmajor<ACT_Q8_0><<<n, 256, sm, s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
-    ++launches_;
+    if (act == ACT_Q8_1) pf::stage_rows_classmajor<ACT_Q8_1><<<n, 256, sm, ps.s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
+    else pf::stage_rows_classmajor<ACT_Q8_0><<<n, 256, sm, ps.s>>>(x, x_stride, nw, w.cols, S, pf_q8_, (float2 *)pf_sc_);
+    ++*ps.counter;
 }
-void LlamaDevice::pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, int n, const DeviceState *state, cudaStream_t s) {
+void LlamaDevice::pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, const Pass &ps) {
     const size_t smem = 1024 + (size_t)pf::kStages * pf::kStageBytes + pf::kStackBytes + 256;
+    const int n = ps.rows;
     const unsigned ty = (unsigned)((n + pf::kTok - 1) / pf::kTok);
     pf::PrefillArgs a = epi;
-    a.rows = p.rows; a.n_tok = n; a.nb = p.nb; a.S = p.S; a.wsc = (const __half2 *)p.sc; a.state = state; a.tab_silu = tab_silu_;
+    a.rows = p.rows; a.n_tok = n; a.nb = p.nb; a.S = p.S; a.wsc = (const __half2 *)p.sc; a.state = ps.state; a.tab_silu = tab_silu_;
     const CUtensorMap *tb = (const CUtensorMap *)(ff_wide ? pf_tmB_ff_ : pf_tmB_e_), *ts = (const CUtensorMap *)(ff_wide ? pf_tmS_ff_ : pf_tmS_e_);
     // K split over subtrees of the class butterfly so that matrices with few 128-row tiles (wo / down: 32) still fill the machine
     const int tiles = p.rows_pad / pf::kRows;
@@ -646,47 +615,12 @@ void LlamaDevice::pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &e
     }
     a.jr_per_z = 32 / nz; a.partial = (float2 *)pf_part_; a.part_tok = n; a.part_rows = p.rows_pad;
     const dim3 grid((unsigned)tiles, ty, (unsigned)nz);
-    if (p.q41) pf::prefill_gemm_q4<true><<<grid, pf::kThreads, smem, s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
-    else pf::prefill_gemm_q4<false><<<grid, pf::kThreads, smem, s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
-    ++launches_;
-    if (nz > 1) { const size_t work = (size_t)n * (p.rows / 2); pf::prefill_combine<<<(unsigned)((work + 255) / 256), 256, 0, s>>>(a, nz); ++launches_; }
+    if (p.q41) pf::prefill_gemm_q4<true><<<grid, pf::kThreads, smem, ps.s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
+    else pf::prefill_gemm_q4<false><<<grid, pf::kThreads, smem, ps.s>>>(*(const CUtensorMap *)p.tm, *tb, *ts, a);
+    ++*ps.counter;
+    if (nz > 1) { const size_t work = (size_t)n * (p.rows / 2); pf::prefill_combine<<<(unsigned)((work + 255) / 256), 256, 0, ps.s>>>(a, nz); ++*ps.counter; }
 }
 
-// one pass of all layers over n (<= kPrefillMax) rows in x_; positions from *state_ (n_past), KV rows appended, logits of the last row
-void LlamaDevice::prefill_chunk(int n, bool want_logits) {
-    const int E = d_.n_embd, El = n_embd_local_, FFl = n_ff_local_, C = d_.n_ctx;
-    const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
-    auto stage = [&](const QMat &w, const float *x, int x_stride, const float *nw, int S) { pf_stage(w, x, x_stride, nw, S, n, stream_); };
-    auto gemm = [&](const PQMat &p, bool ff_wide, const pf::PrefillArgs &a) { pf_gemm(p, ff_wide, a, n, state_, stream_); };
-    for (int il = 0; il < d_.n_layer; ++il) {
-        Layer &L = layers_[(size_t)il];
-        __half *kc = kcache_ + (size_t)il * C * El, *vc = vcache_ + (size_t)il * C * El;
-        stage(L.qkv, x_, E, L.attn_norm, pf_S_e_);
-        { pf::PrefillArgs a{}; a.epi = EPI_QKV; a.q_out = q_; a.kcache = kc; a.vcache = vc; a.rope = rope_; a.e_local = El; a.half_dim = 64; gemm(L.pqkv, false, a); }
-        attn_kernel<<<dim3((unsigned)n_head_local_, (unsigned)n), 256, (size_t)C * 6, stream_>>>(q_, kc, vc, att_, state_, El, C, kq_scale, tab_exp_); ++launches_;
-        stage(L.wo, att_, El, nullptr, pf_S_e_);
-        { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = x_; a.out_stride = E; a.resid = x_; gemm(L.pwo, false, a); }
-        stage(L.w13, x_, E, L.ffn_norm, pf_S_e_);
-        { pf::PrefillArgs a{}; a.epi = EPI_SWIGLU; a.out = act_; a.out_stride = FFl; gemm(L.pw13, false, a); }
-        stage(L.w2, act_, FFl, nullptr, pf_S_ff_);
-        { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = x_; a.out_stride = E; a.resid = x_; gemm(L.pw2, true, a); }
-    }
-    CUDA_CHECK(cudaGetLastError());
-    if (want_logits) {
-        MatvecArgs o{};
-        o.w = output_; o.x = x_ + (size_t)(n - 1) * E; o.x_stride = E; o.norm_w = final_norm_; o.ntok = 1; o.epi = EPI_LOGITS; o.out = logits_; o.n_valid = d_.n_vocab;
-        o.state = state_; o.tab_silu = tab_silu_; o.staged = qact_;
-        launch_matvec(o, 1, sm_count_, stream_, &launches_);
-    }
-    finalize_kernel<<<1, 32, 0, stream_>>>(state_, want_logits ? 1 : 0, nullptr); ++launches_;
-    CUDA_CHECK(cudaGetLastError());
-    if (want_logits) CUDA_CHECK(cudaMemcpyAsync(h_argmax_, &state_->argmax_id, 4, cudaMemcpyDeviceToHost, stream_));
-}
-
-// ------------------------------------------------------------------------------------------------
-// decode step as a CUDA graph: embed(tokens[0]) -> layers -> logits/arg-max -> finalize (n_past++, tokens[0] = arg-max)
-// positions and the token come from *state_, so the same graph serves every step
-// ------------------------------------------------------------------------------------------------
 // ------------------------------------------------------------------------------------------------
 // persistent megakernel program (llama_mega6.cuh)
 // ------------------------------------------------------------------------------------------------
@@ -707,20 +641,9 @@ bool LlamaDevice::build_mega() {
     dmalloc(&mega_barrier_, 64); CUDA_CHECK(cudaMemset(mega_barrier_, 0, 64));
     mega_n_ops_ = (tp ? 7 : 5) * d_.n_layer + 3;
     if (getenv("MINIGPT4_B200_MEGA_TRACE")) { dmalloc(&mega_trace_, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long)); CUDA_CHECK(cudaMemset(mega_trace_, 0, (size_t)(mega_n_ops_ + 1) * 32 * sizeof(long long))); }
-    mega_gen_ = 6;
-    if (!build_mega6()) return false;
-    const void *fn = mega_fn();
-    CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_));
-    int occ = 0;
-    CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, mk6::kThreads, mega_smem_));
-    if (occ < 1) { MG4_ERR("megakernel does not fit on an SM (smem %zu)", mega_smem_); return false; }
-    return true;
-}
 
-// generation 6: self-refilled per-warp streams (llama_mega6.cuh)
-bool LlamaDevice::build_mega6() {
+    // generation 6: self-refilled per-warp streams
     using namespace mk6;
-    const bool tp = tp_ && tp_->world > 1;
     const int E = d_.n_embd, FF = n_ff_local_;   // (tensor parallel: this rank's feed-forward columns)
     size_t act_b = mega_type_ == GG_Q5_K ? std::max(act_bytes(ACT_Q8_K, FF), act_bytes(ACT_Q8_K, E)) : std::max(act6_bytes(FF), act6_bytes(E));
     act_b = std::max(act_b, (size_t)d_.n_ctx * 6);  // the attention op (which stages no activations) uses the region as its scratch
@@ -730,7 +653,7 @@ bool LlamaDevice::build_mega6() {
     // a slot holds a row pair of an n_embd-wide matrix or ONE row of an n_ff-wide matrix (whose pair then takes both slots of the warp)
     int slot = std::max(2 * rb_e, rb_ff);
     slot = (slot + 15) & ~15;
-    cudaDeviceProp prop; int dev = 0; CUDA_CHECK(cudaGetDevice(&dev)); CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
+    cudaDeviceProp prop; CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
     const size_t stat = 10240;  // static shared memory of decode_megakernel6 (red, redf, qh, part) + slack
     const long long room = (long long)prop.sharedMemPerBlockOptin - (long long)stat - (long long)act_b - 2 * kConsumerWarps * 8;
     int W = (int)std::min<long long>(kConsumerWarps, room / (2LL * slot));
@@ -780,6 +703,11 @@ bool LlamaDevice::build_mega6() {
     mega_smem_ = (size_t)2 * W * slot + act_b + (size_t)2 * W * 8;
     MG4_INFO("decode megakernel (generation 6): %d ops/token, %d stream warps x 2 slots x %d B, act %zu B, %zu B dynamic shared per CTA, register-resident blocks per lane %d, grid %d",
              n, W, slot, act_b, mega_smem_, mega6_nbl_, sm_count_);
+    const void *fn = mega_fn();
+    CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mega_smem_));
+    int occ = 0;
+    CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, mk6::kThreads, mega_smem_));
+    if (occ < 1) { MG4_ERR("megakernel does not fit on an SM (smem %zu)", mega_smem_); return false; }
     return true;
 }
 
@@ -805,22 +733,19 @@ void LlamaDevice::launch_mega() {
     CUDA_CHECK(cudaMemcpyAsync(h_argmax_, &state_->argmax_id, 4, cudaMemcpyDeviceToHost, stream_));
 }
 
+// the decode step as a CUDA graph: the megakernel, or embed(tokens[0]) -> layers -> logits/arg-max -> finalize (n_past++, tokens[0] =
+// arg-max).  Positions and the token come from *state_, so the same graph serves every step.
 void LlamaDevice::build_graph() {
     cudaGraph_t g = nullptr;
     const unsigned long long before = launches_;
     mega_ = build_mega();
     CUDA_CHECK(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
     if (mega_) launch_mega();
-    else {
-        if (tok_type_ == GG_Q4_K) embed_q4k_kernel<<<1, 256, 0, stream_>>>((const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        else if (tok_type_ == GG_Q5_0 || tok_type_ == GG_Q5_1 || tok_type_ == GG_Q8_0) embed_b32_kernel<<<1, 256, 0, stream_>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        else embed_kernel<<<1, 256, 0, stream_>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)d_.n_embd), d_.n_embd, state_, x_);
-        launch_layers(1, 1, true);
-    }
+    else { launch_embed(1, state_, x_, stream_, &launches_); record_pass(1, true); }
     CUDA_CHECK(cudaStreamEndCapture(stream_, &g));
     CUDA_CHECK(cudaGraphInstantiate(&graph_, g, 0));
     CUDA_CHECK(cudaGraphDestroy(g));
-    graph_kernels_ = (int)(launches_ - before) + (mega_ ? 0 : 1);
+    graph_kernels_ = (int)(launches_ - before);
     launches_ = before;
 }
 bool LlamaDevice::decode_step(int32_t id, int n_past) {
@@ -855,80 +780,49 @@ float LlamaDevice::decode_chain(int steps, int n_past, int32_t *ids_out) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// batched decode step over B contexts of one group (llama_sessions.cuh): prepare (tokens) -> embed B rows -> layers (QKV and attention
-// per column through the slot table; wo / gate-up / down through matvec_kernel at ntok = B) -> logits of every column into its own
-// context -> finalize every context's DeviceState -> the B ids to pinned memory.  Captured once per B on the group stream.
+// the group workspace of the batched passes (llama_sessions.cuh), built by the group's first decode_batch or batched flush: kPrefillMax
+// rows of activations, a row table for the prompt pass and a context table for the decode step and the contexts that end in a prompt
+// pass.  Both users run synchronously on the group stream, so they share it; the batch graphs capture its pointers.
 // ------------------------------------------------------------------------------------------------
-static void attn_sessions_smem(int n_ctx) {   // attention scratch = n_ctx * 6 bytes; the attribute only grows (groups of one process may differ in n_ctx)
-    static int attn_smem[64] = {};
-    int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
-    const int need = std::max(49152, n_ctx * 6);
-    if (need > attn_smem[dev & 63]) { CUDA_CHECK(cudaFuncSetAttribute(attn_sessions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, need)); attn_smem[dev & 63] = need; }
+void LlamaDevice::build_group_workspace() {
+    LlamaGroup &G = *group_;
+    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_;
+    const size_t R = (size_t)kPrefillMax, b0 = t_dev_bytes;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
+    dmalloc(&G.x, R * E * 4);
+    dmalloc(&G.q, R * El * 4);
+    dmalloc(&G.att, R * El * 4);
+    dmalloc(&G.act, R * std::max(FFl, 3 * El) * 4);
+    dmalloc(&G.last, (size_t)8 * E * 4);
+    dmalloc(&G.qact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
+    dmalloc(&G.state, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.state, 0, sizeof(DeviceState)));
+    dmalloc(&G.rows, R * sizeof(SessionSlot));
+    dmalloc(&G.slots, 8 * sizeof(SessionSlot));
+    dmalloc(&G.ids, 8 * sizeof(int));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_rows, R * sizeof(SessionSlot), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, 8 * sizeof(int), cudaHostAllocDefault));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    G.batch_bytes += t_dev_bytes - b0;
 }
+
+// ------------------------------------------------------------------------------------------------
+// batched decode step over B contexts of one group: prepare (tokens) -> embed B rows -> layers (QKV and attention per column through the
+// context table; wo / gate-up / down through matvec_kernel at ntok = B) -> logits of every column into its own context -> finalize every
+// context's DeviceState -> the B ids to pinned memory.  Captured once per B on the group stream.
+// ------------------------------------------------------------------------------------------------
 void LlamaDevice::build_batch_graph(int B) {
     LlamaGroup &G = *group_;
-    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_, C = d_.n_ctx, nt = nt_for(B);
-    if (!G.x) {
-        const size_t b0 = t_dev_bytes;
-        if (!G.stream) CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
-        dmalloc(&G.x, (size_t)8 * E * 4);
-        dmalloc(&G.q, (size_t)8 * El * 4);
-        dmalloc(&G.att, (size_t)8 * El * 4);
-        dmalloc(&G.act, (size_t)8 * FFl * 4);
-        dmalloc(&G.qact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
-        dmalloc(&G.state, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.state, 0, sizeof(DeviceState)));
-        dmalloc(&G.slots, 8 * sizeof(SessionSlot));
-        dmalloc(&G.ids, 8 * sizeof(int));
-        CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
-        CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, 8 * sizeof(int), cudaHostAllocDefault));
-        CUDA_CHECK(cudaDeviceSynchronize());
-        G.batch_bytes += t_dev_bytes - b0;
-    }
-    attn_sessions_smem(C);
-    const float kq_scale = 1.0f / sqrtf((float)d_.n_embd / (float)d_.n_head);
     cudaStream_t s = G.stream;
     unsigned long long n = 0;
     cudaGraph_t g = nullptr;
     CUDA_CHECK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
     prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.state); ++n;
-    const size_t trb = gg_row_bytes(tok_type_, (size_t)E);
-    if (tok_type_ == GG_Q4_K) embed_q4k_kernel<<<B, 256, 0, s>>>((const unsigned char *)tok_raw_, trb, E, G.state, G.x);
-    else if (tok_type_ == GG_Q5_0 || tok_type_ == GG_Q5_1 || tok_type_ == GG_Q8_0) embed_b32_kernel<<<B, 256, 0, s>>>(tok_type_, (const unsigned char *)tok_raw_, trb, E, G.state, G.x);
-    else embed_kernel<<<B, 256, 0, s>>>(tok_type_, (const unsigned char *)tok_raw_, trb, E, G.state, G.x);
-    ++n;
-    for (int il = 0; il < d_.n_layer; ++il) {
-        Layer &L = layers_[(size_t)il];
-        const size_t kv_off = (size_t)il * C * El;
-        MatvecArgs a{};
-        a.x = G.x; a.x_stride = E; a.norm_w = L.attn_norm; a.ntok = B; a.epi = EPI_QKV; a.staged = G.qact;
-        a.q_out = G.q; a.rope = rope_; a.e_local = El; a.half_dim = 64; a.state = G.state; a.tab_silu = tab_silu_;
-        if (L.fused_qkv) { a.w = L.qkv; a.part = -1; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.slots, kv_off, nt, sm_count_, s, &n); }
-        else {
-            const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
-            for (int part = 0; part < 3; ++part) {
-                const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
-                a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.slots, kv_off, nt, sm_count_, s, &n, !same);
-            }
-        }
-        attn_sessions_kernel<<<dim3((unsigned)n_head_local_, (unsigned)B), 256, (size_t)C * 6, s>>>(G.q, G.slots, kv_off, G.att, El, C, kq_scale, tab_exp_);
-        CUDA_CHECK(cudaGetLastError()); ++n;
-        MatvecArgs b{};
-        b.w = L.wo; b.x = G.att; b.x_stride = El; b.ntok = B; b.n_valid = b.w.rows; b.state = G.state; b.tab_silu = tab_silu_; b.staged = G.qact;
-        b.epi = EPI_RESID; b.out = G.x; b.out_stride = E; b.resid = G.x;
-        launch_matvec(b, nt, sm_count_, s, &n);
-        MatvecArgs c{};
-        c.w = L.w13; c.x = G.x; c.x_stride = E; c.norm_w = L.ffn_norm; c.ntok = B; c.epi = EPI_SWIGLU; c.out = G.act; c.out_stride = FFl; c.n_valid = c.w.rows;
-        c.state = G.state; c.tab_silu = tab_silu_; c.staged = G.qact;
-        launch_matvec(c, nt, sm_count_, s, &n);
-        MatvecArgs e{};
-        e.w = L.w2; e.x = G.act; e.x_stride = FFl; e.ntok = B; e.n_valid = e.w.rows; e.state = G.state; e.tab_silu = tab_silu_; e.staged = G.qact;
-        e.epi = EPI_RESID; e.out = G.x; e.out_stride = E; e.resid = G.x;
-        launch_matvec(e, nt, sm_count_, s, &n);
-    }
-    MatvecArgs o{};
-    o.w = output_; o.x = G.x; o.x_stride = E; o.norm_w = final_norm_; o.ntok = B; o.epi = EPI_LOGITS; o.n_valid = d_.n_vocab;
-    o.state = G.state; o.tab_silu = tab_silu_; o.staged = G.qact;
-    launch_matvec_sessions(o, G.slots, 0, nt, sm_count_, s, &n);
+    launch_embed(B, G.state, G.x, s, &n);
+    record_layers(Pass{B, G.x, G.q, G.att, G.act, G.qact, G.state, G.slots, false, s, &n});
+    MatvecArgs o = mv_args(output_, B, G.state, G.qact, tab_silu_);
+    o.x = G.x; o.x_stride = d_.n_embd; o.norm_w = final_norm_; o.epi = EPI_LOGITS; o.n_valid = d_.n_vocab;
+    launch_matvec(o, sm_count_, s, &n, G.slots, 0);
     finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.ids); ++n;
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaMemcpyAsync(G.h_ids, G.ids, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
@@ -944,6 +838,7 @@ void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids,
     // a context's own decode step may still be running on its stream (decode_step returns before it finishes): it has to be done
     // before the group stream reads and writes that context's cache, logits and state
     for (int i = 0; i < n; ++i) c[i]->sync();
+    if (!G.x) L0.build_group_workspace();
     if (!G.graph[n]) L0.build_batch_graph(n);
     for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], ids[i], c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
     CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, G.stream));
@@ -954,43 +849,17 @@ void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids,
 }
 
 // ------------------------------------------------------------------------------------------------
-// batched prompt pass over the queued rows of several contexts of one group (llama_sessions.cuh).  Each pass takes the next <=
-// kPrefillMax rows of the contexts in order; row t carries its own position and its context's caches in a row slot (rslots).  Per layer:
-// qkv with RoPE and KV append at each row's position into its context's cache (tensor-core GEMM + qkv_rows_kernel, or per-op
-// matvec_sessions_kernel over 8-row chunks), attn_sessions_kernel over all rows, then wo / gate-up / down exactly as a single context's
-// pass.  Contexts whose last row is in the pass get their logits, arg-max and DeviceState through the context slots (cslots), as the
-// batched decode step does.  Every row is quantised and reduced on its own, so each context gets the bits of its own eval_rows.
+// batched prompt pass over the queued rows of several contexts of one group.  Each pass takes the next <= kPrefillMax rows of the
+// contexts in order; row t carries its own position and its context's caches in the row table, and record_layers runs the pass with it.
+// Contexts whose last row is in the pass get their logits, arg-max and DeviceState through the context table, as the batched decode
+// step does.  Every row is quantised and reduced on its own, so each context gets the bits of its own eval_rows.
 // ------------------------------------------------------------------------------------------------
-void LlamaDevice::build_prompt_workspace() {
-    LlamaGroup &G = *group_;
-    const int E = d_.n_embd, El = n_embd_local_, FF = d_.n_ff, FFl = n_ff_local_;
-    const size_t R = (size_t)kPrefillMax, b0 = t_dev_bytes;
-    if (!G.stream) CUDA_CHECK(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
-    dmalloc(&G.px, R * E * 4);
-    dmalloc(&G.pq, R * El * 4);
-    dmalloc(&G.patt, R * El * 4);
-    dmalloc(&G.pact, R * std::max(FFl, 3 * El) * 4);
-    dmalloc(&G.plast, (size_t)8 * E * 4);
-    dmalloc(&G.pqact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
-    dmalloc(&G.pstate, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.pstate, 0, sizeof(DeviceState)));
-    dmalloc(&G.rslots, R * sizeof(SessionSlot));
-    dmalloc(&G.cslots, 8 * sizeof(SessionSlot));
-    dmalloc(&G.pids, 8 * sizeof(int));
-    CUDA_CHECK(cudaHostAlloc((void **)&G.h_rslots, R * sizeof(SessionSlot), cudaHostAllocDefault));
-    CUDA_CHECK(cudaHostAlloc((void **)&G.h_cslots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
-    CUDA_CHECK(cudaHostAlloc((void **)&G.h_pids, 8 * sizeof(int), cudaHostAllocDefault));
-    CUDA_CHECK(cudaDeviceSynchronize());
-    G.batch_bytes += t_dev_bytes - b0;
-    attn_sessions_smem(d_.n_ctx);
-}
-
 void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past) {
     LlamaDevice &L0 = *c[0];
     LlamaGroup &G = *L0.group_;
     for (int i = 0; i < n; ++i) c[i]->sync();   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
-    if (!G.px) L0.build_prompt_workspace();
-    const int E = L0.d_.n_embd, El = L0.n_embd_local_, FFl = L0.n_ff_local_, C = L0.d_.n_ctx, S = kPrefillMax;
-    const float kq_scale = 1.0f / sqrtf((float)L0.d_.n_embd / (float)L0.d_.n_head);
+    if (!G.x) L0.build_group_workspace();
+    const int E = L0.d_.n_embd, S = kPrefillMax;
     cudaStream_t s = G.stream;
     std::vector<int32_t> pid((size_t)S);
     int ci = 0, cj = 0;   // next row: row cj of context ci
@@ -1005,7 +874,7 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
             int k0 = -1, k1 = -1;
             for (int j = 0; j < take; ++j) {
                 const int id = ids[ci][cj + j], r = rows + j;
-                G.h_rslots[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+                G.h_rows[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
                 if (id >= 0) pid[(size_t)r] = id;
                 else {
                     const int k = -1 - id;
@@ -1020,91 +889,34 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
             }
             rows += take; cj += take;
             if (cj < n_rows[ci]) break;   // the context continues in the next pass
-            G.h_cslots[nf] = SessionSlot{n_past[ci] + n_rows[ci] - 1, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+            G.h_slots[nf] = SessionSlot{n_past[ci] + n_rows[ci] - 1, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
             last.r[nf] = rows - 1; fin_ctx[nf] = ci; fin_first[nf] = rows - take;
             ++nf;
         }
-        CUDA_CHECK(cudaMemcpyAsync(G.rslots, G.h_rslots, (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(G.rows, G.h_rows, (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(L0.tok_ids_, pid.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s));
-        if (nf) CUDA_CHECK(cudaMemcpyAsync(G.cslots, G.h_cslots, (size_t)nf * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
-        embed_rows_kernel<<<rows, 256, 0, s>>>(L0.tok_type_, (const unsigned char *)L0.tok_raw_, gg_row_bytes(L0.tok_type_, (size_t)E), E, L0.tok_ids_, L0.embd_in_, G.px);
+        if (nf) CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)nf * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+        embed_rows_kernel<<<rows, 256, 0, s>>>(L0.tok_type_, (const unsigned char *)L0.tok_raw_, gg_row_bytes(L0.tok_type_, (size_t)E), E, L0.tok_ids_, L0.embd_in_, G.x);
         ++L0.launches_;
-
-        // ---- the layers
-        const bool gemm = L0.pf_ready_ && rows >= 2;
-        for (int il = 0; il < L0.d_.n_layer; ++il) {
-            Layer &L = L0.layers_[(size_t)il];
-            const size_t kv_off = (size_t)il * C * El;
-            if (gemm) {
-                L0.pf_stage(L.qkv, G.px, E, L.attn_norm, L0.pf_S_e_, rows, s);
-                { pf::PrefillArgs a{}; a.epi = EPI_PLAIN; a.out = G.pact; a.out_stride = 3 * El; L0.pf_gemm(L.pqkv, false, a, rows, G.pstate, s); }
-                qkv_rows_kernel<<<dim3((unsigned)((3 * El / 2 + 255) / 256), (unsigned)rows), 256, 0, s>>>(G.pact, G.rslots, kv_off, G.pq, L0.rope_, El, 64);
-                ++L0.launches_;
-            } else {
-                for (int t0 = 0; t0 < rows; t0 += 8) {
-                    const int m = std::min(8, rows - t0);
-                    MatvecArgs a{};
-                    a.x = G.px + (size_t)t0 * E; a.x_stride = E; a.norm_w = L.attn_norm; a.ntok = m; a.epi = EPI_QKV; a.staged = G.pqact;
-                    a.q_out = G.pq + (size_t)t0 * El; a.rope = L0.rope_; a.e_local = El; a.half_dim = 64; a.state = G.pstate; a.tab_silu = L0.tab_silu_;
-                    if (L.fused_qkv) { a.w = L.qkv; a.part = -1; a.n_valid = a.w.rows; launch_matvec_sessions(a, G.rslots + t0, kv_off, nt_for(m), L0.sm_count_, s, &L0.launches_); }
-                    else {
-                        const QMat *ms[3] = {&L.wq, &L.wk, &L.wv};
-                        for (int part = 0; part < 3; ++part) {
-                            const bool same = part > 0 && act_of(ms[part]->type) == act_of(ms[part - 1]->type);
-                            a.w = *ms[part]; a.part = part; a.n_valid = a.w.rows;
-                            launch_matvec_sessions(a, G.rslots + t0, kv_off, nt_for(m), L0.sm_count_, s, &L0.launches_, !same);
-                        }
-                    }
-                }
-            }
-            attn_sessions_kernel<<<dim3((unsigned)L0.n_head_local_, (unsigned)rows), 256, (size_t)C * 6, s>>>(G.pq, G.rslots, kv_off, G.patt, El, C, kq_scale, L0.tab_exp_);
-            CUDA_CHECK(cudaGetLastError()); ++L0.launches_;
-            if (gemm) {
-                L0.pf_stage(L.wo, G.patt, El, nullptr, L0.pf_S_e_, rows, s);
-                { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = G.px; a.out_stride = E; a.resid = G.px; L0.pf_gemm(L.pwo, false, a, rows, G.pstate, s); }
-                L0.pf_stage(L.w13, G.px, E, L.ffn_norm, L0.pf_S_e_, rows, s);
-                { pf::PrefillArgs a{}; a.epi = EPI_SWIGLU; a.out = G.pact; a.out_stride = FFl; L0.pf_gemm(L.pw13, false, a, rows, G.pstate, s); }
-                L0.pf_stage(L.w2, G.pact, FFl, nullptr, L0.pf_S_ff_, rows, s);
-                { pf::PrefillArgs a{}; a.epi = EPI_RESID; a.out = G.px; a.out_stride = E; a.resid = G.px; L0.pf_gemm(L.pw2, true, a, rows, G.pstate, s); }
-            } else {
-                for (int t0 = 0; t0 < rows; t0 += 8) {
-                    const int m = std::min(8, rows - t0), nt = nt_for(m);
-                    float *x = G.px + (size_t)t0 * E, *act = G.pact + (size_t)t0 * FFl;
-                    MatvecArgs b{};
-                    b.w = L.wo; b.x = G.patt + (size_t)t0 * El; b.x_stride = El; b.ntok = m; b.n_valid = b.w.rows; b.state = G.pstate; b.tab_silu = L0.tab_silu_;
-                    b.staged = G.pqact; b.epi = EPI_RESID; b.out = x; b.out_stride = E; b.resid = x;
-                    launch_matvec(b, nt, L0.sm_count_, s, &L0.launches_);
-                    MatvecArgs g{};
-                    g.w = L.w13; g.x = x; g.x_stride = E; g.norm_w = L.ffn_norm; g.ntok = m; g.epi = EPI_SWIGLU; g.out = act; g.out_stride = FFl; g.n_valid = g.w.rows;
-                    g.state = G.pstate; g.tab_silu = L0.tab_silu_; g.staged = G.pqact;
-                    launch_matvec(g, nt, L0.sm_count_, s, &L0.launches_);
-                    MatvecArgs e{};
-                    e.w = L.w2; e.x = act; e.x_stride = FFl; e.ntok = m; e.n_valid = e.w.rows; e.state = G.pstate; e.tab_silu = L0.tab_silu_; e.staged = G.pqact;
-                    e.epi = EPI_RESID; e.out = x; e.out_stride = E; e.resid = x;
-                    launch_matvec(e, nt, L0.sm_count_, s, &L0.launches_);
-                }
-            }
-        }
-        CUDA_CHECK(cudaGetLastError());
+        L0.record_layers(Pass{rows, G.x, G.q, G.att, G.act, G.qact, G.state, G.rows, L0.pf_ready_ && rows >= 2, s, &L0.launches_});
 
         // ---- contexts that end in this pass: logits + arg-max of their last row, DeviceState, hidden rows, pinned arg-max
         if (nf) {
-            gather_rows_kernel<<<nf, 256, 0, s>>>(G.px, last, E, G.plast);
-            prepare_sessions_kernel<<<1, 32, 0, s>>>(G.cslots, nf, G.pstate);
-            MatvecArgs o{};
-            o.w = L0.output_; o.x = G.plast; o.x_stride = E; o.norm_w = L0.final_norm_; o.ntok = nf; o.epi = EPI_LOGITS; o.n_valid = L0.d_.n_vocab;
-            o.state = G.pstate; o.tab_silu = L0.tab_silu_; o.staged = G.pqact;
-            launch_matvec_sessions(o, G.cslots, 0, nt_for(nf), L0.sm_count_, s, &L0.launches_);
-            finalize_sessions_kernel<<<1, 32, 0, s>>>(G.cslots, nf, G.pids);
+            gather_rows_kernel<<<nf, 256, 0, s>>>(G.x, last, E, G.last);
+            prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, nf, G.state);
+            MatvecArgs o = mv_args(L0.output_, nf, G.state, G.qact, L0.tab_silu_);
+            o.x = G.last; o.x_stride = E; o.norm_w = L0.final_norm_; o.epi = EPI_LOGITS; o.n_valid = L0.d_.n_vocab;
+            launch_matvec(o, L0.sm_count_, s, &L0.launches_, G.slots, 0);
+            finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots, nf, G.ids);
             CUDA_CHECK(cudaGetLastError()); L0.launches_ += 3;
-            CUDA_CHECK(cudaMemcpyAsync(G.h_pids, G.pids, (size_t)nf * 4, cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaMemcpyAsync(G.h_ids, G.ids, (size_t)nf * 4, cudaMemcpyDeviceToHost, s));
             for (int f = 0; f < nf; ++f) {
                 const int k = last.r[f] + 1 - fin_first[f];
-                CUDA_CHECK(cudaMemcpyAsync(c[fin_ctx[f]]->x_, G.px + (size_t)fin_first[f] * E, (size_t)k * E * 4, cudaMemcpyDeviceToDevice, s));
+                CUDA_CHECK(cudaMemcpyAsync(c[fin_ctx[f]]->x_, G.x + (size_t)fin_first[f] * E, (size_t)k * E * 4, cudaMemcpyDeviceToDevice, s));
             }
         }
-        CUDA_CHECK(cudaStreamSynchronize(s));   // (the pinned tables and the shared prompt scratch are reused by the next pass)
-        for (int f = 0; f < nf; ++f) *c[fin_ctx[f]]->h_argmax_ = G.h_pids[f];
+        CUDA_CHECK(cudaStreamSynchronize(s));   // (the pinned tables and the shared workspace are reused by the next pass)
+        for (int f = 0; f < nf; ++f) *c[fin_ctx[f]]->h_argmax_ = G.h_ids[f];
     }
 }
 
@@ -1155,7 +967,7 @@ float LlamaDevice::time_matvec(int kind, int reps, double *bytes_per_launch) {
         }
         if (kind != 4) a.n_valid = a.w.rows;
         bytes = (double)a.w.bytes;
-        launch_matvec(a, 1, sm_count_, stream_, &launches_);
+        launch_matvec(a, sm_count_, stream_, &launches_);
     };
     for (int il = 0; il < d_.n_layer; ++il) one(il);  // warm-up pass (instruction cache, smem attributes)
     CUDA_CHECK(cudaStreamSynchronize(stream_));
@@ -1201,7 +1013,7 @@ void LlamaDevice::test_matvec(int gg, int rows, int cols, const void *w_host, co
         const int c = std::min(8, n - i);
         MatvecArgs a{};
         a.w = m; a.x = x + (size_t)i * cols; a.x_stride = cols; a.ntok = c; a.epi = EPI_PLAIN; a.out = y + (size_t)i * m.rows; a.out_stride = m.rows; a.n_valid = rows; a.state = stt; a.staged = stg;
-        launch_matvec(a, nt_for(c), prop.multiProcessorCount, 0, nullptr);
+        launch_matvec(a, prop.multiProcessorCount, 0, nullptr);
     }
     CUDA_CHECK(cudaDeviceSynchronize());
     std::vector<float> tmp((size_t)n * m.rows);

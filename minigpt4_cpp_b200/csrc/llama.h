@@ -17,6 +17,7 @@ namespace mg4 {
 
 struct TPLink;  // tensor-parallel communicator (tp.h)
 namespace pf { struct PrefillArgs; }   // llama_prefill.cuh
+namespace k { struct MatvecArgs; }    // llama_kernels.cuh
 
 struct QMat {          // one repacked weight matrix (or a fused group of matrices of one type)
     int type = -1;     // GGType
@@ -77,12 +78,9 @@ public:
     // last row.  Synchronous.  The caller validates (distinct, one group, rows checked when they were queued).
     static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past);
     const LlamaDims &dims() const { return d_; }
-    // Evaluate `n` tokens / embedding rows starting at position n_past. Afterwards logits of the last row are
-    // on device and the arg-max id is known.  Returns false if the context would overflow.
-    bool eval_tokens(const int32_t *ids, int n, int n_past);
-    bool eval_embd(const float *rows_host, int n, int n_past);
-    bool eval_rows(const int32_t *ids, int n, const float *emb_host, int n_emb, int n_past);  // mixed token / embedding rows (ids < 0: row -1 - id of emb_host)
-    bool rows_mergeable() const;     // eval_rows supports this file's token-embedding type
+    // Evaluate `n` mixed token / embedding rows (ids < 0: row -1 - id of emb_host) starting at position n_past.  Afterwards logits of the
+    // last row are on device and the arg-max id is known.  Returns false if the context would overflow.
+    bool eval_rows(const int32_t *ids, int n, const float *emb_host, int n_emb, int n_past);
     void logits_to_host(float *dst);   // n_vocab floats, synchronous
     int32_t argmax();                  // greedy id of the current logits (already in pinned host memory after a sync)
     void sync();
@@ -91,7 +89,7 @@ public:
     bool uses_megakernel() const { return mega_; }
     bool uses_prefill_gemm() const { return pf_ready_; }
     static constexpr int kPrefillMax = 512;   // rows per prefill pass (the reference's default n_batch)
-    int mega_generation() const { return mega_ ? mega_gen_ : 0; }
+    int mega_generation() const { return mega_ ? 6 : 0; }
     int mega_trace(long long *out, int max_values);  // debug: per-op clock64 stamps of the last megakernel launch (env MINIGPT4_B200_MEGA_TRACE)
     // one decode step through the captured CUDA graph: feeds `id` (or, if id < 0, the on-device arg-max of the
     // previous step), leaves new logits/arg-max on device.
@@ -115,20 +113,29 @@ public:
 
 private:
     struct Layer { QMat qkv, wq, wk, wv, wo, w13, w2; bool fused_qkv; float *attn_norm, *ffn_norm; PQMat pqkv, pwo, pw13, pw2; };
+    struct Pass {                    // one pass of all layers over `rows` rows that sit in x (record_layers)
+        int rows;
+        float *x, *q, *att, *act;    // [rows] activations (act also takes the qkv GEMM's [rows][3 n_embd] output when slots is set)
+        unsigned char *qact;         // staged matvec inputs of <= 8 rows
+        DeviceState *state;          // what MatvecArgs / PrefillArgs read
+        const SessionSlot *slots;    // [rows] each row's position and caches; null: positions state->n_past + t in this context's caches
+        bool gemm;                   // tensor-core GEMMs (pf_ready_, rows >= 2); otherwise matvecs over <= 8-row chunks
+        cudaStream_t s;
+        unsigned long long *counter; // kernel launches
+    };
+    void record_layers(const Pass &p);
+    void add_matvec(k::MatvecArgs a, float *x, const Pass &p);   // wo / down into the residual rows x (+ the tensor-parallel reduce)
+    void record_pass(int n, bool want_logits);   // this context's pass over n rows in x_: layers, logits, finalize
+    void launch_embed(int n, const DeviceState *st, float *x, cudaStream_t s, unsigned long long *counter) const;
     bool build_prefill();            // tensor-core prefill (llama_prefill.cuh): homogeneous Q4_0 / Q4_1 layers, single GPU
-    void prefill_chunk(int n, bool want_logits);   // n <= kPrefillMax rows that sit in x_
-    // one matrix of a prefill pass over n rows on stream s: stage the input rows into the shared operand scratch, then the GEMM
-    // (state: the n_past that EPI_QKV reads)
-    void pf_stage(const QMat &w, const float *x, int x_stride, const float *norm_w, int S, int n, cudaStream_t s);
-    void pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, int n, const DeviceState *state, cudaStream_t s);
+    // one matrix of a prefill pass: stage the input rows into the shared operand scratch, then the GEMM
+    void pf_stage(const QMat &w, const float *x, int x_stride, const float *norm_w, int S, const Pass &ps);
+    void pf_gemm(const PQMat &p, bool ff_wide, const pf::PrefillArgs &epi, const Pass &ps);
     bool pf_ready_ = false; int pf_S_e_ = 0, pf_S_ff_ = 0;
     signed char *pf_q8_ = nullptr; void *pf_sc_ = nullptr; int32_t *tok_ids_ = nullptr; void *pf_part_ = nullptr; size_t pf_part_bytes_ = 0;
     alignas(64) unsigned char pf_tmB_e_[128], pf_tmS_e_[128], pf_tmB_ff_[128], pf_tmS_ff_[128];
-    void run_chunk(int n, bool want_logits, bool from_tokens);
-    void launch_layers(int nt, int ntok, bool want_logits);
     void build_graph();
-    bool build_mega();               // persistent one-launch-per-token decode (homogeneous Q4_0/Q4_1, single GPU)
-    bool build_mega6();
+    bool build_mega();               // persistent one-launch-per-token decode, generation 6 (llama_mega6.cuh): homogeneous Q4_0 / Q4_1 / Q5_K
     void launch_mega();
     const void *mega_fn() const;
     LlamaDims d_{};
@@ -154,7 +161,7 @@ private:
     unsigned long long launches_ = 0;
     int graph_kernels_ = 0;
     long long *mega_trace_ = nullptr; int mega_n_ops_ = 0;
-    int mega_gen_ = 6; void *mega6_params_ = nullptr; int mega6_nbl_ = 0;  // generation 6 (llama_mega6.cuh)
+    void *mega6_params_ = nullptr; int mega6_nbl_ = 0;
     bool h_state_busy_ = false;
     bool mega_ = false; unsigned *mega_barrier_ = nullptr; size_t mega_smem_ = 0; int mega_type_ = -1;
     int sm_count_ = 132;
@@ -163,8 +170,8 @@ private:
     size_t owned_bytes_ = 0;
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group
+    void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)
     void build_batch_graph(int B);   // decode_batch's graph for B columns, captured on the group stream
-    void build_prompt_workspace();   // eval_rows_batch's rows, slot tables and stream (group-owned, at the first batched flush)
 };
 
 }  // namespace mg4

@@ -776,46 +776,56 @@ __global__ void embed_ids_kernel(int type, const unsigned char *tok, size_t row_
     const unsigned char *row = tok + (size_t)ids[t] * row_bytes;
     for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = dequant_elem(type, row, i);
 }
+// Q4_K and Q5_0 / Q5_1 / Q8_0 token-embedding elements (ggml dequantize_row_q4_K / q5_0 / q5_1 / q8_0), raw ggml blocks: kept out of
+// dequant_elem so that the kernels which inline it (embed_kernel, the decode megakernel) stay byte-identical to the measured build
+__device__ __forceinline__ float dequant_q4k_elem(const unsigned char *row, int i) {
+    const unsigned char *b = row + (i / 256) * 144; const int e = i % 256, sub = e / 32, l = e % 32;
+    const float d = __half2float(*(const __half *)b), dmin = __half2float(*(const __half *)(b + 2));
+    int sc, mn; scale_min_k4(b + 4, sub, sc, mn);
+    const unsigned char qb = b[16 + (sub / 2) * 32 + l]; const int nib = (sub & 1) ? (qb >> 4) : (qb & 0xF);
+    return (d * (float)sc) * (float)nib - dmin * (float)mn;
+}
+// element i of a Q5_0 / Q5_1 / Q8_0 row into a new float v.  A macro, not a __device__ function: inlined as a function it changes
+// embed_b32_kernel's address arithmetic, and that kernel stays byte-identical to the measured build.
+#define MG4_DEQUANT_B32_ELEM(v, type, row, i) \
+    const int j = (i) % 32, jj = j & 15; \
+    float v; \
+    if ((type) == GG_Q8_0) { const unsigned char *b = (row) + ((i) / 32) * 34; v = (float)(int)(signed char)b[2 + j] * __half2float(*(const __half *)b); } \
+    else { \
+        const int hdr = (type) == GG_Q5_1 ? 4 : 2; \
+        const unsigned char *b = (row) + ((i) / 32) * (hdr + 20); \
+        const unsigned qh = b[hdr] | (b[hdr + 1] << 8) | (b[hdr + 2] << 16) | ((unsigned)b[hdr + 3] << 24); \
+        const int q = (j < 16 ? (b[hdr + 4 + jj] & 0xF) : (b[hdr + 4 + jj] >> 4)) | (int)(((qh >> j) & 1u) << 4); \
+        const float d = __half2float(*(const __half *)b); \
+        v = (type) == GG_Q5_1 ? (float)q * d + __half2float(*(const __half *)(b + 2)) : (float)(q - 16) * d; \
+    }
 // mixed rows of one prefill pass: ids[t] >= 0 = token (gather + dequantise), ids[t] < 0 = embedding row -1 - ids[t] of `emb` (the 32 image rows)
 __global__ void embed_rows_kernel(int type, const unsigned char *tok, size_t row_bytes, int E, const int *ids, const float *emb, float *x) {
     const int t = blockIdx.x, id = ids[t];
     if (id >= 0) {
         const unsigned char *row = tok + (size_t)id * row_bytes;
-        for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = dequant_elem(type, row, i);
+        if (type == GG_Q4_K) for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = dequant_q4k_elem(row, i);
+        else if (type == GG_Q5_0 || type == GG_Q5_1 || type == GG_Q8_0) for (int i = threadIdx.x; i < E; i += blockDim.x) {
+            MG4_DEQUANT_B32_ELEM(v, type, row, i)
+            x[(size_t)t * E + i] = v;
+        }
+        else for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = dequant_elem(type, row, i);
     } else {
         const float *src = emb + (size_t)(-1 - id) * E;
         for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = src[i];
     }
 }
-// Q4_K token-embedding rows: kept out of dequant_elem so that the kernels which inline it
-// (embed_kernel, the decode megakernel) stay byte-identical to the measured build
+// the decode graphs' gathers of Q4_K and Q5_0 / Q5_1 / Q8_0 rows: row t is DeviceState::tokens[t]
 __global__ void embed_q4k_kernel(const unsigned char *tok, size_t row_bytes, int E, const DeviceState *st, float *x) {
     const int t = blockIdx.x;
     const unsigned char *row = tok + (size_t)st->tokens[t] * row_bytes;
-    for (int i = threadIdx.x; i < E; i += blockDim.x) {
-        const unsigned char *b = row + (i / 256) * 144; const int e = i % 256, sub = e / 32, l = e % 32;
-        const float d = __half2float(*(const __half *)b), dmin = __half2float(*(const __half *)(b + 2));
-        int sc, mn; scale_min_k4(b + 4, sub, sc, mn);
-        const unsigned char qb = b[16 + (sub / 2) * 32 + l]; const int nib = (sub & 1) ? (qb >> 4) : (qb & 0xF);
-        x[(size_t)t * E + i] = (d * (float)sc) * (float)nib - dmin * (float)mn;
-    }
+    for (int i = threadIdx.x; i < E; i += blockDim.x) x[(size_t)t * E + i] = dequant_q4k_elem(row, i);
 }
-// token-embedding rows of Q5_0 / Q5_1 / Q8_0 files (ggml dequantize_row_q5_0 / q5_1 / q8_0), raw ggml blocks; kept out of dequant_elem (see above)
 __global__ void embed_b32_kernel(int type, const unsigned char *tok, size_t row_bytes, int E, const DeviceState *st, float *x) {
     const int t = blockIdx.x;
     const unsigned char *row = tok + (size_t)st->tokens[t] * row_bytes;
     for (int i = threadIdx.x; i < E; i += blockDim.x) {
-        const int j = i % 32, jj = j & 15;
-        float v;
-        if (type == GG_Q8_0) { const unsigned char *b = row + (i / 32) * 34; v = (float)(int)(signed char)b[2 + j] * __half2float(*(const __half *)b); }
-        else {
-            const int hdr = type == GG_Q5_1 ? 4 : 2;
-            const unsigned char *b = row + (i / 32) * (hdr + 20);
-            const unsigned qh = b[hdr] | (b[hdr + 1] << 8) | (b[hdr + 2] << 16) | ((unsigned)b[hdr + 3] << 24);
-            const int q = (j < 16 ? (b[hdr + 4 + jj] & 0xF) : (b[hdr + 4 + jj] >> 4)) | (int)(((qh >> j) & 1u) << 4);
-            const float d = __half2float(*(const __half *)b);
-            v = type == GG_Q5_1 ? (float)q * d + __half2float(*(const __half *)(b + 2)) : (float)(q - 16) * d;
-        }
+        MG4_DEQUANT_B32_ELEM(v, type, row, i)
         x[(size_t)t * E + i] = v;
     }
 }

@@ -20,6 +20,21 @@ def test_q4_k_matvec_is_bit_identical(ext, orc, mg, shape, n):
     assert np.array_equal(ext.op_matvec(12, raw, rows, cols, x), orc.mul_mat(12, raw, rows, cols, x))
 
 
+def queued_mixed_prompt_matches_oracle(ext, orc, llm):
+    """tokens, embedding rows, tokens: queued and evaluated in one flush (embed_rows_kernel decodes the file's token-embedding type), bit for
+    bit the oracle's piecewise run"""
+    c = ext.llm_load(llm, n_ctx=256)
+    e = orc.OracleEngine(None, llm, n_ctx=256)
+    rng = np.random.default_rng(5)
+    head, rows, tail = rng.integers(3, 1024, size=9).tolist(), rng.standard_normal((6, e.n_embd)).astype(np.float32), rng.integers(3, 1024, size=4).tolist()
+    ext.eval_tokens(c, head); ext.eval_embd(c, rows); ext.eval_tokens(c, tail); ext.flush(c)
+    e.eval_tokens(head); e.eval_embd(rows)
+    assert np.array_equal(ext.logits(c), e.eval_tokens(tail))
+    for _ in range(4):
+        t = ext.greedy_id(c); ext.eval_tokens(c, [t]); assert t == e.end_chat_greedy()[0]
+    ext.base.minigpt4_free(c)
+
+
 def test_q4_k_llama_file_matches_oracle(ext, orc, mg, tmp_path):
     llm = str(tmp_path / "llama-q4_k.bin")
     mg.write_llama_ggjt(llm, mg.LlamaSpec(n_vocab=1024, n_embd=512, n_head=4, n_layer=2, wtype="q4_k", output_type="q6_k"))
@@ -33,6 +48,7 @@ def test_q4_k_llama_file_matches_oracle(ext, orc, mg, tmp_path):
         t = ext.greedy_id(c); a.append(t); ext.eval_tokens(c, [t]); b.append(e.end_chat_greedy()[0])
     assert a == b
     ext.base.minigpt4_free(c)
+    queued_mixed_prompt_matches_oracle(ext, orc, llm)
 
 
 @pytest.mark.parametrize("name,gt", [("q5_0", 6), ("q5_1", 7), ("q8_0", 8)])
@@ -63,3 +79,4 @@ def test_b32_family_llama_file_matches_oracle(ext, orc, mg, tmp_path, name):
         t = ext.greedy_id(c); a.append(t); ext.eval_tokens(c, [t]); b.append(e.end_chat_greedy()[0])
     assert a == b
     ext.base.minigpt4_free(c)
+    queued_mixed_prompt_matches_oracle(ext, orc, llm)

@@ -169,6 +169,22 @@ def test_queued_prompt_pieces_equal_piecewise_evaluation(ext, tiny):
         ext.base.minigpt4_free(c1); ext.base.minigpt4_free(c2)
 
 
+def test_smaller_n_ctx_load_keeps_attention_of_a_larger_context(ext, orc, tiny):
+    """The attention kernels' shared-memory attribute (6 n_ctx bytes) is per device and only grows: loading a context with a small n_ctx
+    after one with a large n_ctx must leave the attention launches of the first one valid."""
+    big = ext.llm_load(tiny["q4_1"], n_ctx=16384)
+    small = ext.llm_load(tiny["q4_1"], n_ctx=256)
+    e = orc.OracleEngine(None, tiny["q4_1"], n_ctx=16384)
+    ids = list(range(5, 26))
+    ext.eval_tokens(big, ids)
+    assert np.array_equal(ext.logits(big), e.eval_tokens(ids))
+    a, b = [], []
+    for _ in range(8):
+        t = ext.greedy_id(big); a.append(t); ext.eval_tokens(big, [t]); b.append(e.end_chat_greedy()[0])
+    assert a == b
+    ext.base.minigpt4_free(small); ext.base.minigpt4_free(big)
+
+
 def test_context_overflow_is_an_error(ext, tiny):
     c = ext.llm_load(tiny["q4_1"], n_ctx=16)
     with pytest.raises(RuntimeError, match="FailedToAddString"):
