@@ -83,6 +83,21 @@ MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n)
 MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p,
                                               float tfs_z, float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
                                               float alpha_frequency, int mirostat, float mirostat_tau, float mirostat_eta, int penalize_nl);
+/* `steps` sampled decode steps of n (1..8) distinct contexts of one group with no return to the host in between: each step samples
+ * every context's logits on the device with the chain of minigpt4_end_chat (top_k, tail_free, typical, top_p, temperature, draw;
+ * no mirostat) and its own generator, then feeds the n ids in one decode step (n = 1: the context's own decode graph or megakernel;
+ * n >= 2: the batched step of minigpt4_b200_decode_batch).  Queued prompt pieces are evaluated first, as in end_chat_batch.
+ * Afterwards every context is where `steps` calls of minigpt4_end_chat (n = 1) or minigpt4_b200_end_chat_batch (n >= 2) with these
+ * parameters leave it: n_past, KV cache, logits, greedy id and the generator, which a later minigpt4_end_chat continues.
+ * ids_out[s * n + i] = the id context i was fed at step s (its text: minigpt4_b200_token_text); *ms_out (may be NULL) the
+ * CUDA-event time of the steps.  temp <= 0 is greedy: the ids of minigpt4_b200_decode_chain / decode_batch, generator untouched.
+ * The ids equal the host sampler's except where candidates tie: equal logits are ordered by lower id here (DESIGN.md §4.9).
+ * A call always runs exactly `steps` steps; there is no stop-token check inside it.  A caller that must stop at "</s>" runs
+ * steps = 1 per call, which still saves the copy of the logits to the host and the host sort of every token.
+ * NULL ctxs / ids_out, NULL or duplicate contexts, contexts of different groups, n outside 1..8, steps < 1, a tensor-parallel
+ * context or n_past + steps > n_ctx for any context return the FailedToAddString error code (8) before any device work. */
+MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int32_t top_k, float top_p,
+                                            float tfs_z, float typical_p, int32_t *ids_out, float *ms_out);
 
 /* batch encode (config 5): n images -> n embeddings, same semantics per image as minigpt4_encode_image */
 MINIGPT4_API int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, IN struct MiniGPT4Images *images, OUT struct MiniGPT4Embeddings *embeddings);
@@ -126,6 +141,16 @@ MINIGPT4_API int minigpt4_b200_host_tokenize(const char *llm_model, const char *
 /* run the sampler chain of minigpt4_end_chat on caller-provided logits (reference minigpt4.cpp:2425-2483) */
 MINIGPT4_API int minigpt4_b200_host_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
                                            float typical_p, int mirostat, float mirostat_tau, float mirostat_eta, int n_draws, int32_t *out_ids);
+/* the device twin of minigpt4_b200_host_sample (no mirostat, temp > 0): n_draws draws over the same logits from one generator
+ * seeded with `seed`, through the kernel of minigpt4_b200_sample_steps; 8 for bad arguments.  The _timed form also returns the
+ * average CUDA-event time of one sampling launch. */
+MINIGPT4_API int minigpt4_b200_op_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
+                                         float typical_p, int n_draws, int32_t *out_ids);
+MINIGPT4_API int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
+                                               float typical_p, int n_draws, int32_t *out_ids, float *kernel_ms);
+/* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with
+ * the host libm's; *mismatches = the number that differ */
+MINIGPT4_API int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches);
 /* block quantiser behind minigpt4_quantize_model (ggml quantize_row_*_reference): n floats (n % 32 == 0) -> ggml blocks of
  * `ggml_type` (2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0); returns the bytes written, -1 for an unsupported type or ragged n */
 MINIGPT4_API long minigpt4_b200_host_quantize_row(int ggml_type, const float *x, long n, void *out_blocks);

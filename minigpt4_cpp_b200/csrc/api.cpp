@@ -6,6 +6,9 @@
 #include <string.h>
 #include <sys/stat.h>
 #include <exception>
+#include <math.h>
+#include <algorithm>
+#include <thread>
 #include <string>
 
 using namespace mg4;
@@ -221,6 +224,11 @@ int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const cha
     SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     return Engine::end_chat_batch(reinterpret_cast<Engine *const *>(ctxs), n, tokens, sp);
 }
+int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int32_t top_k, float top_p, float tfs_z, float typical_p,
+                               int32_t *ids_out, float *ms_out) {
+    if (!ctxs) return ErrFailedToAddString;
+    return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out, ms_out);
+}
 int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, struct MiniGPT4Images *images, struct MiniGPT4Embeddings *embeddings) {
     if (embeddings->n_embeddings < images->n_images) return ErrImageSize;
     return E(ctx)->encode_images(images->images, images->n_images, embeddings->embeddings, nullptr);
@@ -282,6 +290,44 @@ int minigpt4_b200_host_sample(const float *logits, int n_vocab, int seed, float 
     Sampler s(seed);
     SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     for (int i = 0; i < n_draws; ++i) out_ids[i] = s.sample(logits, n_vocab, sp);
+    return 0;
+}
+int minigpt4_b200_op_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z, float typical_p,
+                            int n_draws, int32_t *out_ids) {
+    return minigpt4_b200_op_sample_timed(logits, n_vocab, seed, temp, top_k, top_p, tfs_z, typical_p, n_draws, out_ids, nullptr);
+}
+int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z, float typical_p,
+                                  int n_draws, int32_t *out_ids, float *kernel_ms) {
+    if (!logits || !out_ids || n_vocab < 1 || n_draws < 1 || !(temp > 0.f)) return ErrFailedToAddString;
+    uint32_t rng[625];
+    Sampler(seed).get_rng(rng);
+    LlamaDevice::test_sample(logits, n_vocab, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, rng, n_draws, out_ids, kernel_ms);
+    return 0;
+}
+int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) {
+    if ((fn != 0 && fn != 1) || hi_bits < lo_bits || !mismatches) return ErrFailedToAddString;
+    const uint64_t total = (uint64_t)hi_bits - lo_bits + 1, chunk = (uint64_t)1 << 26;
+    std::vector<float> dev((size_t)std::min(total, chunk));
+    const unsigned nt = std::max(1u, std::min(64u, std::thread::hardware_concurrency()));
+    long long bad = 0;
+    for (uint64_t base = 0; base < total; base += chunk) {
+        const uint32_t lo = (uint32_t)(lo_bits + base), c = (uint32_t)std::min(chunk, total - base);
+        LlamaDevice::test_libm(fn, lo, c, dev.data());
+        std::vector<long long> part(nt, 0);
+        std::vector<std::thread> th;
+        for (unsigned t = 0; t < nt; ++t) th.emplace_back([&, t] {
+            long long m = 0;
+            for (uint32_t i = (uint32_t)((uint64_t)c * t / nt); i < (uint32_t)((uint64_t)c * (t + 1) / nt); ++i) {
+                float x; const uint32_t u = lo + i; memcpy(&x, &u, 4);
+                const float h = fn == 0 ? expf(x) : logf(x);
+                if (memcmp(&h, &dev[i], 4) != 0) ++m;
+            }
+            part[t] = m;
+        });
+        for (auto &x : th) x.join();
+        for (long long m : part) bad += m;
+    }
+    *mismatches = bad;
     return 0;
 }
 int minigpt4_b200_host_inspect_container(const char *path, int *n_models, int *n_tensors, int *n_embd_llm) {

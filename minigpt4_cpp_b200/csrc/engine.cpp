@@ -124,6 +124,22 @@ Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const
     for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
     return decode_batch(e, n, ids, out);
 }
+Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out) {
+    if (!ids_out || !group_valid(e, n, "sample_steps")) return ErrFailedToAddString;
+    if (steps < 1) { MG4_ERR("sample_steps: %d steps", steps); return ErrFailedToAddString; }
+    for (int i = 0; i < n; ++i) {
+        if (e[i]->tp.world > 1) { MG4_ERR("sample_steps: context %d is tensor-parallel", i); return ErrFailedToAddString; }
+        const int n_ctx = e[i]->llm_->dims().n_ctx;
+        if (e[i]->n_past_ + steps > n_ctx) { MG4_ERR("sample_steps: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, steps, n_ctx); return ErrFailedToAddString; }
+    }
+    if (!flush_group(e, n)) return ErrFailedToAddString;
+    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625];
+    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; e[i]->sampler_->get_rng(rng[i]); }
+    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, ids_out);
+    for (int i = 0; i < n; ++i) { if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]); e[i]->n_past_ += steps; }
+    if (ms_out) *ms_out = ms;
+    return ErrNone;
+}
 Error Engine::flush_batch(Engine *const *e, int n) {
     if (!group_valid(e, n, "flush_batch")) return ErrFailedToAddString;
     return flush_group(e, n) ? ErrNone : ErrFailedToAddString;

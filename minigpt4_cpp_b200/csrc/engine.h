@@ -28,6 +28,9 @@ public:
     static Error decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out);
     // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
     static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
+    // `steps` decode steps of n (1..8) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
+    // own generator (see minigpt4_b200_sample_steps); ids_out[s * n + i]; all or nothing
+    static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
     // the queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
     static Error flush_batch(Engine *const *e, int n);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);

@@ -3,6 +3,7 @@
 #include "llama_mega6.cuh"
 #include "llama_prefill.cuh"
 #include "llama_sessions.cuh"
+#include "llama_sample.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -39,6 +40,34 @@ struct LlamaGroup {
             if (p) cudaFree(p);
         for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids}) if (p) cudaFreeHost(p);
         if (stream) cudaStreamDestroy(stream);
+    }
+};
+
+// device sampler (llama_sample.cuh): a context's generator state, candidate scratch and the ids of a call, in one allocation; the
+// generator state and the ids go through pinned staging
+struct SamplerScratch {
+    void *dev = nullptr;
+    smp::MtState *mt = nullptr;
+    int *ids = nullptr, *id = nullptr;
+    unsigned long long *keys = nullptr;
+    float *logit = nullptr, *p = nullptr, *aux = nullptr;
+    uint32_t *h_rng = nullptr;   // [625] pinned
+    int32_t *h_ids = nullptr;    // [n_ids] pinned
+    size_t bytes = 0;
+    SamplerScratch(int n_vocab, int n_ids) {
+        const size_t V = (size_t)n_vocab, P = (size_t)std::max(2, 1 << (int)ceil(log2((double)std::max(2, n_vocab))));
+        const size_t o_ids = (sizeof(smp::MtState) + 255) / 256 * 256, o_keys = o_ids + ((size_t)n_ids * 4 + 255) / 256 * 256, o_id = o_keys + P * 8;
+        bytes = o_id + 4 * V * 4;
+        CUDA_CHECK(cudaMalloc(&dev, bytes));
+        unsigned char *b = (unsigned char *)dev;
+        mt = (smp::MtState *)b; ids = (int *)(b + o_ids); keys = (unsigned long long *)(b + o_keys);
+        id = (int *)(b + o_id); logit = (float *)(b + o_id + V * 4); p = (float *)(b + o_id + 2 * V * 4); aux = (float *)(b + o_id + 3 * V * 4);
+        CUDA_CHECK(cudaHostAlloc((void **)&h_rng, 625 * 4, cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_ids, (size_t)n_ids * 4, cudaHostAllocDefault));
+    }
+    ~SamplerScratch() { if (dev) cudaFree(dev); if (h_rng) cudaFreeHost(h_rng); if (h_ids) cudaFreeHost(h_ids); }
+    smp::SampleCtx ctx(const float *logits, DeviceState *state, SessionSlot *slot, int n_past0) const {
+        return smp::SampleCtx{logits, state, slot, n_past0, mt, ids, keys, id, logit, p, aux};
     }
 };
 
@@ -209,6 +238,7 @@ LlamaDevice::~LlamaDevice() {
     if (ev0_) cudaEventDestroy(ev0_);
     if (ev1_) cudaEventDestroy(ev1_);
     if (stream_) cudaStreamDestroy(stream_);
+    smp_.reset();
 }
 void LlamaDevice::free_weights() {
     for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
@@ -1020,6 +1050,109 @@ void LlamaDevice::test_matvec(int gg, int rows, int cols, const void *w_host, co
     CUDA_CHECK(cudaMemcpy(tmp.data(), y, tmp.size() * 4, cudaMemcpyDeviceToHost));
     for (int i = 0; i < n; ++i) memcpy(y_host + (size_t)i * rows, tmp.data() + (size_t)i * m.rows, (size_t)rows * 4);
     cudaFree(x); cudaFree(y); cudaFree(stt); cudaFree(stg); qmat_free(m);
+}
+
+
+void LlamaDevice::ensure_sampler() {
+    if (smp_) return;
+    smp_.reset(new SamplerScratch(d_.n_vocab, d_.n_ctx));
+    owned_bytes_ += smp_->bytes;
+}
+
+static smp::SampleArgs sample_args(const SamplingArgs &p, int n_vocab) {
+    smp::SampleArgs a{};
+    a.n_vocab = n_vocab; a.top_k = p.top_k; a.temp = p.temp; a.top_p = p.top_p; a.tfs_z = p.tfs_z; a.typical_p = p.typical_p;
+    return a;
+}
+
+float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out) {
+    LlamaDevice &L0 = *c[0];
+    const bool sampled = p.temp > 0.f;
+    smp::SampleArgs a = sample_args(p, L0.d_.n_vocab);
+    cudaStream_t s = L0.stream_;
+    if (n >= 2) {   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
+        for (int i = 0; i < n; ++i) c[i]->sync();
+        LlamaGroup &G = *L0.group_;
+        if (!G.x) L0.build_group_workspace();
+        if (!G.graph[n]) L0.build_batch_graph(n);
+        s = G.stream;
+    }
+    for (int i = 0; i < n; ++i) {
+        LlamaDevice &L = *c[i];
+        L.ensure_sampler();
+        SessionSlot *slot = n >= 2 ? L0.group_->slots + i : nullptr;
+        a.c[i] = L.smp_->ctx(L.logits_, L.state_, slot, n_past[i]);
+        if (sampled) {
+            memcpy(L.smp_->h_rng, rng[i], 625 * 4);
+            CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, 625 * 4, cudaMemcpyHostToDevice, s));
+        }
+    }
+    if (n >= 2) {
+        LlamaGroup &G = *L0.group_;
+        for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
+        CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+    }
+    CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
+    for (int t = 0; t < steps; ++t) {
+        a.step = t;
+        smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
+        CUDA_CHECK(cudaGetLastError());
+        if (n == 1) {
+            L0.decode_step(-1, n_past[0] + t);
+            ++L0.launches_;
+        } else {
+            CUDA_CHECK(cudaGraphLaunch(L0.group_->graph[n], s));
+            L0.launches_ += (unsigned long long)L0.group_->graph_kernels[n] + 1;
+        }
+    }
+    CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
+    for (int i = 0; i < n; ++i) {
+        LlamaDevice &L = *c[i];
+        CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_ids, L.smp_->ids, (size_t)steps * 4, cudaMemcpyDeviceToHost, s));
+        if (sampled) CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_rng, L.smp_->mt, 625 * 4, cudaMemcpyDeviceToHost, s));
+    }
+    if (n == 1) L0.sync_decode();
+    else {
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        for (int i = 0; i < n; ++i) *c[i]->h_argmax_ = L0.group_->h_ids[i];   // (as decode_batch: the greedy id of the last step)
+    }
+    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, L0.ev0_, L0.ev1_));
+    for (int i = 0; i < n; ++i) {
+        LlamaDevice &L = *c[i];
+        for (int t = 0; t < steps; ++t) ids_out[(size_t)t * n + i] = L.smp_->h_ids[t];
+        if (sampled) memcpy(rng[i], L.smp_->h_rng, 625 * 4);
+    }
+    return ms;
+}
+
+void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms) {
+    SamplerScratch ss(n_vocab, n_draws);
+    float *lg = nullptr; DeviceState *st = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&lg, (size_t)n_vocab * 4));
+    CUDA_CHECK(cudaMalloc((void **)&st, sizeof(DeviceState))); CUDA_CHECK(cudaMemset(st, 0, sizeof(DeviceState)));
+    CUDA_CHECK(cudaMemcpy(lg, logits, (size_t)n_vocab * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(ss.mt, rng, 625 * 4, cudaMemcpyHostToDevice));
+    smp::SampleArgs a = sample_args(p, n_vocab);
+    a.c[0] = ss.ctx(lg, st, nullptr, 0);
+    cudaEvent_t e0, e1;
+    CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+    CUDA_CHECK(cudaEventRecord(e0, 0));
+    for (int i = 0; i < n_draws; ++i) { a.step = i; smp::sample_kernel<<<1, smp::kThreads>>>(a); CUDA_CHECK(cudaGetLastError()); }
+    CUDA_CHECK(cudaEventRecord(e1, 0));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    if (kernel_ms) *kernel_ms = n_draws > 0 ? ms / (float)n_draws : 0.f;
+    CUDA_CHECK(cudaMemcpy(out, ss.ids, (size_t)n_draws * 4, cudaMemcpyDeviceToHost));
+    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(lg); cudaFree(st);
+}
+
+void LlamaDevice::test_libm(int fn, uint32_t lo, uint32_t n, float *out_host) {
+    float *d = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&d, (size_t)n * 4));
+    smp::libm_kernel<<<1024, 256>>>(fn, lo, n, d);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpy(out_host, d, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    cudaFree(d);
 }
 
 }  // namespace mg4

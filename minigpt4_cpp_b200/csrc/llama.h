@@ -52,6 +52,9 @@ struct SessionSlot {   // one column of a batched decode step (device table of t
     DeviceState *state;
 };
 
+struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; };   // the non-mirostat chain of Sampler::sample
+struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
+
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
 
 class LlamaDevice {
@@ -77,6 +80,12 @@ public:
     // (KV cache, logits, arg-max, DeviceState) and the first rows of its hidden state are its rows of the pass that evaluated its
     // last row.  Synchronous.  The caller validates (distinct, one group, rows checked when they were queued).
     static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past);
+    // `steps` sampled decode steps of n (1..8) distinct contexts of one group with no host round trip: each step samples every context's
+    // current logits on the device (llama_sample.cuh; p.temp <= 0: the greedy id) into its DeviceState, then runs the decode step (n = 1:
+    // the context's own graph or megakernel; n >= 2: the batch graph, every column fed its DeviceState::tokens[0]).  rng[i] holds context
+    // i's mt19937 state (624 words and the position) on entry and on return; ids_out[s * n + i] is the id context i was fed at step s.
+    // One synchronisation at the end; returns the device ms of the steps.  The caller validates (distinct, one group, room for steps).
+    static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out);
     const LlamaDims &dims() const { return d_; }
     // Evaluate `n` mixed token / embedding rows (ids < 0: row -1 - id of emb_host) starting at position n_past.  Afterwards logits of the
     // last row are on device and the arg-max id is known.  Returns false if the context would overflow.
@@ -110,6 +119,11 @@ public:
     // kernel-level test hook: y[n][rows] = W x (W given as raw ggml blocks on host), through the same
     // repack + matvec kernels the engine uses.
     static void test_matvec(int gg, int rows, int cols, const void *w_host, const float *x_host, int n, float *y_host);
+    // sampler test hook: n_draws draws from one generator (rng: 624 words and the position) over the same n_vocab logits, as n_draws calls
+    // of Sampler::sample make (p.temp > 0); kernel_ms (optional): the average CUDA-event time of one sampling launch
+    static void test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms);
+    // the device expf (fn 0) / logf (fn 1) of the float bit patterns lo .. lo + n - 1
+    static void test_libm(int fn, uint32_t lo, uint32_t n, float *out_host);
 
 private:
     struct Layer { QMat qkv, wq, wk, wv, wo, w13, w2; bool fused_qkv; float *attn_norm, *ffn_norm; PQMat pqkv, pwo, pw13, pw2; };
@@ -168,6 +182,8 @@ private:
     // sessions: every context of a group holds the same weight pointers above; group_ counts the contexts
     std::shared_ptr<LlamaGroup> group_;
     size_t owned_bytes_ = 0;
+    std::unique_ptr<SamplerScratch> smp_;   // allocated by the context's first sample_steps call (counted in owned_bytes_ from then on)
+    void ensure_sampler();
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group
     void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)

@@ -1,0 +1,409 @@
+// llama_sample.cuh — sm_90a kernels of the device sampler (minigpt4_b200_sample_steps; host side LlamaDevice::sample_steps in llama.cu,
+// DESIGN.md §4.9): the reference's non-mirostat chain (minigpt4.cpp:2472-2477: top_k -> tail_free -> typical -> top_p -> temperature ->
+// draw) restated operation for operation from the host Sampler (text.cpp), so that a context draws the ids its host Sampler would draw
+// from the same mt19937 state.
+//
+// One CTA per context.  Element-wise work is spread over the CTA; every float sum the host takes sequentially (softmax, tail_free's
+// accumulate, the entropy, the cumulative cuts, the double sums of std::discrete_distribution) is taken by thread 0 in candidate order.
+// The build passes -fmad=false, so nothing is contracted except the fma() calls written out in the libm twins below.
+//
+// The one way the device can differ from the host: candidates with EQUAL sort keys (equal logits in the top-k / softmax sort, equal
+// |-log p - H| in typical's sort) are ordered by lower id (lower index) here, while libstdc++'s heap / introsort leaves them in an
+// order of its own.  Equal values give equal float results, so a tie can only change which of the tied ids is returned.
+#pragma once
+#include "llama.h"
+
+namespace mg4 {
+namespace smp {
+
+constexpr int kThreads = 1024;
+constexpr int kSmemSort = 4096;   // sorts of up to this many keys run in shared memory, larger ones in the context's scratch
+constexpr int kMtN = 624, kMtM = 397;
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// glibc's expf / logf (the ARM optimized-routines algorithms glibc ships, as its x86-64 FMA variants evaluate them), bit for bit.
+// CUDA's expf / logf round differently; the host Sampler calls glibc's.
+// ---------------------------------------------------------------------------------------------------------------------------------
+__constant__ unsigned long long kExp2fTab[32] = {   // asuint64(2^(i/32)) - (i << 47)
+    0x3ff0000000000000ull, 0x3fefd9b0d3158574ull, 0x3fefb5586cf9890full, 0x3fef9301d0125b51ull, 0x3fef72b83c7d517bull, 0x3fef54873168b9aaull,
+    0x3fef387a6e756238ull, 0x3fef1e9df51fdee1ull, 0x3fef06fe0a31b715ull, 0x3feef1a7373aa9cbull, 0x3feedea64c123422ull, 0x3feece086061892dull,
+    0x3feebfdad5362a27ull, 0x3feeb42b569d4f82ull, 0x3feeab07dd485429ull, 0x3feea47eb03a5585ull, 0x3feea09e667f3bcdull, 0x3fee9f75e8ec5f74ull,
+    0x3feea11473eb0187ull, 0x3feea589994cce13ull, 0x3feeace5422aa0dbull, 0x3feeb737b0cdc5e5ull, 0x3feec49182a3f090ull, 0x3feed503b23e255dull,
+    0x3feee89f995ad3adull, 0x3feeff76f2fb5e47ull, 0x3fef199bdd85529cull, 0x3fef3720dcef9069ull, 0x3fef5818dcfba487ull, 0x3fef7c97337b9b5full,
+    0x3fefa4afa2a490daull, 0x3fefd0765b6e4540ull};
+__constant__ double kLogfTab[16][2] = {   // {1/c, log c} of the 16 subintervals
+    {0x1.661ec79f8f3bep+0, -0x1.57bf7808caadep-2}, {0x1.571ed4aaf883dp+0, -0x1.2bef0a7c06ddbp-2}, {0x1.49539f0f010bp+0, -0x1.01eae7f513a67p-2},
+    {0x1.3c995b0b80385p+0, -0x1.b31d8a68224e9p-3}, {0x1.30d190c8864a5p+0, -0x1.6574f0ac07758p-3}, {0x1.25e227b0b8eap+0, -0x1.1aa2bc79c81p-3},
+    {0x1.1bb4a4a1a343fp+0, -0x1.a4e76ce8c0e5ep-4}, {0x1.12358f08ae5bap+0, -0x1.1973c5a611cccp-4}, {0x1.0953f419900a7p+0, -0x1.252f438e10c1ep-5},
+    {0x1p+0, 0x0p+0}, {0x1.e608cfd9a47acp-1, 0x1.aa5aa5df25984p-5}, {0x1.ca4b31f026aap-1, 0x1.c5e53aa362eb4p-4},
+    {0x1.b2036576afce6p-1, 0x1.526e57720db08p-3}, {0x1.9c2d163a1aa2dp-1, 0x1.bc2860d22477p-3}, {0x1.886e6037841edp-1, 0x1.1058bc8a07ee1p-2},
+    {0x1.767dcf5534862p-1, 0x1.4043057b6ee09p-2}};
+
+__device__ __forceinline__ float glibc_expf(float x) {
+    const unsigned ux = __float_as_uint(x), abstop = (ux >> 20) & 0x7ff;
+    if (abstop >= 0x42b) {   // |x| >= 88 or not finite
+        if (ux == 0xff800000u) return 0.0f;
+        if (abstop >= 0x7f8) return x + x;
+        if (x > 0x1.62e42ep6f) return __int_as_float(0x7f800000);
+        if (x < -0x1.9fe368p6f) return 0.0f;
+    }
+    const double inv_ln2_n = 0x1.71547652b82fep+0 * 32, shift = 0x1.8p+52;
+    const double c0 = 0x1.c6af84b912394p-5 / 32 / 32 / 32, c1 = 0x1.ebfce50fac4f3p-3 / 32 / 32, c2 = 0x1.62e42ff0c52d6p-1 / 32;
+    const double xd = (double)x;
+    double kd = __fma_rn(inv_ln2_n, xd, shift);   // x N / ln2 = k + r, rounded to nearest through the shift
+    const unsigned long long ki = (unsigned long long)__double_as_longlong(kd);
+    kd = __dsub_rn(kd, shift);
+    const double r = __fma_rn(inv_ln2_n, xd, -kd);
+    const unsigned long long t = kExp2fTab[ki % 32] + (ki << 47);
+    const double s = __longlong_as_double((long long)t);
+    const double z = __fma_rn(c0, r, c1), r2 = __dmul_rn(r, r);
+    double y = __fma_rn(c2, r, 1.0);
+    y = __fma_rn(z, r2, y);
+    return __double2float_rn(__dmul_rn(y, s));
+}
+
+__device__ __forceinline__ float glibc_logf(float x) {
+    unsigned ix = __float_as_uint(x);
+    if (ix == 0x3f800000u) return 0.0f;
+    if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u) {   // x < 0x1p-126, inf or nan
+        if (ix * 2 == 0) return __int_as_float(0xff800000);
+        if (ix == 0x7f800000u) return x;
+        if ((ix & 0x80000000u) || ix * 2 >= 0xff000000u) return __int_as_float(0x7fc00000);
+        ix = __float_as_uint(__fmul_rn(x, 0x1p23f));   // subnormal: normalise
+        ix -= 23u << 23;
+    }
+    const double ln2 = 0x1.62e42fefa39efp-1, a0 = -0x1.00ea348b88334p-2, a1 = 0x1.5575b0be00b6ap-2, a2 = -0x1.ffffef20a4123p-2;
+    const unsigned tmp = ix - 0x3f330000u;
+    const int i = (int)((tmp >> 19) % 16), kx = (int)tmp >> 23;
+    const unsigned iz = ix - (tmp & (0x1ffu << 23));
+    const double invc = kLogfTab[i][0], logc = kLogfTab[i][1], z = (double)__uint_as_float(iz);
+    const double r = __fma_rn(z, invc, -1.0);
+    const double y0 = __fma_rn((double)kx, ln2, logc);
+    const double r2 = __dmul_rn(r, r);
+    double y = __fma_rn(a1, r, a2);
+    y = __fma_rn(a0, r2, y);
+    y = __fma_rn(y, r2, __dadd_rn(y0, r));
+    return __double2float_rn(y);
+}
+
+// fn 0: expf, 1: logf of the float bit patterns lo .. lo + n - 1
+__global__ void libm_kernel(int fn, unsigned lo, unsigned n, float *out) {
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float x = __uint_as_float(lo + i);
+        out[i] = fn == 0 ? glibc_expf(x) : glibc_logf(x);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// the sampler
+// ---------------------------------------------------------------------------------------------------------------------------------
+struct MtState { unsigned x[kMtN]; unsigned p; };   // std::mt19937's state: 624 words and the position in them
+
+// one context's column of a sampling launch; the scratch pointers are its SamplerScratch (LlamaDevice::ensure_sampler)
+struct SampleCtx {
+    const float *logits;
+    DeviceState *state;          // tokens[0] takes the sampled id, which the decode step then feeds
+    SessionSlot *slot;           // batched steps: the context's column, whose position is n_past0 + step
+    int n_past0;
+    MtState *mt;
+    int *ids;                    // [n_ctx] the id fed at each step of a call
+    unsigned long long *keys;    // [pow2 >= n_vocab] sort keys; the discrete distribution's cumulative doubles afterwards
+    int *id; float *logit, *p, *aux;   // [n_vocab] candidates (id, logit, probability); tail_free's d2 / typical's terms
+};
+struct SampleArgs {
+    SampleCtx c[8];
+    int n_vocab, step, top_k;
+    float temp, top_p, tfs_z, typical_p;
+};
+
+// float -> key that orders like the float (-0 as +0, so that equal logits are equal keys), and back
+__device__ __forceinline__ unsigned ord_key(float v) {
+    const unsigned u = __float_as_uint(v == 0.0f ? 0.0f : v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ord_val(unsigned o) { return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o); }
+// descending order of these keys = logit descending, ties by lower id
+__device__ __forceinline__ unsigned long long desc_key(float v, int id) { return ((unsigned long long)ord_key(v) << 32) | (0xFFFFFFFFu - (unsigned)id); }
+__device__ __forceinline__ int key_id(unsigned long long k) { return (int)(0xFFFFFFFFu - (unsigned)(k & 0xFFFFFFFFull)); }
+
+__device__ __forceinline__ int pow2_at_least(int n) { int P = 2; while (P < n) P <<= 1; return P; }
+
+// one bitonic compare-exchange pass of stride st over buf[0, n) whose element 0 is element base of the whole sequence (the direction of
+// a pair follows its position in the whole sequence: descending where (position & size) == 0)
+__device__ __forceinline__ void bitonic_pass(unsigned long long *buf, int n, int base, int size, int st) {
+    for (int i = threadIdx.x; i < n / 2; i += blockDim.x) {
+        const int lo = 2 * i - (i & (st - 1)), hi = lo + st;
+        const bool desc = ((base + lo) & size) == 0;
+        const unsigned long long a = buf[lo], b = buf[hi];
+        if ((a < b) == desc) { buf[lo] = b; buf[hi] = a; }
+    }
+    __syncthreads();
+}
+
+// bitonic sort of buf[0, P) (P a power of two >= 2), descending.  Up to kSmemSort keys buf is sbuf itself; larger sequences live in
+// global scratch, and every run of passes with strides below kSmemSort is done chunk by chunk in sbuf, so only the strides of
+// kSmemSort and above make passes over global memory.
+__device__ void bitonic_desc(unsigned long long *buf, int P, unsigned long long *sbuf) {
+    constexpr int C = kSmemSort;
+    if (P <= C) {
+        for (int size = 2; size <= P; size <<= 1)
+            for (int st = size >> 1; st > 0; st >>= 1) bitonic_pass(buf, P, 0, size, st);
+        return;
+    }
+    auto local = [&](int size, int st0, bool all_sizes) {   // strides st0 .. 1 of every chunk (all_sizes: every size up to C first)
+        for (int base = 0; base < P; base += C) {
+            for (int i = threadIdx.x; i < C; i += blockDim.x) sbuf[i] = buf[base + i];
+            __syncthreads();
+            if (all_sizes) {
+                for (int sz = 2; sz <= C; sz <<= 1)
+                    for (int st = sz >> 1; st > 0; st >>= 1) bitonic_pass(sbuf, C, base, sz, st);
+            } else {
+                for (int st = st0; st > 0; st >>= 1) bitonic_pass(sbuf, C, base, size, st);
+            }
+            for (int i = threadIdx.x; i < C; i += blockDim.x) buf[base + i] = sbuf[i];
+            __syncthreads();
+        }
+    };
+    local(0, 0, true);
+    for (int size = 2 * C; size <= P; size <<= 1) {
+        int st = size >> 1;
+        for (; st >= C; st >>= 1) bitonic_pass(buf, P, 0, size, st);
+        local(size, st, false);
+    }
+}
+
+// the n candidates sorted by logit, descending (Sampler's by_logit_desc), ties by lower id; p is recomputed by the softmax that follows
+__device__ void sort_by_logit(const SampleCtx &c, int n, unsigned long long *sbuf) {
+    const int P = pow2_at_least(n);
+    unsigned long long *buf = P <= kSmemSort ? sbuf : c.keys;
+    for (int i = threadIdx.x; i < P; i += blockDim.x) buf[i] = i < n ? desc_key(c.logit[i], c.id[i]) : 0ull;
+    __syncthreads();
+    bitonic_desc(buf, P, sbuf);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { c.id[i] = key_id(buf[i]); c.logit[i] = ord_val((unsigned)(buf[i] >> 32)); }
+    __syncthreads();
+}
+
+// thread 0's in-order walk over x[0, n) for the sequential sums and cuts: 16 loads are issued before the 16 steps that use them, so their
+// latencies overlap; the steps themselves run one after another in index order.  f(i, x[i]) returns false to stop.
+template <class F> __device__ __forceinline__ void walk(const float *x, int n, F f) {
+    int i = 0;
+    for (; i + 16 <= n; i += 16) {
+        float v[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) v[j] = x[i + j];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) if (!f(i + j, v[j])) return;
+    }
+    for (; i < n; ++i) if (!f(i, x[i])) return;
+}
+
+// Sampler::softmax over sorted candidates: p = expf(logit - max), summed in order, p /= sum
+__device__ void softmax_sorted(const SampleCtx &c, int n, float *red) {
+    const float mx = c.logit[0];
+    for (int i = threadIdx.x; i < n; i += blockDim.x) c.p[i] = glibc_expf(c.logit[i] - mx);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float sum = 0.f;
+        walk(c.p, n, [&](int, float v) { sum += v; return true; });
+        *red = sum;
+    }
+    __syncthreads();
+    const float sum = *red;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) c.p[i] = c.p[i] / sum;
+    __syncthreads();
+}
+
+// std::mt19937's next output, as libstdc++ produces it: all 624 words are regenerated when the position reaches the end
+__device__ unsigned mt_next(MtState &m) {
+    if (m.p >= (unsigned)kMtN) {
+        const unsigned upper = 0x80000000u, lower = 0x7fffffffu, a = 0x9908b0dfu;
+        int k = 0;
+        for (; k < kMtN - kMtM; ++k) { const unsigned y = (m.x[k] & upper) | (m.x[k + 1] & lower); m.x[k] = m.x[k + kMtM] ^ (y >> 1) ^ ((y & 1u) ? a : 0u); }
+        for (; k < kMtN - 1; ++k) { const unsigned y = (m.x[k] & upper) | (m.x[k + 1] & lower); m.x[k] = m.x[k + kMtM - kMtN] ^ (y >> 1) ^ ((y & 1u) ? a : 0u); }
+        const unsigned y = (m.x[kMtN - 1] & upper) | (m.x[0] & lower);
+        m.x[kMtN - 1] = m.x[kMtM - 1] ^ (y >> 1) ^ ((y & 1u) ? a : 0u);
+        m.p = 0;
+    }
+    unsigned z = m.x[m.p++];
+    z ^= z >> 11;
+    z ^= (z << 7) & 0x9d2c5680u;
+    z ^= (z << 15) & 0xefc60000u;
+    z ^= z >> 18;
+    return z;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits as Sampler::sample does (temp <= 0: the
+// greedy id the logits epilogue already left in tokens[0]), writes the id into tokens[0] and ids[step], and moves a batched column to
+// its next position.
+// ---------------------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
+    __shared__ unsigned long long sbuf[kSmemSort];
+    __shared__ MtState mt;
+    __shared__ unsigned hist[256];
+    __shared__ unsigned long long sh_prefix;
+    __shared__ int sh_need, sh_done, sh_n;
+    __shared__ float red;
+    const SampleCtx &c = a.c[blockIdx.x];
+    const int tid = threadIdx.x, n = a.n_vocab;
+    if (a.temp <= 0.f) {
+        if (tid == 0) {
+            c.ids[a.step] = c.state->tokens[0];
+            if (c.slot) c.slot->n_past = c.n_past0 + a.step;
+        }
+        return;
+    }
+    for (int i = tid; i < kMtN; i += blockDim.x) mt.x[i] = c.mt->x[i];
+    if (tid == 0) mt.p = c.mt->p;
+
+    // ---- top_k: the k largest (logit desc, id asc) keys; k = top_k (<= 0: n_vocab) clamped to [1, n_vocab] as Sampler::top_k does
+    const int k = min(max(a.top_k <= 0 ? n : a.top_k, 1), n);
+    if (k == n) {
+        for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i]; }
+    } else {
+        // radix select, 8 bits at a time from the top: the threshold T with exactly k keys >= T (keys are distinct: they carry the id)
+        unsigned long long mask = 0ull;
+        if (tid == 0) { sh_prefix = 0ull; sh_need = k; }
+        for (int shift = 56; shift >= 0; shift -= 8) {
+            for (int i = tid; i < 256; i += blockDim.x) hist[i] = 0u;
+            __syncthreads();
+            const unsigned long long pre = sh_prefix;
+            for (int i = tid; i < n; i += blockDim.x) {
+                const unsigned long long key = desc_key(c.logits[i], i);
+                if ((key & mask) == pre) atomicAdd(&hist[(key >> shift) & 255], 1u);
+            }
+            __syncthreads();
+            if (tid == 0) {
+                int need = sh_need, d = 255; unsigned cum = 0;
+                for (; d > 0; --d) { if (cum + hist[d] >= (unsigned)need) break; cum += hist[d]; }
+                need -= (int)cum;
+                sh_prefix = pre | ((unsigned long long)d << shift);
+                sh_need = need;
+                sh_done = hist[d] == (unsigned)need;   // every key of this prefix is in: T = the prefix
+            }
+            __syncthreads();
+            mask |= 255ull << shift;
+            if (sh_done) break;
+        }
+        if (tid == 0) sh_n = 0;
+        __syncthreads();
+        const unsigned long long T = sh_prefix;
+        for (int i = tid; i < n; i += blockDim.x) {
+            const float v = c.logits[i];
+            if (desc_key(v, i) >= T) { const int j = atomicAdd(&sh_n, 1); c.id[j] = i; c.logit[j] = v; }
+        }
+    }
+    __syncthreads();
+    sort_by_logit(c, k, sbuf);
+    int m = k;
+    bool sorted = true;
+
+    // ---- tail_free
+    if (a.tfs_z < 1.0f && m > 2) {
+        softmax_sorted(c, m, &red);
+        for (int i = tid; i < m - 2; i += blockDim.x) {
+            const float d1a = c.p[i] - c.p[i + 1], d1b = c.p[i + 1] - c.p[i + 2];
+            c.aux[i] = fabsf(d1a - d1b);
+        }
+        __syncthreads();
+        if (tid == 0) {
+            float s = 0.f;
+            walk(c.aux, m - 2, [&](int, float v) { s += v; return true; });
+            float cum = 0.f; int last = m;
+            walk(c.aux, m - 2, [&](int i, float v) { cum += v / s; if (cum > a.tfs_z && i >= 1) { last = i; return false; } return true; });
+            sh_n = last;
+        }
+        __syncthreads();
+        m = sh_n;
+    }
+
+    // ---- typical: the candidates in order of |-log p - H| (ties by index) until their mass exceeds typical_p; leaves them unsorted
+    if (a.typical_p < 1.0f) {
+        softmax_sorted(c, m, &red);
+        for (int i = tid; i < m; i += blockDim.x) c.aux[i] = -c.p[i] * glibc_logf(c.p[i]);
+        __syncthreads();
+        if (tid == 0) {
+            float entropy = 0.f;
+            walk(c.aux, m, [&](int, float v) { entropy += v; return true; });
+            red = entropy;
+        }
+        __syncthreads();
+        const float entropy = red;
+        const int P = pow2_at_least(m);
+        unsigned long long *buf = P <= kSmemSort ? sbuf : c.keys;
+        for (int i = tid; i < P; i += blockDim.x) {   // descending order of ~shifted = ascending shifted, ties by lower index
+            if (i < m) {
+                const float shifted = fabsf(-glibc_logf(c.p[i]) - entropy);
+                buf[i] = ((unsigned long long)(~ord_key(shifted)) << 32) | (0xFFFFFFFFu - (unsigned)i);
+            } else buf[i] = 0ull;
+        }
+        __syncthreads();
+        bitonic_desc(buf, P, sbuf);
+        if (tid == 0) {
+            float cum = 0.f; int last = m;
+            for (int i = 0; i < m; ++i) { cum += c.p[key_id(buf[i])]; if (cum > a.typical_p) { last = i + 1; break; } }
+            sh_n = last;
+        }
+        __syncthreads();
+        const int last = sh_n;
+        for (int i = tid; i < last; i += blockDim.x) {   // gather the kept candidates in that order (through buf: in place)
+            const int j = key_id(buf[i]);
+            buf[i] = ((unsigned long long)(unsigned)c.id[j] << 32) | __float_as_uint(c.logit[j]);
+        }
+        __syncthreads();
+        for (int i = tid; i < last; i += blockDim.x) { c.id[i] = (int)(buf[i] >> 32); c.logit[i] = __uint_as_float((unsigned)buf[i]); }
+        __syncthreads();
+        m = last;
+        sorted = false;
+    }
+
+    // ---- top_p
+    if (a.top_p < 1.0f) {
+        if (!sorted) { sort_by_logit(c, m, sbuf); sorted = true; }
+        softmax_sorted(c, m, &red);
+        if (tid == 0) {
+            float cum = 0.f; int last = m;
+            walk(c.p, m, [&](int i, float v) { cum += v; if (cum >= a.top_p) { last = i + 1; return false; } return true; });
+            sh_n = last;
+        }
+        __syncthreads();
+        m = sh_n;
+    }
+
+    // ---- temperature, then draw: softmax, std::discrete_distribution<int> over the float probabilities
+    for (int i = tid; i < m; i += blockDim.x) c.logit[i] = c.logit[i] / a.temp;
+    __syncthreads();
+    if (!sorted) sort_by_logit(c, m, sbuf);
+    softmax_sorted(c, m, &red);
+    if (tid == 0) {
+        int idx = 0;   // one candidate: index 0, no draw from the generator
+        if (m >= 2) {
+            double sum = 0.0;
+            walk(c.p, m, [&](int, float v) { sum += (double)v; return true; });
+            double *cp = (double *)c.keys, acc = 0.0;
+            walk(c.p, m, [&](int i, float v) { acc += (double)v / sum; cp[i] = acc; return true; });
+            cp[m - 1] = 1.0;
+            // generate_canonical<double, 53>: two 32-bit outputs, (a + b 2^32) / 2^64, kept below 1
+            const double lo = (double)mt_next(mt), hi = (double)mt_next(mt);
+            double u = (lo + hi * 4294967296.0) / 18446744073709551616.0;
+            if (u >= 1.0) u = 0x1.fffffffffffffp-1;
+            int first = 0, len = m;   // std::lower_bound
+            while (len > 0) {
+                const int half = len >> 1, mid = first + half;
+                if (cp[mid] < u) { first = mid + 1; len = len - half - 1; }
+                else len = half;
+            }
+            idx = first;
+        }
+        const int id = c.id[idx];
+        c.state->tokens[0] = id;
+        c.ids[a.step] = id;
+        if (c.slot) c.slot->n_past = c.n_past0 + a.step;
+    }
+    __syncthreads();
+    for (int i = tid; i < kMtN; i += blockDim.x) c.mt->x[i] = mt.x[i];
+    if (tid == 0) c.mt->p = mt.p;
+}
+
+}  // namespace smp
+}  // namespace mg4

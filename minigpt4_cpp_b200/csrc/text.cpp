@@ -4,6 +4,7 @@
 #include <math.h>
 #include <numeric>
 #include <queue>
+#include <sstream>
 #include <time.h>
 
 namespace mg4 {
@@ -136,6 +137,17 @@ int32_t Sampler::draw(std::vector<Candidate> &c, bool &sorted) {
     for (auto &x : c) probs.push_back(x.p);
     std::discrete_distribution<> dist(probs.begin(), probs.end());
     return c[(size_t)dist(rng_)].id;
+}
+
+void Sampler::get_rng(uint32_t state[625]) const {
+    std::stringstream ss;
+    ss << rng_;
+    for (int i = 0; i < 625; ++i) ss >> state[i];
+}
+void Sampler::set_rng(const uint32_t state[625]) {
+    std::stringstream ss;
+    for (int i = 0; i < 625; ++i) ss << state[i] << ' ';
+    ss >> rng_;
 }
 
 int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingParams &sp) {

@@ -45,6 +45,9 @@ public:
     static void typical(std::vector<Candidate> &c, bool &sorted, float p, size_t min_keep);
     static void temperature(std::vector<Candidate> &c, float t);
     int32_t draw(std::vector<Candidate> &c, bool &sorted);
+    // the generator's state through its textual representation (operator<< / >>): the 624 words, then the position in them
+    void get_rng(uint32_t state[625]) const;
+    void set_rng(const uint32_t state[625]);
 private:
     std::mt19937 rng_;
     float mu_v1_ = 0, mu_v2_ = 0; bool mu_v1_init_ = false, mu_v2_init_ = false;

@@ -221,6 +221,7 @@ _EXT = {
     "minigpt4_b200_decode_batch": ([_VP, _I, _VP, _VP], _I),
     "minigpt4_b200_flush_batch": ([_VP, _I], _I),
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
+    "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
@@ -233,6 +234,9 @@ _EXT = {
     "minigpt4_b200_host_quantize_row": ([_I, _VP, C.c_long, _VP], C.c_long),
     "minigpt4_b200_host_tokenize": ([_S, _S, _I, _VP, _I], _I),
     "minigpt4_b200_host_sample": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _F, _F, _I, _VP], _I),
+    "minigpt4_b200_op_sample": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _VP], _I),
+    "minigpt4_b200_op_sample_timed": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_op_check_libm": ([_I, C.c_uint32, C.c_uint32, C.POINTER(C.c_longlong)], _I),
     "minigpt4_b200_host_inspect_container": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
     "minigpt4_b200_host_inspect_ggjt": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
 }
@@ -348,6 +352,17 @@ class B200:
                                                       mirostat_tau, mirostat_eta, penalize_nl))
         return [toks[i].decode("utf-8", errors="ignore") for i in range(n)]
 
+    def sample_steps(self, ctxs, steps: int, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0,
+                     typical_p: float = 1.0) -> tuple[np.ndarray, float]:
+        """`steps` device-sampled decode steps of every context in `ctxs` (1..8 of one group) with no host round trip in between;
+        returns the fed ids [steps, n] and the device ms of the steps"""
+        n = len(ctxs)
+        ids = np.zeros((max(1, steps), max(1, n)), np.int32)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_sample_steps(C.cast(self._ctx_array(ctxs), C.c_void_p), n, steps, temp, top_k, top_p, tfs_z, typical_p,
+                                                    _ptr(ids), C.byref(ms)))
+        return ids[:steps, :n], ms.value
+
     def time_matvec(self, ctx, kind: int, reps: int = 3) -> tuple[float, float]:
         ms, nb = C.c_float(0), C.c_double(0)
         self._chk(self.L.minigpt4_b200_time_matvec(ctx.ptr, kind, reps, C.byref(ms), C.byref(nb)))
@@ -409,6 +424,21 @@ class B200:
         return out
 
     # kernel seams
+    def op_sample(self, logits: np.ndarray, seed: int, n_draws: int = 1, temp=0.8, top_k=40, top_p=0.9, tfs_z=1.0, typical_p=1.0,
+                  timed: bool = False):
+        """the device twin of host_sample (no mirostat, temp > 0); timed: also the average ms of one sampling launch"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        out = np.zeros(n_draws, np.int32)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_op_sample_timed(_ptr(lg), lg.size, seed, temp, top_k, top_p, tfs_z, typical_p, n_draws, _ptr(out), C.byref(ms)))
+        return (out, ms.value) if timed else out
+
+    def op_check_libm(self, fn: int, lo_bits: int, hi_bits: int) -> int:
+        """device expf (fn 0) / logf (fn 1) against the host libm over the float bit patterns lo_bits..hi_bits; returns the mismatches"""
+        bad = C.c_longlong(0)
+        self._chk(self.L.minigpt4_b200_op_check_libm(fn, lo_bits, hi_bits, C.byref(bad)))
+        return bad.value
+
     def op_matvec(self, gtype: int, w_raw: np.ndarray, rows: int, cols: int, x: np.ndarray) -> np.ndarray:
         x = np.ascontiguousarray(x, np.float32).reshape(-1, cols)
         w = np.ascontiguousarray(w_raw)
