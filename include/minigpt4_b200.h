@@ -92,12 +92,33 @@ MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int
  * ids_out[s * n + i] = the id context i was fed at step s (its text: minigpt4_b200_token_text); *ms_out (may be NULL) the
  * CUDA-event time of the steps.  temp <= 0 is greedy: the ids of minigpt4_b200_decode_chain / decode_batch, generator untouched.
  * The ids equal the host sampler's except where candidates tie: equal logits are ordered by lower id here (DESIGN.md §4.9).
- * A call always runs exactly `steps` steps; there is no stop-token check inside it.  A caller that must stop at "</s>" runs
- * steps = 1 per call, which still saves the copy of the logits to the host and the host sort of every token.
+ * A call always runs exactly `steps` steps; to stop at the end of a reply use minigpt4_b200_sample_until.
  * NULL ctxs / ids_out, NULL or duplicate contexts, contexts of different groups, n outside 1..8, steps < 1, a tensor-parallel
  * context or n_past + steps > n_ctx for any context return the FailedToAddString error code (8) before any device work. */
 MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int32_t top_k, float top_p,
                                             float tfs_z, float typical_p, int32_t *ids_out, float *ms_out);
+/* A whole reply (or a chunk of one) for n (1..8) contexts of one group: the steps of minigpt4_b200_sample_steps, each context stopping
+ * where the reference's chat loop (MiniGPT4ChatBot.generate) stops its reply.  That loop appends the text of every token to the reply,
+ * skips the check for a token that is exactly "##", and otherwise stops once the reply ends with "###"; the stopping token is fed.  Here
+ * context i stops after the first step whose id's text is not exactly "##" and leaves the reply ending with `stop`, or after max_steps.
+ *   stop: NULL means "###" (the reference's EOS_SUFFIX); "" means no text stop; at most 32 bytes.
+ *   Texts are the bytes of the C strings minigpt4_end_chat returns (id 2 is "</s>"), with no UTF-8 decoding.
+ *   The reply is the text fed since the context's last system_prompt, begin_chat, begin_chat_image, reset_chat, b200_eval_tokens or
+ *   b200_eval_embd, by end_chat, end_chat_image, end_chat_batch, sample_steps and sample_until alike: a reply streamed as several calls
+ *   stops at the same step as one call, also when the stop text spans two calls.
+ * ids_out[s * n + i] = the id context i was fed at step s, -1 after its last step (room for max_steps * n); n_out[i] = the ids fed
+ * (1..max_steps); stopped[i] (may be NULL) = 1 if the stop text ended it, 0 if max_steps did; *ms_out (may be NULL) the CUDA-event time.
+ * Afterwards context i is where n_out[i] calls of minigpt4_end_chat (n = 1) or end_chat_batch (n >= 2) with these parameters leave it:
+ * n_past, logits, greedy id and generator.  A context that stops early is not changed by the steps the others still run.
+ * The host checks the stop flags every 4 steps without stalling the device, so up to 7 steps run past the last stop; their K/V writes
+ * lie above each context's final position, where its next token overwrites them.  The first call of a group builds a device table of
+ * every id's text (counted in minigpt4_b200_session_info's shared bytes); each context's first call allocates its stop state and a
+ * snapshot of its logits (owned bytes).
+ * NULL ctxs / ids_out / n_out, NULL or duplicate contexts, contexts of different groups, n outside 1..8, max_steps < 1, a stop text
+ * over 32 bytes, a tensor-parallel context or n_past + max_steps > n_ctx for any context return 8 before any device work. */
+MINIGPT4_API int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
+                                            float top_p, float tfs_z, float typical_p, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
+                                            float *ms_out);
 
 /* batch encode (config 5): n images -> n embeddings, same semantics per image as minigpt4_encode_image */
 MINIGPT4_API int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, IN struct MiniGPT4Images *images, OUT struct MiniGPT4Embeddings *embeddings);
@@ -148,6 +169,11 @@ MINIGPT4_API int minigpt4_b200_op_sample(const float *logits, int n_vocab, int s
                                          float typical_p, int n_draws, int32_t *out_ids);
 MINIGPT4_API int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
                                                float typical_p, int n_draws, int32_t *out_ids, float *kernel_ms);
+/* minigpt4_b200_sample_until's stop rule on the device, over the ids ids[0..n) of ctx's vocabulary from a reply that ends with `tail`
+ * (NULL: empty; its last 32 bytes count): *stop_at = the index of the id after which the reply ends, -1 if none; stop as in
+ * sample_until.  Changes nothing in ctx.  8 for a NULL ctx / stop_at, an id outside the vocabulary or a stop text over 32 bytes. */
+MINIGPT4_API int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail,
+                                             int32_t *stop_at);
 /* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with
  * the host libm's; *mismatches = the number that differ */
 MINIGPT4_API int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches);

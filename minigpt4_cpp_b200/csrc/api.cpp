@@ -88,6 +88,7 @@ int minigpt4_encode_image(struct MiniGPT4Context *ctx, struct MiniGPT4Image *ima
 
 int minigpt4_begin_chat_image(struct MiniGPT4Context *ctx, struct MiniGPT4Embedding *image_embedding, const char *s, size_t) {
     Engine *e = E(ctx);
+    e->reply_clear();
     if (Error err = e->add_strings("Human: <Img>")) return err;
     if (image_embedding->elements != 32u * 5120u && image_embedding->elements != 32u * 4096u) {
         MG4_ERR("LLAMA projection image embedding size not valid: %zu", image_embedding->elements);
@@ -108,13 +109,15 @@ int minigpt4_end_chat_image(struct MiniGPT4Context *ctx, const char **token, siz
     const int32_t id = e->sample_token(sp);
     *token = e->id_to_token(id);
     e->add_tokens({id});  // the reference ignores this return value too (minigpt4.cpp:2715)
+    e->reply_take(*token);
     return ErrNone;
 }
 
-int minigpt4_system_prompt(struct MiniGPT4Context *ctx, size_t) { return E(ctx)->add_strings(kSystemPrompt); }
+int minigpt4_system_prompt(struct MiniGPT4Context *ctx, size_t) { E(ctx)->reply_clear(); return E(ctx)->add_strings(kSystemPrompt); }
 
 int minigpt4_begin_chat(struct MiniGPT4Context *ctx, const char *s, size_t) {
     Engine *e = E(ctx);
+    e->reply_clear();
     if (Error err = e->add_strings("Human: ")) return err;
     if (Error err = e->add_strings(s)) return err;
     if (Error err = e->add_strings("### Assistant:")) return err;
@@ -184,8 +187,11 @@ int minigpt4_b200_tokenize(struct MiniGPT4Context *ctx, const char *text, int ad
     memcpy(out, t.data(), t.size() * sizeof(int32_t));
     return (int)t.size();
 }
-int minigpt4_b200_eval_tokens(struct MiniGPT4Context *ctx, const int32_t *ids, int n) { return n <= 0 ? 0 : E(ctx)->add_tokens(std::vector<int32_t>(ids, ids + n)); }
-int minigpt4_b200_eval_embd(struct MiniGPT4Context *ctx, const float *rows, int n) { return E(ctx)->add_embedding(rows, n); }
+int minigpt4_b200_eval_tokens(struct MiniGPT4Context *ctx, const int32_t *ids, int n) {
+    E(ctx)->reply_clear();
+    return n <= 0 ? 0 : E(ctx)->add_tokens(std::vector<int32_t>(ids, ids + n));
+}
+int minigpt4_b200_eval_embd(struct MiniGPT4Context *ctx, const float *rows, int n) { E(ctx)->reply_clear(); return E(ctx)->add_embedding(rows, n); }
 int minigpt4_b200_flush(struct MiniGPT4Context *ctx) { return E(ctx)->flush() ? 0 : ErrFailedToAddString; }
 int minigpt4_b200_get_logits(struct MiniGPT4Context *ctx, float *out) { E(ctx)->flush(); E(ctx)->llm().logits_to_host(out); return 0; }
 int minigpt4_b200_greedy_id(struct MiniGPT4Context *ctx) { E(ctx)->flush(); return E(ctx)->llm().argmax(); }
@@ -228,6 +234,12 @@ int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, 
                                int32_t *ids_out, float *ms_out) {
     if (!ctxs) return ErrFailedToAddString;
     return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out, ms_out);
+}
+int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k, float top_p,
+                               float tfs_z, float typical_p, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out) {
+    if (!ctxs) return ErrFailedToAddString;
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out,
+                                n_out, stopped, ms_out);
 }
 int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, struct MiniGPT4Images *images, struct MiniGPT4Embeddings *embeddings) {
     if (embeddings->n_embeddings < images->n_images) return ErrImageSize;
@@ -303,6 +315,10 @@ int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab, int seed, fl
     Sampler(seed).get_rng(rng);
     LlamaDevice::test_sample(logits, n_vocab, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, rng, n_draws, out_ids, kernel_ms);
     return 0;
+}
+int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at) {
+    if (!ctx) return ErrFailedToAddString;
+    return E(ctx)->reply_stop(ids, n, stop, tail, stop_at);
 }
 int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) {
     if ((fn != 0 && fn != 1) || hi_bits < lo_bits || !mismatches) return ErrFailedToAddString;

@@ -122,7 +122,9 @@ Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const
     if (!flush_group(e, n)) return ErrFailedToAddString;   // so that each sample_token finds its queue empty
     int32_t ids[8], out[8];
     for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
-    return decode_batch(e, n, ids, out);
+    const Error err = decode_batch(e, n, ids, out);
+    for (int i = 0; i < n; ++i) e[i]->reply_take(tokens[i]);
+    return err;
 }
 Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out) {
     if (!ids_out || !group_valid(e, n, "sample_steps")) return ErrFailedToAddString;
@@ -136,9 +138,57 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
     LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625];
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; e[i]->sampler_->get_rng(rng[i]); }
     const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, ids_out);
-    for (int i = 0; i < n; ++i) { if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]); e[i]->n_past_ += steps; }
+    for (int i = 0; i < n; ++i) {
+        if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]);
+        e[i]->n_past_ += steps;
+        for (int t = 0; t < steps; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
+    }
     if (ms_out) *ms_out = ms;
     return ErrNone;
+}
+Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
+                           int32_t *stopped, float *ms_out) {
+    if (!ids_out || !n_out || !group_valid(e, n, "sample_until")) return ErrFailedToAddString;
+    if (max_steps < 1) { MG4_ERR("sample_until: %d steps", max_steps); return ErrFailedToAddString; }
+    const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
+    if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("sample_until: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
+    for (int i = 0; i < n; ++i) {
+        if (e[i]->tp.world > 1) { MG4_ERR("sample_until: context %d is tensor-parallel", i); return ErrFailedToAddString; }
+        const int n_ctx = e[i]->llm_->dims().n_ctx;
+        if (e[i]->n_past_ + max_steps > n_ctx) { MG4_ERR("sample_until: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, max_steps, n_ctx); return ErrFailedToAddString; }
+    }
+    if (!flush_group(e, n)) return ErrFailedToAddString;
+    e[0]->ensure_token_table();
+    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; std::string tail[8];
+    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; e[i]->sampler_->get_rng(rng[i]); tail[i] = e[i]->reply_; }
+    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, st, tail, ids_out, n_out, stopped);
+    for (int i = 0; i < n; ++i) {
+        if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]);
+        e[i]->n_past_ += n_out[i];
+        for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
+    }
+    if (ms_out) *ms_out = ms;
+    return ErrNone;
+}
+Error Engine::reply_stop(const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at) {
+    const std::string st = stop ? stop : "###";
+    if (!stop_at || n < 0 || (n > 0 && !ids) || st.size() > (size_t)LlamaDevice::kStopMax) return ErrFailedToAddString;
+    for (int i = 0; i < n; ++i) if (ids[i] < 0 || ids[i] >= llm_->dims().n_vocab) { MG4_ERR("reply_stop: token id %d out of range", ids[i]); return ErrFailedToAddString; }
+    ensure_token_table();
+    *stop_at = llm_->test_reply_stop(ids, n, st, tail ? tail : "");
+    return ErrNone;
+}
+void Engine::ensure_token_table() {
+    if (llm_->has_token_table()) return;
+    const int V = llm_->dims().n_vocab;
+    std::vector<int> off((size_t)V + 1, 0);
+    std::string bytes;
+    for (int id = 0; id < V; ++id) { bytes += id_to_token(id); off[(size_t)id + 1] = (int)bytes.size(); }
+    llm_->set_token_table(off, bytes);
+}
+void Engine::reply_take(const char *text) {
+    reply_ += text;
+    if (reply_.size() > (size_t)LlamaDevice::kStopMax) reply_.erase(0, reply_.size() - LlamaDevice::kStopMax);
 }
 Error Engine::flush_batch(Engine *const *e, int n) {
     if (!group_valid(e, n, "flush_batch")) return ErrFailedToAddString;

@@ -31,6 +31,12 @@ public:
     // `steps` decode steps of n (1..8) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
     // own generator (see minigpt4_b200_sample_steps); ids_out[s * n + i]; all or nothing
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
+    // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
+    // "###"; all or nothing
+    static Error sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
+                              int32_t *stopped, float *ms_out);
+    // sample_until's text check over ids from the reply `tail` (see minigpt4_b200_op_reply_stop); -1: no id ends the reply
+    Error reply_stop(const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at);
     // the queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
     static Error flush_batch(Engine *const *e, int n);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
@@ -41,7 +47,11 @@ public:
     Error add_embedding(const float *rows, int n_rows);
     int32_t sample_token(const SamplingParams &p);
     const char *id_to_token(int32_t id) const;
-    void reset() { n_past_ = 0; pend_ids_.clear(); pend_emb_.clear(); }
+    void reset() { n_past_ = 0; pend_ids_.clear(); pend_emb_.clear(); reply_.clear(); }
+    // the current reply's last LlamaDevice::kStopMax bytes (the reference's `chat` of a turn): a new turn or prompt clears it, every
+    // fed id's text extends it, so a reply streamed over several sample_until calls stops where one call would
+    void reply_clear() { reply_.clear(); }
+    void reply_take(const char *text);
     bool flush();                     // evaluate the queued prompt rows (see add_tokens)
     static constexpr int kMaxPending = LlamaDevice::kPrefillMax;
 
@@ -71,6 +81,8 @@ private:
     std::vector<int32_t> pend_ids_;   // queued rows: token id, or -1 - k for row k of pend_emb_
     std::vector<float> pend_emb_;
     int pend_base_ = 0;               // position of the first queued row
+    std::string reply_;
+    void ensure_token_table();          // the group's device table of id_to_token (sample_until's stop rule)
     int n_batch_ = 512;
 };
 

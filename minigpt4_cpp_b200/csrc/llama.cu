@@ -34,9 +34,11 @@ struct LlamaGroup {
     int *ids = nullptr, *h_ids = nullptr;               // [8] their new arg-max ids
     cudaGraphExec_t graph[9] = {};
     int graph_kernels[9] = {};
+    smp::TokenTable tokens{};      // every id's text for sample_until's stop rule (built by the group's first call)
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
-        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)rows, (void *)slots, (void *)ids})
+        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)rows, (void *)slots, (void *)ids,
+                        (void *)tokens.off, (void *)tokens.bytes})
             if (p) cudaFree(p);
         for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids}) if (p) cudaFreeHost(p);
         if (stream) cudaStreamDestroy(stream);
@@ -68,6 +70,30 @@ struct SamplerScratch {
     ~SamplerScratch() { if (dev) cudaFree(dev); if (h_rng) cudaFreeHost(h_rng); if (h_ids) cudaFreeHost(h_ids); }
     smp::SampleCtx ctx(const float *logits, DeviceState *state, SessionSlot *slot, int n_past0) const {
         return smp::SampleCtx{logits, state, slot, n_past0, mt, ids, keys, id, logit, p, aux};
+    }
+};
+
+// sample_until's per-context state (llama_sample.cuh): the ReplyState and the logits snapshot on the device, a pinned mirror of the
+// ReplyState, and the done flags and chunk events of the calls this context leads (its column 0)
+struct ReplyScratch {
+    smp::ReplyState *r = nullptr, *h_r = nullptr;
+    float *snap = nullptr;
+    int *h_done = nullptr;   // [2][8] pinned: the done flags after the last two chunks issued
+    cudaEvent_t ev[2] = {};
+    size_t bytes = 0;
+    explicit ReplyScratch(int n_vocab) {
+        bytes = sizeof(smp::ReplyState) + (size_t)n_vocab * 4;
+        CUDA_CHECK(cudaMalloc((void **)&r, bytes));
+        snap = (float *)(r + 1);
+        CUDA_CHECK(cudaHostAlloc((void **)&h_r, sizeof(smp::ReplyState), cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_done, 16 * sizeof(int), cudaHostAllocDefault));
+        for (cudaEvent_t &e : ev) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    ~ReplyScratch() {
+        if (r) cudaFree(r);
+        if (h_r) cudaFreeHost(h_r);
+        if (h_done) cudaFreeHost(h_done);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
     }
 };
 
@@ -239,6 +265,7 @@ LlamaDevice::~LlamaDevice() {
     if (ev1_) cudaEventDestroy(ev1_);
     if (stream_) cudaStreamDestroy(stream_);
     smp_.reset();
+    reply_.reset();
 }
 void LlamaDevice::free_weights() {
     for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
@@ -1065,10 +1092,9 @@ static smp::SampleArgs sample_args(const SamplingArgs &p, int n_vocab) {
     return a;
 }
 
-float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out) {
+cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], smp::SampleArgs &a) {
     LlamaDevice &L0 = *c[0];
-    const bool sampled = p.temp > 0.f;
-    smp::SampleArgs a = sample_args(p, L0.d_.n_vocab);
+    a = sample_args(p, L0.d_.n_vocab);
     cudaStream_t s = L0.stream_;
     if (n >= 2) {   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
         for (int i = 0; i < n; ++i) c[i]->sync();
@@ -1082,7 +1108,7 @@ float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const i
         L.ensure_sampler();
         SessionSlot *slot = n >= 2 ? L0.group_->slots + i : nullptr;
         a.c[i] = L.smp_->ctx(L.logits_, L.state_, slot, n_past[i]);
-        if (sampled) {
+        if (p.temp > 0.f) {
             memcpy(L.smp_->h_rng, rng[i], 625 * 4);
             CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, 625 * 4, cudaMemcpyHostToDevice, s));
         }
@@ -1092,19 +1118,25 @@ float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const i
         for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
         CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
     }
-    CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
-    for (int t = 0; t < steps; ++t) {
-        a.step = t;
-        smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
-        CUDA_CHECK(cudaGetLastError());
-        if (n == 1) {
-            L0.decode_step(-1, n_past[0] + t);
-            ++L0.launches_;
-        } else {
-            CUDA_CHECK(cudaGraphLaunch(L0.group_->graph[n], s));
-            L0.launches_ += (unsigned long long)L0.group_->graph_kernels[n] + 1;
-        }
+    return s;
+}
+
+// the decode step after a sampling launch (counted with it): every column is fed its DeviceState::tokens[0]
+void LlamaDevice::sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s) {
+    LlamaDevice &L0 = *c[0];
+    CUDA_CHECK(cudaGetLastError());
+    if (n == 1) {
+        L0.decode_step(-1, n_past);
+        ++L0.launches_;
+    } else {
+        CUDA_CHECK(cudaGraphLaunch(L0.group_->graph[n], s));
+        L0.launches_ += (unsigned long long)L0.group_->graph_kernels[n] + 1;
     }
+}
+
+// after `steps` steps: the fed ids and generators to the host, one synchronisation; returns the device ms since ev0_
+float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, bool sampled, uint32_t (*rng)[625], int32_t *ids_out, cudaStream_t s) {
+    LlamaDevice &L0 = *c[0];
     CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
@@ -1123,6 +1155,119 @@ float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const i
         if (sampled) memcpy(rng[i], L.smp_->h_rng, 625 * 4);
     }
     return ms;
+}
+
+float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out) {
+    smp::SampleArgs a;
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, a);
+    CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
+    for (int t = 0; t < steps; ++t) {
+        a.step = t;
+        smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
+        sampled_decode(c, n, n_past[0] + t, s);
+    }
+    return end_sampling(c, n, steps, p.temp > 0.f, rng, ids_out, s);
+}
+
+void LlamaDevice::ensure_reply() {
+    if (reply_) return;
+    reply_.reset(new ReplyScratch(d_.n_vocab));
+    owned_bytes_ += reply_->bytes;
+}
+bool LlamaDevice::has_token_table() const { return group_->tokens.off != nullptr; }
+void LlamaDevice::set_token_table(const std::vector<int> &off, const std::string &bytes) {
+    LlamaGroup &G = *group_;
+    const size_t b0 = t_dev_bytes;
+    int *o = nullptr; unsigned char *b = nullptr;
+    dmalloc(&o, off.size() * 4);
+    dmalloc(&b, std::max<size_t>(1, bytes.size()));
+    CUDA_CHECK(cudaMemcpy(o, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(b, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+    G.tokens = smp::TokenTable{o, b};
+    G.batch_bytes += t_dev_bytes - b0;
+}
+
+// a context's ReplyState at the start of a call: its reply's last kStopMax bytes, the stop text, nothing fed
+static void reply_init(smp::ReplyState &r, const std::string &stop, const std::string &tail) {
+    memset(&r, 0, sizeof(r));
+    const size_t keep = std::min(tail.size(), (size_t)smp::kStopMax);
+    memcpy(r.tail, tail.data() + tail.size() - keep, keep);
+    r.tail_len = (int)keep;
+    memcpy(r.stop, stop.data(), stop.size());
+    r.stop_len = (int)stop.size();
+}
+
+float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
+                                const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped) {
+    LlamaDevice &L0 = *c[0];
+    smp::SampleArgs a;
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, a);
+    smp::StopArgs sa{};
+    sa.tab = L0.group_->tokens;
+    for (int i = 0; i < n; ++i) {
+        LlamaDevice &L = *c[i];
+        L.ensure_reply();
+        reply_init(*L.reply_->h_r, stop, tail[i]);
+        CUDA_CHECK(cudaMemcpyAsync(L.reply_->r, L.reply_->h_r, sizeof(smp::ReplyState), cudaMemcpyHostToDevice, s));
+        sa.r[i] = L.reply_->r; sa.snap[i] = L.reply_->snap;
+    }
+    ReplyScratch &R0 = *L0.reply_;
+    CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
+    int issued = 0;
+    for (int j = 0; issued < max_steps; ++j) {
+        if (j >= 2) {   // chunk j - 2's flags; chunk j - 1 keeps the device busy meanwhile
+            CUDA_CHECK(cudaEventSynchronize(R0.ev[j % 2]));
+            bool all = true;
+            for (int i = 0; i < n; ++i) all = all && R0.h_done[(j % 2) * 8 + i] != 0;
+            if (all) break;
+        }
+        for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
+            a.step = issued;
+            smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
+            sampled_decode(c, n, n_past[0] + issued, s);
+        }
+        for (int i = 0; i < n; ++i)
+            CUDA_CHECK(cudaMemcpyAsync(R0.h_done + (j % 2) * 8 + i, &c[i]->reply_->r->done, sizeof(int), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaEventRecord(R0.ev[j % 2], s));
+    }
+    for (int i = 0; i < n; ++i)
+        CUDA_CHECK(cudaMemcpyAsync(c[i]->reply_->h_r, c[i]->reply_->r, sizeof(smp::ReplyState), cudaMemcpyDeviceToHost, s));
+    const float ms = end_sampling(c, n, issued, p.temp > 0.f, rng, ids_out, s);
+    // a context that stopped before the last issued step gets back what its stopping step left
+    for (int i = 0; i < n; ++i) {
+        LlamaDevice &L = *c[i];
+        const smp::ReplyState &r = *L.reply_->h_r;
+        n_out[i] = r.n_fed;
+        if (stopped) stopped[i] = r.done != 0 ? 1 : 0;
+        for (int t = r.n_fed; t < issued; ++t) ids_out[(size_t)t * n + i] = -1;
+        if (r.done == 2) {
+            CUDA_CHECK(cudaMemcpyAsync(L.logits_, L.reply_->snap, (size_t)L.d_.n_vocab * 4, cudaMemcpyDeviceToDevice, s));
+            CUDA_CHECK(cudaMemcpyAsync(L.state_, &L.reply_->r->snap, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
+            *L.h_argmax_ = r.snap.argmax_id;
+        }
+    }
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    for (int t = issued; t < max_steps; ++t)
+        for (int i = 0; i < n; ++i) ids_out[(size_t)t * n + i] = -1;
+    return ms;
+}
+
+// the seam of the stop rule: one thread of reply_check_kernel over the ids, with this context's ReplyState and the group's table
+int LlamaDevice::test_reply_stop(const int32_t *ids, int n, const std::string &stop, const std::string &tail) {
+    ensure_reply();
+    sync();
+    reply_init(*reply_->h_r, stop, tail);
+    int *d = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&d, ((size_t)n + 1) * 4));
+    CUDA_CHECK(cudaMemcpyAsync(reply_->r, reply_->h_r, sizeof(smp::ReplyState), cudaMemcpyHostToDevice, stream_));
+    CUDA_CHECK(cudaMemcpyAsync(d + 1, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_));
+    smp::reply_check_kernel<<<1, 1, 0, stream_>>>(reply_->r, group_->tokens, d + 1, n, d);
+    CUDA_CHECK(cudaGetLastError());
+    int at = -1;
+    CUDA_CHECK(cudaMemcpyAsync(&at, d, 4, cudaMemcpyDeviceToHost, stream_));
+    sync();
+    cudaFree(d);
+    return at;
 }
 
 void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms) {

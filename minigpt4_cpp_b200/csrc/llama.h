@@ -54,6 +54,8 @@ struct SessionSlot {   // one column of a batched decode step (device table of t
 
 struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; };   // the non-mirostat chain of Sampler::sample
 struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
+struct ReplyScratch;   // a context's stop state in sample_until: reply tail, stop text, done flag, snapshot (llama.cu, llama_sample.cuh)
+namespace smp { struct SampleArgs; }
 
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
 
@@ -86,6 +88,21 @@ public:
     // i's mt19937 state (624 words and the position) on entry and on return; ids_out[s * n + i] is the id context i was fed at step s.
     // One synchronisation at the end; returns the device ms of the steps.  The caller validates (distinct, one group, room for steps).
     static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out);
+    // sample_steps that stops each context after the step whose id's text (not exactly "##") makes its reply end with `stop` (0..32
+    // bytes, "" no text stop), or after max_steps.  tail[i]: context i's reply so far (its last 32 bytes decide).  The steps are issued
+    // kReplyChunk at a time; the host waits for chunk j - 1's done flags before it issues chunk j + 1 and stops issuing once every
+    // context is done, so at most 2 kReplyChunk - 1 steps run past the last stop.  Afterwards context i holds what n_out[i] steps left
+    // (logits, DeviceState, arg-max; rng[i]), and ids_out[s * n + i] = -1 for s >= n_out[i]; stopped[i] = the text ended it.  Needs the
+    // group's token table (set_token_table).  One wait per chunk, none of them stalling the device; returns the device ms.
+    static constexpr int kReplyChunk = 4;
+    static constexpr int kStopMax = 32;   // longest stop text
+    static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
+                              const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped);
+    // the group's device table of every id's text (off: n_vocab + 1 offsets into bytes), counted in shared_bytes
+    bool has_token_table() const;
+    void set_token_table(const std::vector<int> &off, const std::string &bytes);
+    // sample_until's text check over ids[0, n) from the reply `tail`; returns the index of the id that ends the reply, -1 if none
+    int test_reply_stop(const int32_t *ids, int n, const std::string &stop, const std::string &tail);
     const LlamaDims &dims() const { return d_; }
     // Evaluate `n` mixed token / embedding rows (ids < 0: row -1 - id of emb_host) starting at position n_past.  Afterwards logits of the
     // last row are on device and the arg-max id is known.  Returns false if the context would overflow.
@@ -184,6 +201,13 @@ private:
     size_t owned_bytes_ = 0;
     std::unique_ptr<SamplerScratch> smp_;   // allocated by the context's first sample_steps call (counted in owned_bytes_ from then on)
     void ensure_sampler();
+    std::unique_ptr<ReplyScratch> reply_;   // sample_until's stop state and snapshot, from the context's first call (owned_bytes_)
+    void ensure_reply();
+    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler and generator; returns the
+    // stream the steps run on
+    static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], smp::SampleArgs &a);
+    static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
+    static float end_sampling(LlamaDevice *const *c, int n, int steps, bool sampled, uint32_t (*rng)[625], int32_t *ids_out, cudaStream_t s);
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group
     void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)

@@ -233,24 +233,20 @@ __device__ unsigned mt_next(MtState &m) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits as Sampler::sample does (temp <= 0: the
-// greedy id the logits epilogue already left in tokens[0]), writes the id into tokens[0] and ids[step], and moves a batched column to
-// its next position.
+// one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits as
+// Sampler::sample does and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in
+// tokens[0] (greedy = true; the generator is not read).  Otherwise the generator is written back after fed returns.
 // ---------------------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
+template <class Fed> __device__ __forceinline__ void sample_body(const SampleArgs &a, const SampleCtx &c, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
     __shared__ MtState mt;
     __shared__ unsigned hist[256];
     __shared__ unsigned long long sh_prefix;
     __shared__ int sh_need, sh_done, sh_n;
     __shared__ float red;
-    const SampleCtx &c = a.c[blockIdx.x];
     const int tid = threadIdx.x, n = a.n_vocab;
     if (a.temp <= 0.f) {
-        if (tid == 0) {
-            c.ids[a.step] = c.state->tokens[0];
-            if (c.slot) c.slot->n_past = c.n_past0 + a.step;
-        }
+        if (tid == 0) fed(c.state->tokens[0], true);
         return;
     }
     for (int i = tid; i < kMtN; i += blockDim.x) mt.x[i] = c.mt->x[i];
@@ -395,14 +391,105 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
             }
             idx = first;
         }
-        const int id = c.id[idx];
-        c.state->tokens[0] = id;
-        c.ids[a.step] = id;
-        if (c.slot) c.slot->n_past = c.n_past0 + a.step;
+        fed(c.id[idx], false);
     }
     __syncthreads();
     for (int i = tid; i < kMtN; i += blockDim.x) c.mt->x[i] = mt.x[i];
     if (tid == 0) c.mt->p = mt.p;
+}
+
+// the id a step feeds: into tokens[0] (the greedy id is already there) and ids[step]; a batched column moves to its next position
+__device__ __forceinline__ void feed(const SampleArgs &a, const SampleCtx &c, int id, bool greedy) {
+    if (!greedy) c.state->tokens[0] = id;
+    c.ids[a.step] = id;
+    if (c.slot) c.slot->n_past = c.n_past0 + a.step;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits, writes the id into tokens[0] and
+// ids[step], and moves a batched column to its next position.
+// ---------------------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    sample_body(a, c, [&](int id, bool greedy) { feed(a, c, id, greedy); });
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// stop on the reply's text (minigpt4_b200_sample_until; host side LlamaDevice::sample_until): the reference's chat loop
+// (MiniGPT4ChatBot.generate) appends each token's text to the reply and stops after a token that is not exactly "##" once the reply
+// ends with "###".  The text of an id is the C string of Engine::id_to_token, from the group's token table.
+// ---------------------------------------------------------------------------------------------------------------------------------
+constexpr int kStopMax = LlamaDevice::kStopMax;   // longest stop text; the reply's last kStopMax bytes decide every later check
+
+struct TokenTable { const int *off; const unsigned char *bytes; };   // id's text: bytes[off[id], off[id + 1])
+
+struct ReplyState {                  // one context's stop state in a call (the host writes it before the first step)
+    unsigned char tail[kStopMax];    // the reply's last tail_len bytes
+    unsigned char stop[kStopMax];
+    int tail_len, stop_len;          // stop_len 0: no text stop
+    int done;                        // 0 running; 1 stopped at the previous step; 2 stopped, logits and state in the snapshot
+    int n_fed;                       // steps that fed an id
+    DeviceState snap;
+};
+
+// the reply takes id's text; returns true if that step ends it.  One thread; no local arrays.
+__device__ __forceinline__ bool reply_take(ReplyState &r, TokenTable t, int id) {
+    const unsigned char *piece = t.bytes + t.off[id];
+    const int len = t.off[id + 1] - t.off[id], tl = r.tail_len;
+    bool stop = r.stop_len > 0 && !(len == 2 && piece[0] == '#' && piece[1] == '#') && tl + len >= r.stop_len;
+    for (int k = 0; stop && k < r.stop_len; ++k) {   // byte k from the end of tail + piece
+        const unsigned char b = k < len ? piece[len - 1 - k] : r.tail[tl - 1 - (k - len)];
+        stop = b == r.stop[r.stop_len - 1 - k];
+    }
+    if (len >= kStopMax) {
+        for (int k = 0; k < kStopMax; ++k) r.tail[k] = piece[len - kStopMax + k];
+        r.tail_len = kStopMax;
+    } else {
+        const int keep = min(tl, kStopMax - len);
+        for (int k = 0; k < keep; ++k) r.tail[k] = r.tail[tl - keep + k];
+        for (int k = 0; k < len; ++k) r.tail[keep + k] = piece[k];
+        r.tail_len = keep + len;
+    }
+    return stop;
+}
+
+struct StopArgs {
+    ReplyState *r[8];
+    float *snap[8];   // [n_vocab] each context's logits after its last step
+    TokenTable tab;
+};
+
+// one step of sample_kernel that stops each context on its reply's text.  A stopped context does not draw (its generator stays); at
+// the next step it saves its logits and DeviceState, which the host restores at the end of the call, and later steps only keep its
+// batched column moving, so the decode work that still runs for it writes K/V above its final position.
+__global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs a, const StopArgs s) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (threadIdx.x == 0) sh_state = r.done;   // (read once: thread 0 writes r.done below)
+    __syncthreads();
+    const int done = sh_state;
+    if (done != 0) {
+        if (done == 1) {
+            float *snap = s.snap[blockIdx.x];
+            for (int i = threadIdx.x; i < a.n_vocab; i += blockDim.x) snap[i] = c.logits[i];
+            if (threadIdx.x == 0) { r.snap = *c.state; r.done = 2; }
+        }
+        if (threadIdx.x == 0 && c.slot) c.slot->n_past = c.n_past0 + a.step;
+        return;
+    }
+    sample_body(a, c, [&](int id, bool greedy) {
+        feed(a, c, id, greedy);
+        r.n_fed = a.step + 1;
+        if (reply_take(r, s.tab, id)) r.done = 1;
+    });
+}
+
+// seam: reply_take over ids[0, n) from r's tail; *stop_at = the index of the id that ends the reply, -1 if none does
+__global__ void reply_check_kernel(ReplyState *r, TokenTable t, const int *ids, int n, int *stop_at) {
+    int at = -1;
+    for (int i = 0; i < n && at < 0; ++i) if (reply_take(*r, t, ids[i])) at = i;
+    *stop_at = at;
 }
 
 }  // namespace smp

@@ -222,6 +222,7 @@ _EXT = {
     "minigpt4_b200_flush_batch": ([_VP, _I], _I),
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
@@ -236,6 +237,7 @@ _EXT = {
     "minigpt4_b200_host_sample": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _F, _F, _I, _VP], _I),
     "minigpt4_b200_op_sample": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _VP], _I),
     "minigpt4_b200_op_sample_timed": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_op_reply_stop": ([_CTX, _VP, _I, _S, _S, C.POINTER(C.c_int32)], _I),
     "minigpt4_b200_op_check_libm": ([_I, C.c_uint32, C.c_uint32, C.POINTER(C.c_longlong)], _I),
     "minigpt4_b200_host_inspect_container": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
     "minigpt4_b200_host_inspect_ggjt": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
@@ -363,6 +365,19 @@ class B200:
                                                     _ptr(ids), C.byref(ms)))
         return ids[:steps, :n], ms.value
 
+    def sample_until(self, ctxs, max_steps: int, stop: str | bytes | None = None, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
+                     tfs_z: float = 1.0, typical_p: float = 1.0) -> tuple[list[list[int]], list[bool], float]:
+        """device-sampled steps of every context in `ctxs` (1..8 of one group), each until its reply ends with `stop` (None: "###"; "": never)
+        or max_steps; returns each context's fed ids, whether the stop text ended it, and the device ms"""
+        n = len(ctxs)
+        ids = np.zeros((max(1, max_steps), max(1, n)), np.int32)
+        n_out, stopped = np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.int32)
+        ms = C.c_float(0)
+        st = stop.encode() if isinstance(stop, str) else stop
+        self._chk(self.L.minigpt4_b200_sample_until(C.cast(self._ctx_array(ctxs), C.c_void_p), n, max_steps, st, temp, top_k, top_p, tfs_z,
+                                                    typical_p, _ptr(ids), _ptr(n_out), _ptr(stopped), C.byref(ms)))
+        return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
     def time_matvec(self, ctx, kind: int, reps: int = 3) -> tuple[float, float]:
         ms, nb = C.c_float(0), C.c_double(0)
         self._chk(self.L.minigpt4_b200_time_matvec(ctx.ptr, kind, reps, C.byref(ms), C.byref(nb)))
@@ -432,6 +447,15 @@ class B200:
         ms = C.c_float(0)
         self._chk(self.L.minigpt4_b200_op_sample_timed(_ptr(lg), lg.size, seed, temp, top_k, top_p, tfs_z, typical_p, n_draws, _ptr(out), C.byref(ms)))
         return (out, ms.value) if timed else out
+
+    def op_reply_stop(self, ctx, ids, stop: str | bytes | None = None, tail: str | bytes = b"") -> int:
+        """sample_until's stop rule on the device over `ids` from a reply ending with `tail`: the index of the id that ends the reply, -1 if none"""
+        a = np.ascontiguousarray(ids, np.int32)
+        at = C.c_int32(0)
+        st = stop.encode() if isinstance(stop, str) else stop
+        tl = tail.encode() if isinstance(tail, str) else tail
+        self._chk(self.L.minigpt4_b200_op_reply_stop(ctx.ptr, _ptr(a), a.size, st, tl, C.byref(at)))
+        return at.value
 
     def op_check_libm(self, fn: int, lo_bits: int, hi_bits: int) -> int:
         """device expf (fn 0) / logf (fn 1) against the host libm over the float bit patterns lo_bits..hi_bits; returns the mismatches"""
@@ -535,6 +559,32 @@ class MiniGPT4ChatBot:
             if self.library.minigpt4_is_eos(chat):
                 break
             yield token
+
+    def generate_on_device(self, message: str, limit: int = 1024, chunk: int = 16, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
+                           tfs_z: float = 1.0, typical_p: float = 1.0):
+        """generate() with the sampling and the stop check on the GPU: minigpt4_b200_sample_until calls of up to `chunk` steps, each
+        stopping where generate()'s loop stops (mirostat 0; the repetition arguments, which generate() passes on unused, are not taken).
+        Yields what generate() yields for the same seed: no "##" token, and not the token that completes "###".
+
+        One difference cannot be avoided: generate() decodes each token's bytes with errors="ignore" before it appends and checks them,
+        so a piece that is not valid UTF-8 on its own drops out of its reply text, while the device compares the bytes.  The two can
+        disagree only where such a piece sits inside or next to the stop text."""
+        if self.is_image_chat:
+            self.is_image_chat = False
+            self.library.minigpt4_begin_chat_image(self.ctx, self.embedding, message, self.n_threads)
+        else:
+            self.library.minigpt4_begin_chat(self.ctx, message, self.n_threads)
+        ext = B200(self.library)
+        done = 0
+        while done < limit:
+            ids, stopped, _ = ext.sample_until([self.ctx], min(chunk, limit - done), None, temp, top_k, top_p, tfs_z, typical_p)
+            done += len(ids[0])
+            for k, t in enumerate(ids[0]):
+                if stopped[0] and k == len(ids[0]) - 1:
+                    return
+                token = ext.L.minigpt4_b200_token_text(self.ctx.ptr, t).decode("utf-8", errors="ignore")
+                if not self.library.minigpt4_contains_eos_token(token):
+                    yield token
 
     def reset_chat(self):
         self.is_image_chat = False
