@@ -85,7 +85,7 @@ MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int
                                               float alpha_frequency, int mirostat, float mirostat_tau, float mirostat_eta, int penalize_nl);
 /* `steps` sampled decode steps of n (1..8) distinct contexts of one group with no return to the host in between: each step samples
  * every context's logits on the device with the chain of minigpt4_end_chat (top_k, tail_free, typical, top_p, temperature, draw;
- * no mirostat) and its own generator, then feeds the n ids in one decode step (n = 1: the context's own decode graph or megakernel;
+ * mirostat: minigpt4_b200_sample_steps_mirostat) and its own generator, then feeds the n ids in one decode step (n = 1: the context's own decode graph or megakernel;
  * n >= 2: the batched step of minigpt4_b200_decode_batch).  Queued prompt pieces are evaluated first, as in end_chat_batch.
  * Afterwards every context is where `steps` calls of minigpt4_end_chat (n = 1) or minigpt4_b200_end_chat_batch (n >= 2) with these
  * parameters leave it: n_past, KV cache, logits, greedy id and the generator, which a later minigpt4_end_chat continues.
@@ -119,6 +119,17 @@ MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n
 MINIGPT4_API int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
                                             float top_p, float tfs_z, float typical_p, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
                                             float *ms_out);
+/* minigpt4_b200_sample_steps and minigpt4_b200_sample_until with the mirostat sampling of minigpt4_end_chat (mirostat 1 or 2,
+ * mirostat_tau, mirostat_eta; as there, top_k, top_p, tfs_z and typical_p do not apply).  Every step sorts the whole vocabulary.
+ * Each context keeps its own μ per mirostat mode, set to 2 mirostat_tau at the mode's first use by end_chat or these calls, whichever
+ * comes first: afterwards a context is also where that many end_chat / end_chat_batch calls leave its μ, which a later end_chat
+ * continues.  temp <= 0 is greedy, and neither μ nor the generator is touched.  Arguments, results and refusals are those of the
+ * non-mirostat call; mirostat outside 1..2 also returns 8 before any device work. */
+MINIGPT4_API int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int mirostat,
+                                                     float mirostat_tau, float mirostat_eta, int32_t *ids_out, float *ms_out);
+MINIGPT4_API int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp,
+                                                     int mirostat, float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out,
+                                                     int32_t *stopped, float *ms_out);
 
 /* batch encode (config 5): n images -> n embeddings, same semantics per image as minigpt4_encode_image */
 MINIGPT4_API int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, IN struct MiniGPT4Images *images, OUT struct MiniGPT4Embeddings *embeddings);
@@ -162,8 +173,8 @@ MINIGPT4_API int minigpt4_b200_host_tokenize(const char *llm_model, const char *
 /* run the sampler chain of minigpt4_end_chat on caller-provided logits (reference minigpt4.cpp:2425-2483) */
 MINIGPT4_API int minigpt4_b200_host_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
                                            float typical_p, int mirostat, float mirostat_tau, float mirostat_eta, int n_draws, int32_t *out_ids);
-/* the device twin of minigpt4_b200_host_sample (no mirostat, temp > 0): n_draws draws over the same logits from one generator
- * seeded with `seed`, through the kernel of minigpt4_b200_sample_steps; 8 for bad arguments.  The _timed form also returns the
+/* the device twin of minigpt4_b200_host_sample (no mirostat, which minigpt4_b200_op_sample_mirostat covers; temp > 0): n_draws draws
+ * over the same logits from one generator seeded with `seed`, through the kernel of minigpt4_b200_sample_steps; 8 for bad arguments.  The _timed form also returns the
  * average CUDA-event time of one sampling launch. */
 MINIGPT4_API int minigpt4_b200_op_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z,
                                          float typical_p, int n_draws, int32_t *out_ids);
@@ -172,11 +183,21 @@ MINIGPT4_API int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab,
 /* minigpt4_b200_sample_until's stop rule on the device, over the ids ids[0..n) of ctx's vocabulary from a reply that ends with `tail`
  * (NULL: empty; its last 32 bytes count): *stop_at = the index of the id after which the reply ends, -1 if none; stop as in
  * sample_until.  Changes nothing in ctx.  8 for a NULL ctx / stop_at, an id outside the vocabulary or a stop text over 32 bytes. */
+/* mirostat (1 or 2) over the same logits from one generator seeded with `seed` and an unset μ: n_draws calls of the host Sampler
+ * (on_device 0) or launches of minigpt4_b200_sample_steps_mirostat's kernel (on_device 1, temp > 0); ids_out[d] = draw d's id and
+ * mu_out[d] = μ after it; *kernel_ms (may be NULL) = the average CUDA-event time of one launch (0 on the host).  8 for NULL
+ * logits / ids_out / mu_out, n_vocab < 1, n_draws < 1, mirostat outside 1..2, on_device outside 0..1, or temp <= 0 on the device. */
+MINIGPT4_API int minigpt4_b200_op_sample_mirostat(const float *logits, int n_vocab, int seed, float temp, int mirostat, float mirostat_tau,
+                                                  float mirostat_eta, int n_draws, int on_device, int32_t *ids_out, float *mu_out, float *kernel_ms);
 MINIGPT4_API int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail,
                                              int32_t *stop_at);
 /* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with
  * the host libm's; *mismatches = the number that differ */
 MINIGPT4_API int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches);
+/* the same for mirostat's log2f over the bit patterns lo_bits .. hi_bits, and its powf(x, y) over the y of those bit patterns; 8 for
+ * hi_bits < lo_bits or a NULL mismatches */
+MINIGPT4_API int minigpt4_b200_op_check_log2f(uint32_t lo_bits, uint32_t hi_bits, long long *mismatches);
+MINIGPT4_API int minigpt4_b200_op_check_powf(float x, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches);
 /* block quantiser behind minigpt4_quantize_model (ggml quantize_row_*_reference): n floats (n % 32 == 0) -> ggml blocks of
  * `ggml_type` (2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0); returns the bytes written, -1 for an unsupported type or ragged n */
 MINIGPT4_API long minigpt4_b200_host_quantize_row(int ggml_type, const float *x, long n, void *out_blocks);

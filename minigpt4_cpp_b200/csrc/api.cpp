@@ -241,6 +241,18 @@ int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_ste
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out,
                                 n_out, stopped, ms_out);
 }
+int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int mirostat, float mirostat_tau,
+                                        float mirostat_eta, int32_t *ids_out, float *ms_out) {
+    if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
+    return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta},
+                                ids_out, ms_out);
+}
+int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int mirostat,
+                                        float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out) {
+    if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop,
+                                SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, ids_out, n_out, stopped, ms_out);
+}
 int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, struct MiniGPT4Images *images, struct MiniGPT4Embeddings *embeddings) {
     if (embeddings->n_embeddings < images->n_images) return ErrImageSize;
     return E(ctx)->encode_images(images->images, images->n_images, embeddings->embeddings, nullptr);
@@ -316,26 +328,50 @@ int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab, int seed, fl
     LlamaDevice::test_sample(logits, n_vocab, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, rng, n_draws, out_ids, kernel_ms);
     return 0;
 }
+int minigpt4_b200_op_sample_mirostat(const float *logits, int n_vocab, int seed, float temp, int mirostat, float mirostat_tau, float mirostat_eta,
+                                     int n_draws, int on_device, int32_t *ids_out, float *mu_out, float *kernel_ms) {
+    if (!logits || !ids_out || !mu_out || n_vocab < 1 || n_draws < 1 || (mirostat != 1 && mirostat != 2) || (on_device != 0 && on_device != 1))
+        return ErrFailedToAddString;
+    if (!on_device) {
+        Sampler s(seed);
+        const SamplingParams sp{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta};
+        for (int d = 0; d < n_draws; ++d) {
+            ids_out[d] = s.sample(logits, n_vocab, sp);
+            float mu[2]; bool init[2];
+            s.get_mu(mu, init);
+            mu_out[d] = mu[mirostat - 1];
+        }
+        if (kernel_ms) *kernel_ms = 0.f;
+        return 0;
+    }
+    if (!(temp > 0.f)) return ErrFailedToAddString;   // greedy: not the sampler
+    uint32_t rng[625];
+    Sampler(seed).get_rng(rng);
+    LlamaDevice::test_sample(logits, n_vocab, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, rng, n_draws, ids_out, kernel_ms,
+                             mu_out);
+    return 0;
+}
 int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at) {
     if (!ctx) return ErrFailedToAddString;
     return E(ctx)->reply_stop(ids, n, stop, tail, stop_at);
 }
-int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) {
-    if ((fn != 0 && fn != 1) || hi_bits < lo_bits || !mismatches) return ErrFailedToAddString;
+// the device libm twin fn (LlamaDevice::test_libm) against the host's libm over the float bit patterns lo_bits .. hi_bits, bit for bit
+static int check_libm(int fn, float x, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) {
+    if (hi_bits < lo_bits || !mismatches) return ErrFailedToAddString;
     const uint64_t total = (uint64_t)hi_bits - lo_bits + 1, chunk = (uint64_t)1 << 26;
     std::vector<float> dev((size_t)std::min(total, chunk));
     const unsigned nt = std::max(1u, std::min(64u, std::thread::hardware_concurrency()));
     long long bad = 0;
     for (uint64_t base = 0; base < total; base += chunk) {
         const uint32_t lo = (uint32_t)(lo_bits + base), c = (uint32_t)std::min(chunk, total - base);
-        LlamaDevice::test_libm(fn, lo, c, dev.data());
+        LlamaDevice::test_libm(fn, lo, c, dev.data(), x);
         std::vector<long long> part(nt, 0);
         std::vector<std::thread> th;
         for (unsigned t = 0; t < nt; ++t) th.emplace_back([&, t] {
             long long m = 0;
             for (uint32_t i = (uint32_t)((uint64_t)c * t / nt); i < (uint32_t)((uint64_t)c * (t + 1) / nt); ++i) {
-                float x; const uint32_t u = lo + i; memcpy(&x, &u, 4);
-                const float h = fn == 0 ? expf(x) : logf(x);
+                float v; const uint32_t u = lo + i; memcpy(&v, &u, 4);
+                const float h = fn == 0 ? expf(v) : fn == 1 ? logf(v) : fn == 2 ? log2f(v) : powf(x, v);
                 if (memcmp(&h, &dev[i], 4) != 0) ++m;
             }
             part[t] = m;
@@ -346,6 +382,12 @@ int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long
     *mismatches = bad;
     return 0;
 }
+int minigpt4_b200_op_check_libm(int fn, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) {
+    if (fn != 0 && fn != 1) return ErrFailedToAddString;
+    return check_libm(fn, 0.f, lo_bits, hi_bits, mismatches);
+}
+int minigpt4_b200_op_check_log2f(uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) { return check_libm(2, 0.f, lo_bits, hi_bits, mismatches); }
+int minigpt4_b200_op_check_powf(float x, uint32_t lo_bits, uint32_t hi_bits, long long *mismatches) { return check_libm(3, x, lo_bits, hi_bits, mismatches); }
 int minigpt4_b200_host_inspect_container(const char *path, int *n_models, int *n_tensors, int *n_embd_llm) {
     VisionFile f;
     if (Error e = f.load(path)) return e;

@@ -126,6 +126,20 @@ Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const
     for (int i = 0; i < n; ++i) e[i]->reply_take(tokens[i]);
     return err;
 }
+// a sampler's generator and mirostat μ, to and from the device sampler's form
+static void sampler_state(const Sampler &s, uint32_t rng[625], MirostatState &mu) {
+    bool init[2];
+    s.get_rng(rng);
+    s.get_mu(mu.mu, init);
+    mu.init[0] = init[0]; mu.init[1] = init[1];
+}
+static void set_sampler_state(Sampler &s, const SamplingArgs &p, const uint32_t rng[625], const MirostatState &mu) {
+    if (p.temp <= 0.f) return;   // greedy: neither was touched
+    s.set_rng(rng);
+    const bool init[2] = {mu.init[0] != 0, mu.init[1] != 0};
+    if (p.mirostat) s.set_mu(mu.mu, init);
+}
+
 Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out) {
     if (!ids_out || !group_valid(e, n, "sample_steps")) return ErrFailedToAddString;
     if (steps < 1) { MG4_ERR("sample_steps: %d steps", steps); return ErrFailedToAddString; }
@@ -135,11 +149,11 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
         if (e[i]->n_past_ + steps > n_ctx) { MG4_ERR("sample_steps: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, steps, n_ctx); return ErrFailedToAddString; }
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
-    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625];
-    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; e[i]->sampler_->get_rng(rng[i]); }
-    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, ids_out);
+    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; MirostatState mu[8];
+    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); }
+    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out);
     for (int i = 0; i < n; ++i) {
-        if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]);
+        set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += steps;
         for (int t = 0; t < steps; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
     }
@@ -159,11 +173,11 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
     e[0]->ensure_token_table();
-    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; std::string tail[8];
-    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; e[i]->sampler_->get_rng(rng[i]); tail[i] = e[i]->reply_; }
-    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, st, tail, ids_out, n_out, stopped);
+    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; MirostatState mu[8]; std::string tail[8];
+    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
+    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped);
     for (int i = 0; i < n; ++i) {
-        if (p.temp > 0.f) e[i]->sampler_->set_rng(rng[i]);
+        set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += n_out[i];
         for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
     }

@@ -29,7 +29,7 @@ public:
     // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
     static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
     // `steps` decode steps of n (1..8) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
-    // own generator (see minigpt4_b200_sample_steps); ids_out[s * n + i]; all or nothing
+    // own generator and mirostat μ (see minigpt4_b200_sample_steps / _mirostat); ids_out[s * n + i]; all or nothing
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
     // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
     // "###"; all or nothing

@@ -45,15 +45,17 @@ struct LlamaGroup {
     }
 };
 
-// device sampler (llama_sample.cuh): a context's generator state, candidate scratch and the ids of a call, in one allocation; the
-// generator state and the ids go through pinned staging
+// device sampler (llama_sample.cuh): a context's generator state and mirostat μ, candidate scratch and the ids of a call, in one
+// allocation; the generator state and μ (one copy: μ follows the generator) and the ids go through pinned staging
 struct SamplerScratch {
     void *dev = nullptr;
     smp::MtState *mt = nullptr;
+    MirostatState *mu = nullptr;   // right after the generator (smp::mirostat_state), in the padding before the ids
     int *ids = nullptr, *id = nullptr;
     unsigned long long *keys = nullptr;
     float *logit = nullptr, *p = nullptr, *aux = nullptr;
-    uint32_t *h_rng = nullptr;   // [625] pinned
+    uint32_t *h_rng = nullptr;   // [625] pinned, then h_mu
+    MirostatState *h_mu = nullptr;
     int32_t *h_ids = nullptr;    // [n_ids] pinned
     size_t bytes = 0;
     SamplerScratch(int n_vocab, int n_ids) {
@@ -62,9 +64,11 @@ struct SamplerScratch {
         bytes = o_id + 4 * V * 4;
         CUDA_CHECK(cudaMalloc(&dev, bytes));
         unsigned char *b = (unsigned char *)dev;
-        mt = (smp::MtState *)b; ids = (int *)(b + o_ids); keys = (unsigned long long *)(b + o_keys);
+        static_assert(sizeof(smp::MtState) == 625 * 4 && sizeof(smp::MtState) + sizeof(MirostatState) <= (sizeof(smp::MtState) + 255) / 256 * 256, "μ fits before the ids");
+        mt = (smp::MtState *)b; mu = (MirostatState *)(b + sizeof(smp::MtState)); ids = (int *)(b + o_ids); keys = (unsigned long long *)(b + o_keys);
         id = (int *)(b + o_id); logit = (float *)(b + o_id + V * 4); p = (float *)(b + o_id + 2 * V * 4); aux = (float *)(b + o_id + 3 * V * 4);
-        CUDA_CHECK(cudaHostAlloc((void **)&h_rng, 625 * 4, cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_rng, 625 * 4 + sizeof(MirostatState), cudaHostAllocDefault));
+        h_mu = (MirostatState *)(h_rng + 625);
         CUDA_CHECK(cudaHostAlloc((void **)&h_ids, (size_t)n_ids * 4, cudaHostAllocDefault));
     }
     ~SamplerScratch() { if (dev) cudaFree(dev); if (h_rng) cudaFreeHost(h_rng); if (h_ids) cudaFreeHost(h_ids); }
@@ -1091,8 +1095,16 @@ static smp::SampleArgs sample_args(const SamplingArgs &p, int n_vocab) {
     a.n_vocab = n_vocab; a.top_k = p.top_k; a.temp = p.temp; a.top_p = p.top_p; a.tfs_z = p.tfs_z; a.typical_p = p.typical_p;
     return a;
 }
+static smp::MirostatArgs mirostat_args(const SamplingArgs &p) {
+    smp::MirostatArgs m{};
+    m.mode = p.mirostat; m.tau = p.mirostat_tau; m.eta = p.mirostat_eta;
+    return m;
+}
+// the bytes of a context's sampler state that a call moves: the generator, and μ after it with mirostat
+static size_t sampler_state_bytes(const SamplingArgs &p) { return 625 * 4 + (p.mirostat ? sizeof(MirostatState) : 0); }
 
-cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], smp::SampleArgs &a) {
+cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
+                                         smp::SampleArgs &a) {
     LlamaDevice &L0 = *c[0];
     a = sample_args(p, L0.d_.n_vocab);
     cudaStream_t s = L0.stream_;
@@ -1110,7 +1122,8 @@ cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int
         a.c[i] = L.smp_->ctx(L.logits_, L.state_, slot, n_past[i]);
         if (p.temp > 0.f) {
             memcpy(L.smp_->h_rng, rng[i], 625 * 4);
-            CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, 625 * 4, cudaMemcpyHostToDevice, s));
+            if (p.mirostat) *L.smp_->h_mu = mu[i];
+            CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, sampler_state_bytes(p), cudaMemcpyHostToDevice, s));
         }
     }
     if (n >= 2) {
@@ -1134,14 +1147,16 @@ void LlamaDevice::sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaS
     }
 }
 
-// after `steps` steps: the fed ids and generators to the host, one synchronisation; returns the device ms since ev0_
-float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, bool sampled, uint32_t (*rng)[625], int32_t *ids_out, cudaStream_t s) {
+// after `steps` steps: the fed ids, generators and μ to the host, one synchronisation; returns the device ms since ev0_
+float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
+                                cudaStream_t s) {
     LlamaDevice &L0 = *c[0];
+    const bool sampled = p.temp > 0.f;
     CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_ids, L.smp_->ids, (size_t)steps * 4, cudaMemcpyDeviceToHost, s));
-        if (sampled) CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_rng, L.smp_->mt, 625 * 4, cudaMemcpyDeviceToHost, s));
+        if (sampled) CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_rng, L.smp_->mt, sampler_state_bytes(p), cudaMemcpyDeviceToHost, s));
     }
     if (n == 1) L0.sync_decode();
     else {
@@ -1153,20 +1168,24 @@ float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, bool sa
         LlamaDevice &L = *c[i];
         for (int t = 0; t < steps; ++t) ids_out[(size_t)t * n + i] = L.smp_->h_ids[t];
         if (sampled) memcpy(rng[i], L.smp_->h_rng, 625 * 4);
+        if (sampled && p.mirostat) mu[i] = *L.smp_->h_mu;
     }
     return ms;
 }
 
-float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out) {
+float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
+                                MirostatState *mu, int32_t *ids_out) {
     smp::SampleArgs a;
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, a);
+    const smp::MirostatArgs m = mirostat_args(p);
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
     CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
     for (int t = 0; t < steps; ++t) {
         a.step = t;
-        smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
+        if (p.mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a, m);
+        else smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
         sampled_decode(c, n, n_past[0] + t, s);
     }
-    return end_sampling(c, n, steps, p.temp > 0.f, rng, ids_out, s);
+    return end_sampling(c, n, steps, p, rng, mu, ids_out, s);
 }
 
 void LlamaDevice::ensure_reply() {
@@ -1198,10 +1217,11 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
 }
 
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                                const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped) {
+                                MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped) {
     LlamaDevice &L0 = *c[0];
     smp::SampleArgs a;
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, a);
+    const smp::MirostatArgs m = mirostat_args(p);
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
     smp::StopArgs sa{};
     sa.tab = L0.group_->tokens;
     for (int i = 0; i < n; ++i) {
@@ -1223,7 +1243,8 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         }
         for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
             a.step = issued;
-            smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
+            if (p.mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, m);
+            else smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
             sampled_decode(c, n, n_past[0] + issued, s);
         }
         for (int i = 0; i < n; ++i)
@@ -1232,7 +1253,7 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
     }
     for (int i = 0; i < n; ++i)
         CUDA_CHECK(cudaMemcpyAsync(c[i]->reply_->h_r, c[i]->reply_->r, sizeof(smp::ReplyState), cudaMemcpyDeviceToHost, s));
-    const float ms = end_sampling(c, n, issued, p.temp > 0.f, rng, ids_out, s);
+    const float ms = end_sampling(c, n, issued, p, rng, mu, ids_out, s);
     // a context that stopped before the last issued step gets back what its stopping step left
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
@@ -1270,31 +1291,43 @@ int LlamaDevice::test_reply_stop(const int32_t *ids, int n, const std::string &s
     return at;
 }
 
-void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms) {
+void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms,
+                              float *mu_out) {
     SamplerScratch ss(n_vocab, n_draws);
-    float *lg = nullptr; DeviceState *st = nullptr;
+    float *lg = nullptr, *mu_d = nullptr; DeviceState *st = nullptr;
     CUDA_CHECK(cudaMalloc((void **)&lg, (size_t)n_vocab * 4));
     CUDA_CHECK(cudaMalloc((void **)&st, sizeof(DeviceState))); CUDA_CHECK(cudaMemset(st, 0, sizeof(DeviceState)));
     CUDA_CHECK(cudaMemcpy(lg, logits, (size_t)n_vocab * 4, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemcpy(ss.mt, rng, 625 * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemset(ss.mu, 0, sizeof(MirostatState)));
+    if (mu_out && p.mirostat) CUDA_CHECK(cudaMalloc((void **)&mu_d, (size_t)n_draws * 4));
     smp::SampleArgs a = sample_args(p, n_vocab);
     a.c[0] = ss.ctx(lg, st, nullptr, 0);
+    const smp::MirostatArgs m = mirostat_args(p);
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     CUDA_CHECK(cudaEventRecord(e0, 0));
-    for (int i = 0; i < n_draws; ++i) { a.step = i; smp::sample_kernel<<<1, smp::kThreads>>>(a); CUDA_CHECK(cudaGetLastError()); }
+    for (int i = 0; i < n_draws; ++i) {
+        a.step = i;
+        if (p.mirostat) smp::sample_mirostat_kernel<<<1, smp::kThreads>>>(a, m);
+        else smp::sample_kernel<<<1, smp::kThreads>>>(a);
+        CUDA_CHECK(cudaGetLastError());
+        if (mu_d) CUDA_CHECK(cudaMemcpyAsync(mu_d + i, &ss.mu->mu[p.mirostat - 1], 4, cudaMemcpyDeviceToDevice, 0));
+    }
     CUDA_CHECK(cudaEventRecord(e1, 0));
     CUDA_CHECK(cudaDeviceSynchronize());
     float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
     if (kernel_ms) *kernel_ms = n_draws > 0 ? ms / (float)n_draws : 0.f;
     CUDA_CHECK(cudaMemcpy(out, ss.ids, (size_t)n_draws * 4, cudaMemcpyDeviceToHost));
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(lg); cudaFree(st);
+    if (mu_d) CUDA_CHECK(cudaMemcpy(mu_out, mu_d, (size_t)n_draws * 4, cudaMemcpyDeviceToHost));
+    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(lg); cudaFree(st); cudaFree(mu_d);
 }
 
-void LlamaDevice::test_libm(int fn, uint32_t lo, uint32_t n, float *out_host) {
+void LlamaDevice::test_libm(int fn, uint32_t lo, uint32_t n, float *out_host, float x) {
     float *d = nullptr;
     CUDA_CHECK(cudaMalloc((void **)&d, (size_t)n * 4));
-    smp::libm_kernel<<<1024, 256>>>(fn, lo, n, d);
+    if (fn <= 1) smp::libm_kernel<<<1024, 256>>>(fn, lo, n, d);
+    else smp::mirostat_libm_kernel<<<1024, 256>>>(fn - 2, x, lo, n, d);
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaMemcpy(out_host, d, (size_t)n * 4, cudaMemcpyDeviceToHost));
     cudaFree(d);

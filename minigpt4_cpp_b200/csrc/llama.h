@@ -52,7 +52,9 @@ struct SessionSlot {   // one column of a batched decode step (device table of t
     DeviceState *state;
 };
 
-struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; };   // the non-mirostat chain of Sampler::sample
+// Sampler::sample's arguments: the non-mirostat chain, or mirostat 1 / 2 (which ignores top_k .. typical_p); mirostat 0: the chain
+struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; int mirostat; float mirostat_tau, mirostat_eta; };
+struct MirostatState { float mu[2]; int init[2]; };   // a context's mirostat μ of v1 / v2 and whether each is set (Sampler::get_mu)
 struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
 struct ReplyScratch;   // a context's stop state in sample_until: reply tail, stop text, done flag, snapshot (llama.cu, llama_sample.cuh)
 namespace smp { struct SampleArgs; }
@@ -85,19 +87,21 @@ public:
     // `steps` sampled decode steps of n (1..8) distinct contexts of one group with no host round trip: each step samples every context's
     // current logits on the device (llama_sample.cuh; p.temp <= 0: the greedy id) into its DeviceState, then runs the decode step (n = 1:
     // the context's own graph or megakernel; n >= 2: the batch graph, every column fed its DeviceState::tokens[0]).  rng[i] holds context
-    // i's mt19937 state (624 words and the position) on entry and on return; ids_out[s * n + i] is the id context i was fed at step s.
+    // i's mt19937 state (624 words and the position) on entry and on return, and with p.mirostat 1 / 2 mu[i] its mirostat μ (mu may be
+    // null without mirostat); ids_out[s * n + i] is the id context i was fed at step s.
     // One synchronisation at the end; returns the device ms of the steps.  The caller validates (distinct, one group, room for steps).
-    static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], int32_t *ids_out);
+    static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
+                              MirostatState *mu, int32_t *ids_out);
     // sample_steps that stops each context after the step whose id's text (not exactly "##") makes its reply end with `stop` (0..32
     // bytes, "" no text stop), or after max_steps.  tail[i]: context i's reply so far (its last 32 bytes decide).  The steps are issued
     // kReplyChunk at a time; the host waits for chunk j - 1's done flags before it issues chunk j + 1 and stops issuing once every
     // context is done, so at most 2 kReplyChunk - 1 steps run past the last stop.  Afterwards context i holds what n_out[i] steps left
-    // (logits, DeviceState, arg-max; rng[i]), and ids_out[s * n + i] = -1 for s >= n_out[i]; stopped[i] = the text ended it.  Needs the
-    // group's token table (set_token_table).  One wait per chunk, none of them stalling the device; returns the device ms.
+    // (logits, DeviceState, arg-max; rng[i], mu[i]), and ids_out[s * n + i] = -1 for s >= n_out[i]; stopped[i] = the text ended it.  Needs
+    // the group's token table (set_token_table).  One wait per chunk, none of them stalling the device; returns the device ms.
     static constexpr int kReplyChunk = 4;
     static constexpr int kStopMax = 32;   // longest stop text
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                              const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped);
+                              MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped);
     // the group's device table of every id's text (off: n_vocab + 1 offsets into bytes), counted in shared_bytes
     bool has_token_table() const;
     void set_token_table(const std::vector<int> &off, const std::string &bytes);
@@ -137,10 +141,12 @@ public:
     // repack + matvec kernels the engine uses.
     static void test_matvec(int gg, int rows, int cols, const void *w_host, const float *x_host, int n, float *y_host);
     // sampler test hook: n_draws draws from one generator (rng: 624 words and the position) over the same n_vocab logits, as n_draws calls
-    // of Sampler::sample make (p.temp > 0); kernel_ms (optional): the average CUDA-event time of one sampling launch
-    static void test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms);
-    // the device expf (fn 0) / logf (fn 1) of the float bit patterns lo .. lo + n - 1
-    static void test_libm(int fn, uint32_t lo, uint32_t n, float *out_host);
+    // of Sampler::sample make (p.temp > 0); kernel_ms (optional): the average CUDA-event time of one sampling launch.  With p.mirostat
+    // 1 / 2, μ starts unset and mu_out (optional) takes μ after each draw (a 4-byte device copy after each launch, inside the timing).
+    static void test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms,
+                            float *mu_out = nullptr);
+    // the device expf (fn 0) / logf (fn 1) / log2f (fn 2) of the float bit patterns lo .. lo + n - 1, or powf(x, y) (fn 3) for the y of them
+    static void test_libm(int fn, uint32_t lo, uint32_t n, float *out_host, float x = 0.f);
 
 private:
     struct Layer { QMat qkv, wq, wk, wv, wo, w13, w2; bool fused_qkv; float *attn_norm, *ffn_norm; PQMat pqkv, pwo, pw13, pw2; };
@@ -203,11 +209,13 @@ private:
     void ensure_sampler();
     std::unique_ptr<ReplyScratch> reply_;   // sample_until's stop state and snapshot, from the context's first call (owned_bytes_)
     void ensure_reply();
-    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler and generator; returns the
-    // stream the steps run on
-    static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], smp::SampleArgs &a);
+    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
+    // returns the stream the steps run on
+    static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
+                                       smp::SampleArgs &a);
     static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
-    static float end_sampling(LlamaDevice *const *c, int n, int steps, bool sampled, uint32_t (*rng)[625], int32_t *ids_out, cudaStream_t s);
+    static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
+                              cudaStream_t s);
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group
     void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)

@@ -1,7 +1,7 @@
 // llama_sample.cuh — sm_90a kernels of the device sampler (minigpt4_b200_sample_steps; host side LlamaDevice::sample_steps in llama.cu,
 // DESIGN.md §4.9): the reference's non-mirostat chain (minigpt4.cpp:2472-2477: top_k -> tail_free -> typical -> top_p -> temperature ->
-// draw) restated operation for operation from the host Sampler (text.cpp), so that a context draws the ids its host Sampler would draw
-// from the same mt19937 state.
+// draw) and its mirostat v1 / v2 branches (:2456-2468) restated operation for operation from the host Sampler (text.cpp), so that a
+// context draws the ids its host Sampler would draw from the same mt19937 state, and leaves the same mirostat μ.
 //
 // One CTA per context.  Element-wise work is spread over the CTA; every float sum the host takes sequentially (softmax, tail_free's
 // accumulate, the entropy, the cumulative cuts, the double sums of std::discrete_distribution) is taken by thread 0 in candidate order.
@@ -91,6 +91,136 @@ __global__ void libm_kernel(int fn, unsigned lo, unsigned n, float *out) {
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float x = __uint_as_float(lo + i);
         out[i] = fn == 0 ? glibc_expf(x) : glibc_logf(x);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// glibc's log2f / powf for mirostat (same algorithms and FMA evaluation as above), bit for bit, NaN results included: where the host's
+// result is a NaN, these give the NaN an x86-64 SSE operation gives (a NaN operand comes back quieted, the first one if both are; an
+// invalid operation gives the default NaN 0xffc00000), while CUDA's float operations always give 0x7fffffff.
+// ---------------------------------------------------------------------------------------------------------------------------------
+__constant__ double kLog2fTab[16][2] = {   // {1/c, log2 c} of the 16 subintervals, shared by log2f and powf's log2
+    {0x1.661ec79f8f3bep+0, -0x1.efec65b963019p-2}, {0x1.571ed4aaf883dp+0, -0x1.b0b6832d4fca4p-2}, {0x1.49539f0f010bp+0, -0x1.7418b0a1fb77bp-2},
+    {0x1.3c995b0b80385p+0, -0x1.39de91a6dcf7bp-2}, {0x1.30d190c8864a5p+0, -0x1.01d9bf3f2b631p-2}, {0x1.25e227b0b8eap+0, -0x1.97c1d1b3b7afp-3},
+    {0x1.1bb4a4a1a343fp+0, -0x1.2f9e393af3c9fp-3}, {0x1.12358f08ae5bap+0, -0x1.960cbbf788d5cp-4}, {0x1.0953f419900a7p+0, -0x1.a6f9db6475fcep-5},
+    {0x1p+0, 0x0p+0}, {0x1.e608cfd9a47acp-1, 0x1.338ca9f24f53dp-4}, {0x1.ca4b31f026aap-1, 0x1.476a9543891bap-3},
+    {0x1.b2036576afce6p-1, 0x1.e840b4ac4e4d2p-3}, {0x1.9c2d163a1aa2dp-1, 0x1.40645f0c6651cp-2}, {0x1.886e6037841edp-1, 0x1.88e9c2c1b9ff8p-2},
+    {0x1.767dcf5534862p-1, 0x1.ce0a44eb17bccp-2}};
+
+// the NaN an x86 operation on a and b returns when its result is a NaN
+__device__ __forceinline__ float x86_nan(float a, float b) {
+    if (isnan(a)) return __uint_as_float(__float_as_uint(a) | 0x00400000u);
+    if (isnan(b)) return __uint_as_float(__float_as_uint(b) | 0x00400000u);
+    return __uint_as_float(0xffc00000u);
+}
+__device__ __forceinline__ float neg(float x) { return __uint_as_float(__float_as_uint(x) ^ 0x80000000u); }   // x86's -x: the sign bit, NaN too
+
+__device__ __forceinline__ float glibc_log2f(float x) {
+    unsigned ix = __float_as_uint(x);
+    if (ix == 0x3f800000u) return 0.0f;
+    if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u) {   // x < 0x1p-126, inf or nan
+        if (ix * 2 == 0) return __int_as_float(0xff800000);
+        if (ix == 0x7f800000u) return x;
+        if ((ix & 0x80000000u) || ix * 2 >= 0xff000000u) return x86_nan(x, x);   // (x - x) / (x - x)
+        ix = __float_as_uint(__fmul_rn(x, 0x1p23f));   // subnormal: normalise
+        ix -= 23u << 23;
+    }
+    const double a0 = -0x1.712b6f70a7e4dp-2, a1 = 0x1.ecabf496832ep-2, a2 = -0x1.715479ffae3dep-1, a3 = 0x1.715475f35c8b8p0;
+    const unsigned tmp = ix - 0x3f330000u;
+    const int i = (int)((tmp >> 19) % 16), k = (int)tmp >> 23;
+    const unsigned iz = ix - (tmp & 0xff800000u);
+    const double invc = kLog2fTab[i][0], logc = kLog2fTab[i][1], z = (double)__uint_as_float(iz);
+    const double r = __fma_rn(z, invc, -1.0);
+    const double y0 = __dadd_rn(logc, (double)k);
+    const double r2 = __dmul_rn(r, r);
+    double y = __fma_rn(a1, r, a2);
+    y = __fma_rn(a0, r2, y);
+    y = __fma_rn(y, r2, __fma_rn(a3, r, y0));
+    return __double2float_rn(y);
+}
+
+// powf's test of a finite non-zero y: 0 not an integer, 1 odd, 2 even
+__device__ __forceinline__ int powf_checkint(unsigned iy) {
+    const int e = iy >> 23 & 0xff;
+    if (e < 0x7f) return 0;
+    if (e > 0x7f + 23) return 2;
+    if (iy & ((1u << (0x7f + 23 - e)) - 1)) return 0;
+    if (iy & (1u << (0x7f + 23 - e))) return 1;
+    return 2;
+}
+__device__ __forceinline__ bool powf_zeroinfnan(unsigned ix) { return 2 * ix - 1 >= 2u * 0x7f800000u - 1; }
+
+__device__ __forceinline__ float glibc_powf(float x, float y) {
+    unsigned sign_bias = 0, ix = __float_as_uint(x);
+    const unsigned iy = __float_as_uint(y);
+    if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u || powf_zeroinfnan(iy)) {   // x < 0x1p-126, inf or nan; or y 0, inf or nan
+        if (powf_zeroinfnan(iy)) {
+            if (2 * iy == 0) return isnan(x) && !(ix & 0x00400000u) ? x86_nan(x, y) : 1.0f;   // (signalling x: x + y)
+            if (ix == 0x3f800000u) return isnan(y) && !(iy & 0x00400000u) ? x86_nan(x, y) : 1.0f;
+            if (2 * ix > 2u * 0x7f800000u || 2 * iy > 2u * 0x7f800000u) return x86_nan(x, y);
+            if (2 * ix == 2 * 0x3f800000u) return 1.0f;
+            if ((2 * ix < 2 * 0x3f800000u) == !(iy & 0x80000000u)) return 0.0f;   // |x| < 1 and y inf, or |x| > 1 and y -inf
+            return __fmul_rn(y, y);
+        }
+        if (powf_zeroinfnan(ix)) {
+            float x2 = isnan(x) ? x86_nan(x, x) : __fmul_rn(x, x);
+            if ((ix & 0x80000000u) && powf_checkint(iy) == 1) x2 = neg(x2);
+            if (iy & 0x80000000u) return isnan(x2) ? x86_nan(x2, x2) : __fdiv_rn(1.0f, x2);
+            return x2;
+        }
+        if (ix & 0x80000000u) {   // finite x < 0
+            const int yint = powf_checkint(iy);
+            if (yint == 0) return __uint_as_float(0xffc00000u);
+            if (yint == 1) sign_bias = 1u << 16;
+            ix &= 0x7fffffffu;
+        }
+        if (ix < 0x00800000u) {   // subnormal x: normalise (the exponent goes negative)
+            ix = __float_as_uint(__fmul_rn(x, 0x1p23f));
+            ix &= 0x7fffffffu;
+            ix -= 23u << 23;
+        }
+    }
+    // log2(x) in double
+    const double a0 = 0x1.27616c9496e0bp-2, a1 = -0x1.71969a075c67ap-2, a2 = 0x1.ec70a6ca7baddp-2, a3 = -0x1.7154748bef6c8p-1,
+                 a4 = 0x1.71547652ab82bp+0;
+    const unsigned tmp = ix - 0x3f330000u, top = tmp & 0xff800000u;
+    const int i = (int)((tmp >> 19) % 16), k = (int)top >> 23;
+    const double invc = kLog2fTab[i][0], logc = kLog2fTab[i][1], z = (double)__uint_as_float(ix - top);
+    const double r = __fma_rn(z, invc, -1.0), y0 = __dadd_rn(logc, (double)k), r2 = __dmul_rn(r, r);
+    double l = __fma_rn(a0, r, a1);
+    const double p = __fma_rn(a2, r, a3), r4 = __dmul_rn(r2, r2);
+    double q = __fma_rn(a4, r, y0);
+    q = __fma_rn(p, r2, q);
+    l = __fma_rn(l, r4, q);
+    const double ylogx = __dmul_rn((double)y, l);
+    if (((unsigned long long)__double_as_longlong(ylogx) >> 47 & 0xffff) >= 0x80bfu) {   // |y log2 x| >= 126 (asuint64(126.0) >> 47)
+        if (ylogx > 0x1.fffffffd1d571p+6) return sign_bias ? __int_as_float(0xff800000) : __int_as_float(0x7f800000);   // overflow
+        if (ylogx <= -150.0) return sign_bias ? -0.0f : 0.0f;                                                             // underflow
+    }
+    // 2^ylogx as expf's exp2 (kExp2fTab), the sign from sign_bias
+    const double shift = 0x1.8p+52 / 32, c0 = 0x1.c6af84b912394p-5, c1 = 0x1.ebfce50fac4f3p-3, c2 = 0x1.62e42ff0c52d6p-1;
+    double kd = __dadd_rn(ylogx, shift);
+    const unsigned long long ki = (unsigned long long)__double_as_longlong(kd);
+    kd = __dsub_rn(kd, shift);
+    const double rr = __dsub_rn(ylogx, kd);
+    const unsigned long long t = kExp2fTab[ki % 32] + ((ki + sign_bias) << 47);
+    const double s = __longlong_as_double((long long)t);
+    const double zz = __fma_rn(c0, rr, c1), rr2 = __dmul_rn(rr, rr);
+    double w = __fma_rn(c2, rr, 1.0);
+    w = __fma_rn(zz, rr2, w);
+    return __double2float_rn(__dmul_rn(w, s));
+}
+
+// (int)f as x86-64's cvttss2si computes it: truncation, and INT_MIN for NaN and for anything outside the int range
+__device__ __forceinline__ int x86_cvtt(float f) {
+    return f >= -2147483648.0f && f < 2147483648.0f ? __float2int_rz(f) : (int)0x80000000u;
+}
+
+// fn 0: log2f of the float bit patterns lo .. lo + n - 1; fn 1: powf(x, y) for the y of those bit patterns
+__global__ void mirostat_libm_kernel(int fn, float x, unsigned lo, unsigned n, float *out) {
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float v = __uint_as_float(lo + i);
+        out[i] = fn == 0 ? glibc_log2f(v) : glibc_powf(x, v);
     }
 }
 
@@ -232,6 +362,31 @@ __device__ unsigned mt_next(MtState &m) {
     return z;
 }
 
+// thread 0's draw over the m candidates whose probabilities softmax_sorted left in c.p: std::discrete_distribution<int> over the float
+// probabilities, as Sampler::draw; hands the drawn index to drawn(idx)
+template <class Drawn> __device__ __forceinline__ void draw(const SampleCtx &c, int m, MtState &mt, Drawn drawn) {
+    int idx = 0;   // one candidate: index 0, no draw from the generator
+    if (m >= 2) {
+        double sum = 0.0;
+        walk(c.p, m, [&](int, float v) { sum += (double)v; return true; });
+        double *cp = (double *)c.keys, acc = 0.0;
+        walk(c.p, m, [&](int i, float v) { acc += (double)v / sum; cp[i] = acc; return true; });
+        cp[m - 1] = 1.0;
+        // generate_canonical<double, 53>: two 32-bit outputs, (a + b 2^32) / 2^64, kept below 1
+        const double lo = (double)mt_next(mt), hi = (double)mt_next(mt);
+        double u = (lo + hi * 4294967296.0) / 18446744073709551616.0;
+        if (u >= 1.0) u = 0x1.fffffffffffffp-1;
+        int first = 0, len = m;   // std::lower_bound
+        while (len > 0) {
+            const int half = len >> 1, mid = first + half;
+            if (cp[mid] < u) { first = mid + 1; len = len - half - 1; }
+            else len = half;
+        }
+        idx = first;
+    }
+    drawn(idx);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------------------
 // one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits as
 // Sampler::sample does and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in
@@ -371,28 +526,77 @@ template <class Fed> __device__ __forceinline__ void sample_body(const SampleArg
     __syncthreads();
     if (!sorted) sort_by_logit(c, m, sbuf);
     softmax_sorted(c, m, &red);
-    if (tid == 0) {
-        int idx = 0;   // one candidate: index 0, no draw from the generator
-        if (m >= 2) {
-            double sum = 0.0;
-            walk(c.p, m, [&](int, float v) { sum += (double)v; return true; });
-            double *cp = (double *)c.keys, acc = 0.0;
-            walk(c.p, m, [&](int i, float v) { acc += (double)v / sum; cp[i] = acc; return true; });
-            cp[m - 1] = 1.0;
-            // generate_canonical<double, 53>: two 32-bit outputs, (a + b 2^32) / 2^64, kept below 1
-            const double lo = (double)mt_next(mt), hi = (double)mt_next(mt);
-            double u = (lo + hi * 4294967296.0) / 18446744073709551616.0;
-            if (u >= 1.0) u = 0x1.fffffffffffffp-1;
-            int first = 0, len = m;   // std::lower_bound
-            while (len > 0) {
-                const int half = len >> 1, mid = first + half;
-                if (cp[mid] < u) { first = mid + 1; len = len - half - 1; }
-                else len = half;
-            }
-            idx = first;
-        }
-        fed(c.id[idx], false);
+    if (tid == 0) draw(c, m, mt, [&](int idx) { fed(c.id[idx], false); });
+    __syncthreads();
+    for (int i = tid; i < kMtN; i += blockDim.x) c.mt->x[i] = mt.x[i];
+    if (tid == 0) c.mt->p = mt.p;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// one context's mirostat step, the body of sample_mirostat_kernel and sample_until_mirostat_kernel: Sampler::sample's mirostat branch
+// (mode 1 or 2) with its μ in `ms`, handing the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id, and neither μ nor the
+// generator is read.  Otherwise μ is set to 2 tau at the mode's first use, as on the host, and updated after the draw.
+// ---------------------------------------------------------------------------------------------------------------------------------
+struct MirostatArgs { int mode; float tau, eta; };   // mode 1 or 2
+
+// a context's μ: right after its generator in its SamplerScratch (llama.cu), so that one copy moves both
+__device__ __forceinline__ MirostatState &mirostat_state(const SampleCtx &c) { return *(MirostatState *)(c.mt + 1); }
+
+template <class Fed>
+__device__ __forceinline__ void mirostat_body(const SampleArgs &a, const MirostatArgs &ma, const SampleCtx &c, MirostatState &ms, Fed fed) {
+    __shared__ unsigned long long sbuf[kSmemSort];
+    __shared__ MtState mt;
+    __shared__ int sh_n;
+    __shared__ float red;
+    const int tid = threadIdx.x, n = a.n_vocab, v = ma.mode - 1;
+    if (a.temp <= 0.f) {
+        if (tid == 0) fed(c.state->tokens[0], true);
+        return;
     }
+    for (int i = tid; i < kMtN; i += blockDim.x) mt.x[i] = c.mt->x[i];
+    if (tid == 0) {
+        mt.p = c.mt->p;
+        if (!ms.init[v]) { ms.mu[v] = 2.0f * ma.tau; ms.init[v] = 1; }
+        sh_n = n;
+    }
+    // temperature over the whole vocabulary, then the sort by the divided logit and the softmax
+    for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i] / a.temp; }
+    __syncthreads();
+    sort_by_logit(c, n, sbuf);
+    softmax_sorted(c, n, &red);
+    const float mu = ms.mu[v];
+    if (v == 0) {
+        // v1: Zipf exponent from the first 100 probabilities (in order, on one thread), then k from it and μ; top_k(k, 1)
+        if (tid == 0) {
+            float s_tb = 0.f, s_tt = 0.f;
+            for (int i = 0; i < 99 && i + 1 < n; ++i) {
+                const float t = glibc_logf((float)(i + 2) / (float)(i + 1)), b = glibc_logf(c.p[i] / c.p[i + 1]);
+                s_tb += t * b; s_tt += t * t;
+            }
+            const float s_hat = s_tb / s_tt, eps = s_hat - 1;
+            const float kf = glibc_powf((eps * glibc_powf(2.0f, mu)) / (1 - glibc_powf((float)n, -eps)), 1 / s_hat);
+            sh_n = min(max(x86_cvtt(kf), 1), n);
+        }
+    } else {
+        // v2: the leading candidates of surprise -log2 p <= μ, at least one (the first that fails ends the host's loop)
+        for (int i = tid; i < n; i += blockDim.x)
+            if (!(-glibc_log2f(c.p[i]) <= mu)) atomicMin(&sh_n, max(i, 1));
+    }
+    __syncthreads();
+    const int m = sh_n;
+    softmax_sorted(c, m, &red);
+    if (tid == 0) draw(c, m, mt, [&](int idx) {
+        fed(c.id[idx], false);
+        // μ -= eta (surprise - tau) with the drawn candidate's probability after the draw's softmax, NaNs as on x86
+        const float s = neg(glibc_log2f(c.p[idx]));
+        float d = s - ma.tau;
+        if (isnan(d)) d = x86_nan(s, ma.tau);
+        float e = ma.eta * d;
+        if (isnan(e)) e = x86_nan(ma.eta, d);
+        float r = mu - e;
+        if (isnan(r)) r = x86_nan(mu, e);
+        ms.mu[v] = r;
+    });
     __syncthreads();
     for (int i = tid; i < kMtN; i += blockDim.x) c.mt->x[i] = mt.x[i];
     if (tid == 0) c.mt->p = mt.p;
@@ -412,6 +616,12 @@ __device__ __forceinline__ void feed(const SampleArgs &a, const SampleCtx &c, in
 __global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
     const SampleCtx &c = a.c[blockIdx.x];
     sample_body(a, c, [&](int id, bool greedy) { feed(a, c, id, greedy); });
+}
+
+// sample_kernel with the mirostat step
+__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a, const MirostatArgs m) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { feed(a, c, id, greedy); });
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -462,11 +672,10 @@ struct StopArgs {
 // one step of sample_kernel that stops each context on its reply's text.  A stopped context does not draw (its generator stays); at
 // the next step it saves its logits and DeviceState, which the host restores at the end of the call, and later steps only keep its
 // batched column moving, so the decode work that still runs for it writes K/V above its final position.
-__global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs a, const StopArgs s) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
-    __shared__ int sh_state;
-    if (threadIdx.x == 0) sh_state = r.done;   // (read once: thread 0 writes r.done below)
+// the start of a step of the stopping kernels (sh_state: a __shared__ int of the kernel): false for a context that has stopped (it saves
+// its snapshot once and keeps its column moving), true for one that samples
+__device__ __forceinline__ bool until_running(const SampleArgs &a, const StopArgs &s, const SampleCtx &c, ReplyState &r, int &sh_state) {
+    if (threadIdx.x == 0) sh_state = r.done;   // (read once: thread 0 writes r.done when it feeds)
     __syncthreads();
     const int done = sh_state;
     if (done != 0) {
@@ -476,13 +685,32 @@ __global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs
             if (threadIdx.x == 0) { r.snap = *c.state; r.done = 2; }
         }
         if (threadIdx.x == 0 && c.slot) c.slot->n_past = c.n_past0 + a.step;
-        return;
+        return false;
     }
-    sample_body(a, c, [&](int id, bool greedy) {
-        feed(a, c, id, greedy);
-        r.n_fed = a.step + 1;
-        if (reply_take(r, s.tab, id)) r.done = 1;
-    });
+    return true;
+}
+// the id a step of the stopping kernels feeds, and the stop check on it
+__device__ __forceinline__ void until_feed(const SampleArgs &a, const StopArgs &s, const SampleCtx &c, ReplyState &r, int id, bool greedy) {
+    feed(a, c, id, greedy);
+    r.n_fed = a.step + 1;
+    if (reply_take(r, s.tab, id)) r.done = 1;
+}
+
+__global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs a, const StopArgs s) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (!until_running(a, s, c, r, sh_state)) return;
+    sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+}
+
+// sample_until_kernel with the mirostat step
+__global__ void __launch_bounds__(kThreads) sample_until_mirostat_kernel(const SampleArgs a, const StopArgs s, const MirostatArgs m) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (!until_running(a, s, c, r, sh_state)) return;
+    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
 
 // seam: reply_take over ids[0, n) from r's tail; *stop_at = the index of the id that ends the reply, -1 if none does

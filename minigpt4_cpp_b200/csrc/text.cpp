@@ -149,6 +149,8 @@ void Sampler::set_rng(const uint32_t state[625]) {
     for (int i = 0; i < 625; ++i) ss << state[i] << ' ';
     ss >> rng_;
 }
+void Sampler::get_mu(float mu[2], bool init[2]) const { mu[0] = mu_v1_; mu[1] = mu_v2_; init[0] = mu_v1_init_; init[1] = mu_v2_init_; }
+void Sampler::set_mu(const float mu[2], const bool init[2]) { mu_v1_ = mu[0]; mu_v2_ = mu[1]; mu_v1_init_ = init[0]; mu_v2_init_ = init[1]; }
 
 int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingParams &sp) {
     if (sp.temp <= 0) return greedy(logits, n_vocab);

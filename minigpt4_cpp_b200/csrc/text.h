@@ -48,6 +48,9 @@ public:
     // the generator's state through its textual representation (operator<< / >>): the 624 words, then the position in them
     void get_rng(uint32_t state[625]) const;
     void set_rng(const uint32_t state[625]);
+    // mirostat's μ of v1 / v2, and whether each has been set by its mode's first use
+    void get_mu(float mu[2], bool init[2]) const;
+    void set_mu(const float mu[2], const bool init[2]);
 private:
     std::mt19937 rng_;
     float mu_v1_ = 0, mu_v2_ = 0; bool mu_v1_init_ = false, mu_v2_init_ = false;

@@ -223,6 +223,8 @@ _EXT = {
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_sample_steps_mirostat": ([_VP, _I, _I, _F, _I, _F, _F, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_sample_until_mirostat": ([_VP, _I, _I, _S, _F, _I, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
@@ -239,6 +241,9 @@ _EXT = {
     "minigpt4_b200_op_sample_timed": ([_VP, _I, _I, _F, _I, _F, _F, _F, _I, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_op_reply_stop": ([_CTX, _VP, _I, _S, _S, C.POINTER(C.c_int32)], _I),
     "minigpt4_b200_op_check_libm": ([_I, C.c_uint32, C.c_uint32, C.POINTER(C.c_longlong)], _I),
+    "minigpt4_b200_op_sample_mirostat": ([_VP, _I, _I, _F, _I, _F, _F, _I, _I, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_op_check_log2f": ([C.c_uint32, C.c_uint32, C.POINTER(C.c_longlong)], _I),
+    "minigpt4_b200_op_check_powf": ([_F, C.c_uint32, C.c_uint32, C.POINTER(C.c_longlong)], _I),
     "minigpt4_b200_host_inspect_container": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
     "minigpt4_b200_host_inspect_ggjt": ([_S, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)], _I),
 }
@@ -355,27 +360,38 @@ class B200:
         return [toks[i].decode("utf-8", errors="ignore") for i in range(n)]
 
     def sample_steps(self, ctxs, steps: int, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0,
-                     typical_p: float = 1.0) -> tuple[np.ndarray, float]:
+                     typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0) -> tuple[np.ndarray, float]:
         """`steps` device-sampled decode steps of every context in `ctxs` (1..8 of one group) with no host round trip in between;
-        returns the fed ids [steps, n] and the device ms of the steps"""
+        returns the fed ids [steps, n] and the device ms of the steps.  mirostat 1 / 2: minigpt4_b200_sample_steps_mirostat (top_k ..
+        typical_p do not apply)"""
         n = len(ctxs)
         ids = np.zeros((max(1, steps), max(1, n)), np.int32)
         ms = C.c_float(0)
-        self._chk(self.L.minigpt4_b200_sample_steps(C.cast(self._ctx_array(ctxs), C.c_void_p), n, steps, temp, top_k, top_p, tfs_z, typical_p,
-                                                    _ptr(ids), C.byref(ms)))
+        ctx = C.cast(self._ctx_array(ctxs), C.c_void_p)
+        if mirostat:
+            self._chk(self.L.minigpt4_b200_sample_steps_mirostat(ctx, n, steps, temp, mirostat, mirostat_tau, mirostat_eta, _ptr(ids), C.byref(ms)))
+        else:
+            self._chk(self.L.minigpt4_b200_sample_steps(ctx, n, steps, temp, top_k, top_p, tfs_z, typical_p, _ptr(ids), C.byref(ms)))
         return ids[:steps, :n], ms.value
 
     def sample_until(self, ctxs, max_steps: int, stop: str | bytes | None = None, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
-                     tfs_z: float = 1.0, typical_p: float = 1.0) -> tuple[list[list[int]], list[bool], float]:
+                     tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0,
+                     mirostat_eta: float = 1.0) -> tuple[list[list[int]], list[bool], float]:
         """device-sampled steps of every context in `ctxs` (1..8 of one group), each until its reply ends with `stop` (None: "###"; "": never)
-        or max_steps; returns each context's fed ids, whether the stop text ended it, and the device ms"""
+        or max_steps; returns each context's fed ids, whether the stop text ended it, and the device ms.  mirostat 1 / 2:
+        minigpt4_b200_sample_until_mirostat"""
         n = len(ctxs)
         ids = np.zeros((max(1, max_steps), max(1, n)), np.int32)
         n_out, stopped = np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.int32)
         ms = C.c_float(0)
         st = stop.encode() if isinstance(stop, str) else stop
-        self._chk(self.L.minigpt4_b200_sample_until(C.cast(self._ctx_array(ctxs), C.c_void_p), n, max_steps, st, temp, top_k, top_p, tfs_z,
-                                                    typical_p, _ptr(ids), _ptr(n_out), _ptr(stopped), C.byref(ms)))
+        ctx = C.cast(self._ctx_array(ctxs), C.c_void_p)
+        if mirostat:
+            self._chk(self.L.minigpt4_b200_sample_until_mirostat(ctx, n, max_steps, st, temp, mirostat, mirostat_tau, mirostat_eta, _ptr(ids),
+                                                                 _ptr(n_out), _ptr(stopped), C.byref(ms)))
+        else:
+            self._chk(self.L.minigpt4_b200_sample_until(ctx, n, max_steps, st, temp, top_k, top_p, tfs_z, typical_p, _ptr(ids), _ptr(n_out),
+                                                        _ptr(stopped), C.byref(ms)))
         return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
 
     def time_matvec(self, ctx, kind: int, reps: int = 3) -> tuple[float, float]:
@@ -462,6 +478,29 @@ class B200:
         bad = C.c_longlong(0)
         self._chk(self.L.minigpt4_b200_op_check_libm(fn, lo_bits, hi_bits, C.byref(bad)))
         return bad.value
+
+    def op_check_log2f(self, lo_bits: int, hi_bits: int) -> int:
+        """device log2f against the host libm over the float bit patterns lo_bits..hi_bits; returns the mismatches"""
+        bad = C.c_longlong(0)
+        self._chk(self.L.minigpt4_b200_op_check_log2f(lo_bits, hi_bits, C.byref(bad)))
+        return bad.value
+
+    def op_check_powf(self, x: float, lo_bits: int, hi_bits: int) -> int:
+        """device powf(x, y) against the host libm for the y of the float bit patterns lo_bits..hi_bits; returns the mismatches"""
+        bad = C.c_longlong(0)
+        self._chk(self.L.minigpt4_b200_op_check_powf(x, lo_bits, hi_bits, C.byref(bad)))
+        return bad.value
+
+    def op_sample_mirostat(self, logits: np.ndarray, seed: int, n_draws: int = 1, temp=0.8, mirostat=1, mirostat_tau=5.0, mirostat_eta=1.0,
+                           on_device: bool = True, timed: bool = False):
+        """mirostat draws over the same logits from one generator and an unset μ, by the device kernel or (on_device False) the host
+        Sampler: (ids, μ after each draw), and with timed the average ms of one sampling launch"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        ids, mu = np.zeros(n_draws, np.int32), np.zeros(n_draws, np.float32)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_op_sample_mirostat(_ptr(lg), lg.size, seed, temp, mirostat, mirostat_tau, mirostat_eta, n_draws, int(on_device),
+                                                          _ptr(ids), _ptr(mu), C.byref(ms)))
+        return (ids, mu, ms.value) if timed else (ids, mu)
 
     def op_matvec(self, gtype: int, w_raw: np.ndarray, rows: int, cols: int, x: np.ndarray) -> np.ndarray:
         x = np.ascontiguousarray(x, np.float32).reshape(-1, cols)
@@ -561,9 +600,10 @@ class MiniGPT4ChatBot:
             yield token
 
     def generate_on_device(self, message: str, limit: int = 1024, chunk: int = 16, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
-                           tfs_z: float = 1.0, typical_p: float = 1.0):
-        """generate() with the sampling and the stop check on the GPU: minigpt4_b200_sample_until calls of up to `chunk` steps, each
-        stopping where generate()'s loop stops (mirostat 0; the repetition arguments, which generate() passes on unused, are not taken).
+                           tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0):
+        """generate() with the sampling and the stop check on the GPU: minigpt4_b200_sample_until (mirostat 1 / 2: _mirostat) calls of up
+        to `chunk` steps, each stopping where generate()'s loop stops (the repetition arguments, which generate() passes on unused, are not
+        taken).
         Yields what generate() yields for the same seed: no "##" token, and not the token that completes "###".
 
         One difference cannot be avoided: generate() decodes each token's bytes with errors="ignore" before it appends and checks them,
@@ -577,7 +617,8 @@ class MiniGPT4ChatBot:
         ext = B200(self.library)
         done = 0
         while done < limit:
-            ids, stopped, _ = ext.sample_until([self.ctx], min(chunk, limit - done), None, temp, top_k, top_p, tfs_z, typical_p)
+            ids, stopped, _ = ext.sample_until([self.ctx], min(chunk, limit - done), None, temp, top_k, top_p, tfs_z, typical_p, mirostat,
+                                               mirostat_tau, mirostat_eta)
             done += len(ids[0])
             for k, t in enumerate(ids[0]):
                 if stopped[0] and k == len(ids[0]) - 1:

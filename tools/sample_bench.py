@@ -7,11 +7,13 @@ minigpt4_begin_chat_image with 32 seeded embedding rows, about 95 rows) and samp
   the ceiling;
 - B = 2, 4, 8 sessions: the minigpt4_b200_end_chat_batch loop against sample_steps(n=B, steps=1) loops and one steps=128 call;
 
-for the web UI's parameters (temp 0.8, top_k 40, top_p 0.9) and for top_k 0 / top_p 0.95.  The sampling kernel's own time is the
-CUDA-event average of one launch over a context's logits (minigpt4_b200_op_sample_timed).  parity: every arm's ids equal the end_chat
-arm's.  Prints one JSON line.
+for the web UI's parameters (temp 0.8, top_k 40, top_p 0.9), for top_k 0 / top_p 0.95, and for mirostat 1 (tau 5, eta 0.1) and
+mirostat 2 (tau 5, eta 1.0) at temp 0.8 (minigpt4_b200_sample_steps_mirostat; both sort the whole vocabulary every step, as top_k 0 does).
+The sampling kernel's own time is the CUDA-event average of one launch over a context's logits (minigpt4_b200_op_sample_timed /
+op_sample_mirostat).  parity: every arm's ids equal the end_chat arm's; parity_mismatch lists the legs that differ, with the session
+and step of their first differing token.  Prints one JSON line.
 
-    python tools/sample_bench.py [--steps 128] [--rounds 3]"""
+    python tools/sample_bench.py [--steps 128] [--rounds 3] [--params webui,top_k0_top_p0.95,mirostat1,mirostat2]"""
 import argparse
 import ctypes
 import json
@@ -29,14 +31,18 @@ from tools.sessions_bench import gpu_card  # noqa: E402
 
 N_CTX = 2048
 QUESTION = "Describe this image in detail, please."
-PARAMS = {"webui": dict(temp=0.8, top_k=40, top_p=0.9), "top_k0_top_p0.95": dict(temp=0.8, top_k=0, top_p=0.95)}
+PARAMS = {"webui": dict(temp=0.8, top_k=40, top_p=0.9), "top_k0_top_p0.95": dict(temp=0.8, top_k=0, top_p=0.95),
+          "mirostat1": dict(temp=0.8, mirostat=1, mirostat_tau=5.0, mirostat_eta=0.1),
+          "mirostat2": dict(temp=0.8, mirostat=2, mirostat_tau=5.0, mirostat_eta=1.0)}
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=128)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--params", default=",".join(PARAMS), help="comma-separated names of PARAMS to run")
     args = ap.parse_args()
+    params = {pn: PARAMS[pn] for pn in args.params.split(",")}
     lib = m.load_library()
     ext = m.B200(lib)
     if ext.L.minigpt4_b200_device_count() < 1:
@@ -86,7 +92,7 @@ def main():
             ext.base.minigpt4_free(c)
         return t, toks
 
-    arms = [(arm, B, pn) for pn in PARAMS for B in (1, 2, 4, 8) for arm in ("host", "device_steps1", "device_steps_all")]
+    arms = [(arm, B, pn) for pn in params for B in (1, 2, 4, 8) for arm in ("host", "device_steps1", "device_steps_all")]
     arms.append(("decode_chain", 1, "greedy"))
     for arm, B, pn in arms:   # warm-up: graphs of every batch size, scratch of every arm
         run(arm, B, PARAMS.get(pn, {}))
@@ -97,7 +103,14 @@ def main():
             t, tk = run(a[0], a[1], PARAMS.get(a[2], {}))
             wall[a].append(t)
             toks.setdefault(a, tk)
-    parity = all(toks[(arm, B, pn)] == toks[("host", B, pn)] for arm, B, pn in arms if arm != "decode_chain")
+    def first_diff(got, want):   # [session, step] of the first token that differs
+        for i, (g, w) in enumerate(zip(got, want)):
+            for s, (x, y) in enumerate(zip(g, w)):
+                if x != y:
+                    return [i, s]
+        return None
+    mismatch = {f"{pn}/B{B}/{arm}": first_diff(toks[(arm, B, pn)], toks[("host", B, pn)]) for arm, B, pn in arms if arm not in ("host", "decode_chain")}
+    mismatch = {k: v for k, v in mismatch.items() if v}
     legs = {}
     for a in arms:
         arm, B, pn = a
@@ -108,13 +121,17 @@ def main():
     logits = ext.logits(c)
     ext.base.minigpt4_free(c)
     kernel = {}
-    for pn, p in PARAMS.items():
-        _, ms = ext.op_sample(logits, 1000, 64, tfs_z=1.0, typical_p=1.0, timed=True, **p)
+    for pn, p in params.items():
+        if p.get("mirostat"):
+            _, _, ms = ext.op_sample_mirostat(logits, 1000, 64, timed=True, **p)
+        else:
+            _, ms = ext.op_sample(logits, 1000, 64, tfs_z=1.0, typical_p=1.0, timed=True, **p)
         kernel[pn] = {"us_per_launch": round(ms * 1e3, 1)}
     st = ext.stats(parent)
     out = {"metric": "sampled decode tokens/s, Vicuna-7B q4_1, n_ctx 2048, after one image-chat turn", "steps": S, "rounds": args.rounds,
            "timing": "best of rounds, wall clock around synchronous calls, arms alternated", "legs": legs, "sample_kernel": kernel,
-           "decode_megakernel": st.decode_megakernel, "parity": parity, **gpu_card()}
+           "decode_megakernel": st.decode_megakernel, "parity": not mismatch,
+           "parity_mismatch": mismatch, **gpu_card()}
     print(json.dumps(out))
     ext.base.minigpt4_free(parent)
 
