@@ -61,20 +61,22 @@ MINIGPT4_API struct MiniGPT4Context *minigpt4_b200_session_create(struct MiniGPT
  * 512 prompt rows and a few small buffers); device bytes it shares with its group (weights, operand cache, tables, prefill
  * scratch, the workspace of the batched calls once built).  Any pointer may be NULL. */
 MINIGPT4_API int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_contexts, double *owned_bytes, double *shared_bytes);
-/* One decode step of n (1..8) distinct contexts of one group: the weights stream once for all of them.  Context i is fed ids[i]
+/* One decode step of n (1..64) distinct contexts of one group: the weights stream once for all of them.  Context i is fed ids[i]
  * (ids[i] < 0: its current on-device greedy id, as in minigpt4_b200_decode_chain) at its own n_past; queued prompt pieces of
  * each context are evaluated first.  Afterwards each context has new logits, n_past + 1, and ids_out[i] = its new greedy id;
- * its logits are the bits a step on its own gives.  Synchronous.  NULL or duplicate contexts, contexts of different groups,
- * n outside 1..8, a full context or an id >= n_vocab return the FailedToAddString error code (8) and change no context. */
+ * its logits are the bits a step on its own gives.  n >= 2 runs one batched step: its layers take the per-op matvecs up to 15
+ * contexts, and from 16 contexts on the tensor-core GEMM of the prompt passes on models with homogeneous Q4_0 / Q4_1 layers (the
+ * per-op matvecs on every other model); either gives the same bits.  Synchronous.  NULL or duplicate contexts, contexts of different groups,
+ * n outside 1..64, a full context or an id >= n_vocab return the FailedToAddString error code (8) and change no context. */
 MINIGPT4_API int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, int32_t *ids_out);
-/* Evaluate the queued prompt rows (add_tokens / add_embedding pieces not yet evaluated) of n (1..8) distinct contexts of one group
+/* Evaluate the queued prompt rows (add_tokens / add_embedding pieces not yet evaluated) of n (1..64) distinct contexts of one group
  * in shared passes over the weights, at most 512 rows per pass; a context's rows may be split across two passes.  Afterwards each
  * context is exactly as minigpt4_b200_flush would have left it: n_past, KV cache, logits (bit for bit), greedy id and the device
  * state the next decode step continues from.  Contexts with an empty queue are left untouched; n = 1 is that context's own flush.
  * minigpt4_b200_get_hidden(ctx, out, k), with k the number of its rows in the pass that evaluated its last row, returns the residual
  * stream of those rows, i.e. of its last k rows (an own flush leaves the rows of its own last pass the same way).
  * minigpt4_b200_decode_batch and end_chat_batch flush their contexts this way.
- * Synchronous.  NULL or duplicate contexts, contexts of different groups or n outside 1..8 return the FailedToAddString error
+ * Synchronous.  NULL or duplicate contexts, contexts of different groups or n outside 1..64 return the FailedToAddString error
  * code (8) and change no context. */
 MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n);
 /* minigpt4_end_chat on each context in turn (each samples from its own logits with its own sampler; greedy uses the device
@@ -83,7 +85,7 @@ MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n)
 MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p,
                                               float tfs_z, float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
                                               float alpha_frequency, int mirostat, float mirostat_tau, float mirostat_eta, int penalize_nl);
-/* `steps` sampled decode steps of n (1..8) distinct contexts of one group with no return to the host in between: each step samples
+/* `steps` sampled decode steps of n (1..64) distinct contexts of one group with no return to the host in between: each step samples
  * every context's logits on the device with the chain of minigpt4_end_chat (top_k, tail_free, typical, top_p, temperature, draw;
  * mirostat: minigpt4_b200_sample_steps_mirostat) and its own generator, then feeds the n ids in one decode step (n = 1: the context's own decode graph or megakernel;
  * n >= 2: the batched step of minigpt4_b200_decode_batch).  Queued prompt pieces are evaluated first, as in end_chat_batch.
@@ -93,11 +95,11 @@ MINIGPT4_API int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int
  * CUDA-event time of the steps.  temp <= 0 is greedy: the ids of minigpt4_b200_decode_chain / decode_batch, generator untouched.
  * The ids equal the host sampler's except where candidates tie: equal logits are ordered by lower id here (DESIGN.md §4.9).
  * A call always runs exactly `steps` steps; to stop at the end of a reply use minigpt4_b200_sample_until.
- * NULL ctxs / ids_out, NULL or duplicate contexts, contexts of different groups, n outside 1..8, steps < 1, a tensor-parallel
+ * NULL ctxs / ids_out, NULL or duplicate contexts, contexts of different groups, n outside 1..64, steps < 1, a tensor-parallel
  * context or n_past + steps > n_ctx for any context return the FailedToAddString error code (8) before any device work. */
 MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int32_t top_k, float top_p,
                                             float tfs_z, float typical_p, int32_t *ids_out, float *ms_out);
-/* A whole reply (or a chunk of one) for n (1..8) contexts of one group: the steps of minigpt4_b200_sample_steps, each context stopping
+/* A whole reply (or a chunk of one) for n (1..64) contexts of one group: the steps of minigpt4_b200_sample_steps, each context stopping
  * where the reference's chat loop (MiniGPT4ChatBot.generate) stops its reply.  That loop appends the text of every token to the reply,
  * skips the check for a token that is exactly "##", and otherwise stops once the reply ends with "###"; the stopping token is fed.  Here
  * context i stops after the first step whose id's text is not exactly "##" and leaves the reply ending with `stop`, or after max_steps.
@@ -114,7 +116,7 @@ MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n
  * lie above each context's final position, where its next token overwrites them.  The first call of a group builds a device table of
  * every id's text (counted in minigpt4_b200_session_info's shared bytes); each context's first call allocates its stop state and a
  * snapshot of its logits (owned bytes).
- * NULL ctxs / ids_out / n_out, NULL or duplicate contexts, contexts of different groups, n outside 1..8, max_steps < 1, a stop text
+ * NULL ctxs / ids_out / n_out, NULL or duplicate contexts, contexts of different groups, n outside 1..64, max_steps < 1, a stop text
  * over 32 bytes, a tensor-parallel context or n_past + max_steps > n_ctx for any context return 8 before any device work. */
 MINIGPT4_API int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
                                             float top_p, float tfs_z, float typical_p, int32_t *ids_out, int32_t *n_out, int32_t *stopped,

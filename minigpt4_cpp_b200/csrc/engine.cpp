@@ -85,7 +85,7 @@ Error Engine::init_session(const Engine &parent, int seed) {
 
 // Batched decode (extension): every check happens before anything runs, so a refused batch leaves every context as it was.
 bool Engine::group_valid(Engine *const *e, int n, const char *what) {
-    if (!e || n < 1 || n > 8) { MG4_ERR("%s: %d contexts (1 .. 8)", what, n); return false; }
+    if (!e || n < 1 || n > LlamaDevice::kMaxBatch) { MG4_ERR("%s: %d contexts (1 .. %d)", what, n, LlamaDevice::kMaxBatch); return false; }
     for (int i = 0; i < n; ++i) {
         if (!e[i]) { MG4_ERR("%s: context %d is NULL", what, i); return false; }
         for (int j = 0; j < i; ++j) if (e[j] == e[i]) { MG4_ERR("%s: context %d appears twice", what, i); return false; }
@@ -110,7 +110,7 @@ Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t 
         if (!c.llm_->decode_step(ids[0], c.n_past_)) return ErrFailedToAddString;
         ids_out[0] = c.llm_->argmax();
     } else {
-        LlamaDevice *L[8]; int np[8];
+        LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch];
         for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; }
         LlamaDevice::decode_batch(L, n, ids, np, ids_out);
     }
@@ -120,7 +120,7 @@ Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t 
 Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p) {
     if (!tokens || !batch_valid(e, n, nullptr)) return ErrFailedToAddString;   // (before any sampler draws)
     if (!flush_group(e, n)) return ErrFailedToAddString;   // so that each sample_token finds its queue empty
-    int32_t ids[8], out[8];
+    int32_t ids[LlamaDevice::kMaxBatch], out[LlamaDevice::kMaxBatch];
     for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
     const Error err = decode_batch(e, n, ids, out);
     for (int i = 0; i < n; ++i) e[i]->reply_take(tokens[i]);
@@ -149,7 +149,9 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
         if (e[i]->n_past_ + steps > n_ctx) { MG4_ERR("sample_steps: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, steps, n_ctx); return ErrFailedToAddString; }
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
-    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; MirostatState mu[8];
+    LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch]; MirostatState mu[LlamaDevice::kMaxBatch];
+    std::vector<uint32_t> rng_words((size_t)n * 625);   // (625 words a generator: 160 KB at kMaxBatch, off the stack)
+    uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); }
     const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out);
     for (int i = 0; i < n; ++i) {
@@ -173,7 +175,9 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
     e[0]->ensure_token_table();
-    LlamaDevice *L[8]; int np[8]; uint32_t rng[8][625]; MirostatState mu[8]; std::string tail[8];
+    LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch]; MirostatState mu[LlamaDevice::kMaxBatch]; std::string tail[LlamaDevice::kMaxBatch];
+    std::vector<uint32_t> rng_words((size_t)n * 625);
+    uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
     const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped);
     for (int i = 0; i < n; ++i) {
@@ -210,10 +214,11 @@ Error Engine::flush_batch(Engine *const *e, int n) {
 }
 // the queues of a validated batch: one context with queued rows is its own flush(), several share the passes of eval_rows_batch
 bool Engine::flush_group(Engine *const *e, int n) {
-    Engine *q[8]; int m = 0;
+    Engine *q[LlamaDevice::kMaxBatch]; int m = 0;
     for (int i = 0; i < n; ++i) if (!e[i]->pend_ids_.empty()) q[m++] = e[i];
     if (m <= 1) return m == 0 || q[0]->flush();
-    LlamaDevice *L[8]; const int32_t *ids[8]; const float *emb[8]; int rows[8], base[8];
+    LlamaDevice *L[LlamaDevice::kMaxBatch]; const int32_t *ids[LlamaDevice::kMaxBatch]; const float *emb[LlamaDevice::kMaxBatch];
+    int rows[LlamaDevice::kMaxBatch], base[LlamaDevice::kMaxBatch];
     for (int i = 0; i < m; ++i) {
         L[i] = q[i]->llm_.get(); ids[i] = q[i]->pend_ids_.data(); emb[i] = q[i]->pend_emb_.data();
         rows[i] = (int)q[i]->pend_ids_.size(); base[i] = q[i]->pend_base_;

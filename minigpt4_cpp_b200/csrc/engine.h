@@ -24,11 +24,11 @@ public:
     // a session: a new conversation over the model of `parent` (language and vision weights, encode lanes, tokenizer shared; own KV
     // cache, prompt queue, logits, state and a sampler seeded with `seed`)
     Error init_session(const Engine &parent, int seed);
-    // one decode step of n (1..8) distinct contexts of one group, weights streamed once (see minigpt4_b200_decode_batch); all or nothing
+    // one decode step of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group, weights streamed once (see minigpt4_b200_decode_batch); all or nothing
     static Error decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out);
     // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
     static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
-    // `steps` decode steps of n (1..8) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
+    // `steps` decode steps of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
     // own generator and mirostat μ (see minigpt4_b200_sample_steps / _mirostat); ids_out[s * n + i]; all or nothing
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
     // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
@@ -37,7 +37,7 @@ public:
                               int32_t *stopped, float *ms_out);
     // sample_until's text check over ids from the reply `tail` (see minigpt4_b200_op_reply_stop); -1: no id ends the reply
     Error reply_stop(const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at);
-    // the queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
+    // the queued prompt rows of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
     static Error flush_batch(Engine *const *e, int n);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
     static constexpr int kEncodeLanes = 8;
@@ -66,7 +66,7 @@ public:
     TPLink tp;
 
 private:
-    static bool group_valid(Engine *const *e, int n, const char *what);   // 1..8 distinct non-NULL contexts of one group
+    static bool group_valid(Engine *const *e, int n, const char *what);   // 1..LlamaDevice::kMaxBatch distinct non-NULL contexts of one group
     static bool batch_valid(Engine *const *e, int n, const int32_t *ids);
     static bool flush_group(Engine *const *e, int n);
     // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)

@@ -19,8 +19,18 @@ static size_t g_max_dyn_smem = 0;
 static thread_local size_t t_dev_bytes = 0;
 template <class T> static void dmalloc(T **p, size_t n) { CUDA_CHECK(cudaMalloc((void **)p, n)); t_dev_bytes += n; }
 
+constexpr int kMaxBatch = LlamaDevice::kMaxBatch;
+
+// Decode steps of more than 8 columns run their layers through the tensor-core prefill GEMM (record_layers' gemm pass with the slot
+// table) from this many columns on, on models that have it (pf_ready_); below it, and on every other model, through the per-op matvecs
+// in 8-column chunks.  Batches of up to 8 columns always take the per-op matvecs.
+// Measured with tools/wide_batch_bench.py (Vicuna-7B Q4_1, n_ctx 512, 1x H100 80GB HBM3 at 700 W), ms per step tensor-core / per-op:
+// B 9: 11.24 / 9.21, 12: 11.53 / 10.02, 16: 12.08 / 12.10, 24: 13.17 / 18.07, 32: 14.33 / 24.31, 48: 21.43 / 36.66, 64: 23.90 / 49.38.
+constexpr int kWideGemmMin = 16;
+
 // what the contexts of one model share besides the weight pointers each of them holds: the workspace of the batched passes (built by
-// the group's first decode_batch or batched flush; decode_batch uses its first 8 rows), their stream and the batched decode step's graphs
+// the group's first decode_batch or batched flush; decode_batch uses its first kMaxBatch rows), their stream and the batched decode
+// step's graphs
 struct LlamaGroup {
     size_t weight_bytes = 0;       // the parent's load minus its own context: weights, operand cache, tables, prefill scratch
     size_t batch_bytes = 0;
@@ -28,16 +38,17 @@ struct LlamaGroup {
     float *x = nullptr, *q = nullptr, *att = nullptr, *act = nullptr;   // [kPrefillMax] rows (act also holds the qkv GEMM's [rows][3 n_embd] output)
     float *last = nullptr;         // [8] the last rows of the contexts that end in a prompt pass
     unsigned char *qact = nullptr;
-    DeviceState *state = nullptr;  // the batch's tokens (the decode graph's embed gathers column t from tokens[t])
+    DeviceState *state = nullptr;  // the batch's tokens (the decode graph's embed gathers column t from tokens[t], up to 8 columns)
+    int *tok = nullptr;            // [kMaxBatch] the tokens of a decode step of more than 8 columns (embed_rows_kernel gathers them)
     SessionSlot *rows = nullptr, *h_rows = nullptr;     // [kPrefillMax] a slot per row of a prompt pass
-    SessionSlot *slots = nullptr, *h_slots = nullptr;   // [8] a slot per context: the columns of a decode step, the contexts that end in a prompt pass
-    int *ids = nullptr, *h_ids = nullptr;               // [8] their new arg-max ids
-    cudaGraphExec_t graph[9] = {};
-    int graph_kernels[9] = {};
+    SessionSlot *slots = nullptr, *h_slots = nullptr;   // [kMaxBatch] a slot per context: the columns of a decode step, the contexts that end in a prompt pass
+    int *ids = nullptr, *h_ids = nullptr;               // [kMaxBatch] their new arg-max ids
+    cudaGraphExec_t graph[kMaxBatch + 1] = {};
+    int graph_kernels[kMaxBatch + 1] = {};
     smp::TokenTable tokens{};      // every id's text for sample_until's stop rule (built by the group's first call)
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
-        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)rows, (void *)slots, (void *)ids,
+        for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)tok, (void *)rows, (void *)slots, (void *)ids,
                         (void *)tokens.off, (void *)tokens.bytes})
             if (p) cudaFree(p);
         for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids}) if (p) cudaFreeHost(p);
@@ -82,7 +93,7 @@ struct SamplerScratch {
 struct ReplyScratch {
     smp::ReplyState *r = nullptr, *h_r = nullptr;
     float *snap = nullptr;
-    int *h_done = nullptr;   // [2][8] pinned: the done flags after the last two chunks issued
+    int *h_done = nullptr;   // [2][kMaxBatch] pinned: the done flags after the last two chunks issued
     cudaEvent_t ev[2] = {};
     size_t bytes = 0;
     explicit ReplyScratch(int n_vocab) {
@@ -90,7 +101,7 @@ struct ReplyScratch {
         CUDA_CHECK(cudaMalloc((void **)&r, bytes));
         snap = (float *)(r + 1);
         CUDA_CHECK(cudaHostAlloc((void **)&h_r, sizeof(smp::ReplyState), cudaHostAllocDefault));
-        CUDA_CHECK(cudaHostAlloc((void **)&h_done, 16 * sizeof(int), cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_done, 2 * kMaxBatch * sizeof(int), cudaHostAllocDefault));
         for (cudaEvent_t &e : ev) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
     ~ReplyScratch() {
@@ -857,12 +868,13 @@ void LlamaDevice::build_group_workspace() {
     dmalloc(&G.last, (size_t)8 * E * 4);
     dmalloc(&G.qact, (size_t)8 * ((size_t)std::max(E, FF) * 2 + 4096));
     dmalloc(&G.state, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.state, 0, sizeof(DeviceState)));
+    dmalloc(&G.tok, kMaxBatch * sizeof(int));
     dmalloc(&G.rows, R * sizeof(SessionSlot));
-    dmalloc(&G.slots, 8 * sizeof(SessionSlot));
-    dmalloc(&G.ids, 8 * sizeof(int));
+    dmalloc(&G.slots, kMaxBatch * sizeof(SessionSlot));
+    dmalloc(&G.ids, kMaxBatch * sizeof(int));
     CUDA_CHECK(cudaHostAlloc((void **)&G.h_rows, R * sizeof(SessionSlot), cudaHostAllocDefault));
-    CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, 8 * sizeof(SessionSlot), cudaHostAllocDefault));
-    CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, 8 * sizeof(int), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_slots, kMaxBatch * sizeof(SessionSlot), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_ids, kMaxBatch * sizeof(int), cudaHostAllocDefault));
     CUDA_CHECK(cudaDeviceSynchronize());
     G.batch_bytes += t_dev_bytes - b0;
 }
@@ -871,20 +883,31 @@ void LlamaDevice::build_group_workspace() {
 // batched decode step over B contexts of one group: prepare (tokens) -> embed B rows -> layers (QKV and attention per column through the
 // context table; wo / gate-up / down through matvec_kernel at ntok = B) -> logits of every column into its own context -> finalize every
 // context's DeviceState -> the B ids to pinned memory.  Captured once per B on the group stream.
+// More than 8 columns: the tokens go through the group's id list (DeviceState holds 8), the layers run in 8-column matvec chunks or, from
+// kWideGemmMin columns on a pf_ready_ model, as the tensor-core pass of the batched prompt pass (one row per column), and the logits in
+// 8-column chunks.  Every column still gets the bits of its own decode step.
 // ------------------------------------------------------------------------------------------------
 void LlamaDevice::build_batch_graph(int B) {
     LlamaGroup &G = *group_;
     cudaStream_t s = G.stream;
     unsigned long long n = 0;
     cudaGraph_t g = nullptr;
+    const int E = d_.n_embd, block = (B + 31) / 32 * 32;   // (prepare / finalize: a thread per column)
     CUDA_CHECK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.state); ++n;
-    launch_embed(B, G.state, G.x, s, &n);
-    record_layers(Pass{B, G.x, G.q, G.att, G.act, G.qact, G.state, G.slots, false, s, &n});
-    MatvecArgs o = mv_args(output_, B, G.state, G.qact, tab_silu_);
-    o.x = G.x; o.x_stride = d_.n_embd; o.norm_w = final_norm_; o.epi = EPI_LOGITS; o.n_valid = d_.n_vocab;
-    launch_matvec(o, sm_count_, s, &n, G.slots, 0);
-    finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.ids); ++n;
+    if (B <= 8) {
+        prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, B, G.state); ++n;
+        launch_embed(B, G.state, G.x, s, &n);
+    } else {
+        prepare_wide_kernel<<<1, block, 0, s>>>(G.slots, B, G.tok); ++n;
+        embed_rows_kernel<<<B, 256, 0, s>>>(tok_type_, (const unsigned char *)tok_raw_, gg_row_bytes(tok_type_, (size_t)E), E, G.tok, embd_in_, G.x); ++n;
+    }
+    record_layers(Pass{B, G.x, G.q, G.att, G.act, G.qact, G.state, G.slots, pf_ready_ && B >= kWideGemmMin, s, &n});
+    for (int t0 = 0; t0 < B; t0 += 8) {
+        MatvecArgs o = mv_args(output_, std::min(8, B - t0), G.state, G.qact, tab_silu_);
+        o.x = G.x + (size_t)t0 * E; o.x_stride = E; o.norm_w = final_norm_; o.epi = EPI_LOGITS; o.n_valid = d_.n_vocab;
+        launch_matvec(o, sm_count_, s, &n, G.slots + t0, 0);
+    }
+    finalize_sessions_kernel<<<1, block, 0, s>>>(G.slots, B, G.ids); ++n;
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaMemcpyAsync(G.h_ids, G.ids, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamEndCapture(s, &g));
@@ -927,8 +950,7 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
     while (ci < n) {
         // ---- the pass: rows, their slots and ids; embedding rows of each context are a contiguous run of its emb[] (queued in order)
         int rows = 0, n_emb = 0, nf = 0;
-        RowList last{};
-        int fin_ctx[8], fin_first[8];
+        int last[kMaxBatch], fin_ctx[kMaxBatch], fin_first[kMaxBatch];
         for (; ci < n && rows < S; ++ci, cj = 0) {
             const int take = std::min(n_rows[ci] - cj, S - rows);
             LlamaDevice &X = *c[ci];
@@ -951,7 +973,7 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
             rows += take; cj += take;
             if (cj < n_rows[ci]) break;   // the context continues in the next pass
             G.h_slots[nf] = SessionSlot{n_past[ci] + n_rows[ci] - 1, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
-            last.r[nf] = rows - 1; fin_ctx[nf] = ci; fin_first[nf] = rows - take;
+            last[nf] = rows - 1; fin_ctx[nf] = ci; fin_first[nf] = rows - take;
             ++nf;
         }
         CUDA_CHECK(cudaMemcpyAsync(G.rows, G.h_rows, (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
@@ -961,18 +983,23 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
         ++L0.launches_;
         L0.record_layers(Pass{rows, G.x, G.q, G.att, G.act, G.qact, G.state, G.rows, L0.pf_ready_ && rows >= 2, s, &L0.launches_});
 
-        // ---- contexts that end in this pass: logits + arg-max of their last row, DeviceState, hidden rows, pinned arg-max
+        // ---- contexts that end in this pass, 8 at a time: logits + arg-max of their last row, DeviceState; then hidden rows, pinned arg-max
         if (nf) {
-            gather_rows_kernel<<<nf, 256, 0, s>>>(G.x, last, E, G.last);
-            prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots, nf, G.state);
-            MatvecArgs o = mv_args(L0.output_, nf, G.state, G.qact, L0.tab_silu_);
-            o.x = G.last; o.x_stride = E; o.norm_w = L0.final_norm_; o.epi = EPI_LOGITS; o.n_valid = L0.d_.n_vocab;
-            launch_matvec(o, L0.sm_count_, s, &L0.launches_, G.slots, 0);
-            finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots, nf, G.ids);
-            CUDA_CHECK(cudaGetLastError()); L0.launches_ += 3;
+            for (int f0 = 0; f0 < nf; f0 += 8) {
+                const int m = std::min(8, nf - f0);
+                RowList lr{};
+                for (int f = 0; f < m; ++f) lr.r[f] = last[f0 + f];
+                gather_rows_kernel<<<m, 256, 0, s>>>(G.x, lr, E, G.last);
+                prepare_sessions_kernel<<<1, 32, 0, s>>>(G.slots + f0, m, G.state);
+                MatvecArgs o = mv_args(L0.output_, m, G.state, G.qact, L0.tab_silu_);
+                o.x = G.last; o.x_stride = E; o.norm_w = L0.final_norm_; o.epi = EPI_LOGITS; o.n_valid = L0.d_.n_vocab;
+                launch_matvec(o, L0.sm_count_, s, &L0.launches_, G.slots + f0, 0);
+                finalize_sessions_kernel<<<1, 32, 0, s>>>(G.slots + f0, m, G.ids + f0);
+                CUDA_CHECK(cudaGetLastError()); L0.launches_ += 3;
+            }
             CUDA_CHECK(cudaMemcpyAsync(G.h_ids, G.ids, (size_t)nf * 4, cudaMemcpyDeviceToHost, s));
             for (int f = 0; f < nf; ++f) {
-                const int k = last.r[f] + 1 - fin_first[f];
+                const int k = last[f] + 1 - fin_first[f];
                 CUDA_CHECK(cudaMemcpyAsync(c[fin_ctx[f]]->x_, G.x + (size_t)fin_first[f] * E, (size_t)k * E * 4, cudaMemcpyDeviceToDevice, s));
             }
         }
@@ -1090,8 +1117,8 @@ void LlamaDevice::ensure_sampler() {
     owned_bytes_ += smp_->bytes;
 }
 
-static smp::SampleArgs sample_args(const SamplingArgs &p, int n_vocab) {
-    smp::SampleArgs a{};
+static smp::SampleArgsWide sample_args(const SamplingArgs &p, int n_vocab) {
+    smp::SampleArgsWide a{};
     a.n_vocab = n_vocab; a.top_k = p.top_k; a.temp = p.temp; a.top_p = p.top_p; a.tfs_z = p.tfs_z; a.typical_p = p.typical_p;
     return a;
 }
@@ -1100,11 +1127,42 @@ static smp::MirostatArgs mirostat_args(const SamplingArgs &p) {
     m.mode = p.mirostat; m.tau = p.mirostat_tau; m.eta = p.mirostat_eta;
     return m;
 }
+// a launch of at most 8 contexts takes the 8-column tables: the first 8 columns of the wide ones
+static smp::SampleArgs narrow(const smp::SampleArgsWide &w) {
+    smp::SampleArgs a{};
+    memcpy(a.c, w.c, sizeof(a.c));
+    a.n_vocab = w.n_vocab; a.step = w.step; a.top_k = w.top_k; a.temp = w.temp; a.top_p = w.top_p; a.tfs_z = w.tfs_z; a.typical_p = w.typical_p;
+    return a;
+}
+static smp::StopArgs narrow(const smp::StopArgsWide &w) {
+    smp::StopArgs s{};
+    memcpy(s.r, w.r, sizeof(s.r)); memcpy(s.snap, w.snap, sizeof(s.snap)); s.tab = w.tab;
+    return s;
+}
+// one sampling step of n contexts in one launch (grid n): the 8-column kernels up to 8 contexts, the wide ones above
+static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArgs &p, const smp::MirostatArgs &m, cudaStream_t s) {
+    if (n <= 8) {
+        const smp::SampleArgs a8 = narrow(a);
+        if (p.mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, m);
+        else smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a8);
+    } else if (p.mirostat) smp::sample_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, m);
+    else smp::sample_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
+}
+static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArgsWide &sa, int n, const SamplingArgs &p, const smp::MirostatArgs &m,
+                                cudaStream_t s) {
+    if (n <= 8) {
+        const smp::SampleArgs a8 = narrow(a);
+        const smp::StopArgs s8 = narrow(sa);
+        if (p.mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8, m);
+        else smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8);
+    } else if (p.mirostat) smp::sample_until_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, m);
+    else smp::sample_until_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
+}
 // the bytes of a context's sampler state that a call moves: the generator, and μ after it with mirostat
 static size_t sampler_state_bytes(const SamplingArgs &p) { return 625 * 4 + (p.mirostat ? sizeof(MirostatState) : 0); }
 
 cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
-                                         smp::SampleArgs &a) {
+                                         smp::SampleArgsWide &a) {
     LlamaDevice &L0 = *c[0];
     a = sample_args(p, L0.d_.n_vocab);
     cudaStream_t s = L0.stream_;
@@ -1175,14 +1233,13 @@ float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const S
 
 float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                                 MirostatState *mu, int32_t *ids_out) {
-    smp::SampleArgs a;
+    smp::SampleArgsWide a;
     const smp::MirostatArgs m = mirostat_args(p);
     cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
     CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
     for (int t = 0; t < steps; ++t) {
         a.step = t;
-        if (p.mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a, m);
-        else smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a);
+        launch_sample(a, n, p, m, s);
         sampled_decode(c, n, n_past[0] + t, s);
     }
     return end_sampling(c, n, steps, p, rng, mu, ids_out, s);
@@ -1219,10 +1276,10 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                                 MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped) {
     LlamaDevice &L0 = *c[0];
-    smp::SampleArgs a;
+    smp::SampleArgsWide a;
     const smp::MirostatArgs m = mirostat_args(p);
     cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
-    smp::StopArgs sa{};
+    smp::StopArgsWide sa{};
     sa.tab = L0.group_->tokens;
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
@@ -1238,17 +1295,16 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         if (j >= 2) {   // chunk j - 2's flags; chunk j - 1 keeps the device busy meanwhile
             CUDA_CHECK(cudaEventSynchronize(R0.ev[j % 2]));
             bool all = true;
-            for (int i = 0; i < n; ++i) all = all && R0.h_done[(j % 2) * 8 + i] != 0;
+            for (int i = 0; i < n; ++i) all = all && R0.h_done[(j % 2) * kMaxBatch + i] != 0;
             if (all) break;
         }
         for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
             a.step = issued;
-            if (p.mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, m);
-            else smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
+            launch_sample_until(a, sa, n, p, m, s);
             sampled_decode(c, n, n_past[0] + issued, s);
         }
         for (int i = 0; i < n; ++i)
-            CUDA_CHECK(cudaMemcpyAsync(R0.h_done + (j % 2) * 8 + i, &c[i]->reply_->r->done, sizeof(int), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaMemcpyAsync(R0.h_done + (j % 2) * kMaxBatch + i, &c[i]->reply_->r->done, sizeof(int), cudaMemcpyDeviceToHost, s));
         CUDA_CHECK(cudaEventRecord(R0.ev[j % 2], s));
     }
     for (int i = 0; i < n; ++i)
@@ -1301,7 +1357,7 @@ void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingAr
     CUDA_CHECK(cudaMemcpy(ss.mt, rng, 625 * 4, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemset(ss.mu, 0, sizeof(MirostatState)));
     if (mu_out && p.mirostat) CUDA_CHECK(cudaMalloc((void **)&mu_d, (size_t)n_draws * 4));
-    smp::SampleArgs a = sample_args(p, n_vocab);
+    smp::SampleArgsWide a = sample_args(p, n_vocab);
     a.c[0] = ss.ctx(lg, st, nullptr, 0);
     const smp::MirostatArgs m = mirostat_args(p);
     cudaEvent_t e0, e1;
@@ -1309,8 +1365,7 @@ void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingAr
     CUDA_CHECK(cudaEventRecord(e0, 0));
     for (int i = 0; i < n_draws; ++i) {
         a.step = i;
-        if (p.mirostat) smp::sample_mirostat_kernel<<<1, smp::kThreads>>>(a, m);
-        else smp::sample_kernel<<<1, smp::kThreads>>>(a);
+        launch_sample(a, 1, p, m, 0);
         CUDA_CHECK(cudaGetLastError());
         if (mu_d) CUDA_CHECK(cudaMemcpyAsync(mu_d + i, &ss.mu->mu[p.mirostat - 1], 4, cudaMemcpyDeviceToDevice, 0));
     }

@@ -57,7 +57,7 @@ struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; int 
 struct MirostatState { float mu[2]; int init[2]; };   // a context's mirostat μ of v1 / v2 and whether each is set (Sampler::get_mu)
 struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
 struct ReplyScratch;   // a context's stop state in sample_until: reply tail, stop text, done flag, snapshot (llama.cu, llama_sample.cuh)
-namespace smp { struct SampleArgs; }
+namespace smp { template <int N> struct SampleArgsN; }
 
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
 
@@ -74,17 +74,22 @@ public:
     int group_size() const { return (int)group_.use_count(); }
     size_t owned_bytes() const { return owned_bytes_; }   // device bytes of this context: KV cache + per-context scratch
     size_t shared_bytes() const;                          // device bytes shared by the group: weights, operand cache, tables, prefill scratch, batch workspace
-    // One decode step of n (2..8) distinct contexts of one group; the weights stream once.  Column i is fed ids[i] (< 0: the context's
+    // the most contexts one batched call takes: two 32-token tiles of the prefill GEMM (pf::kTok), and about the 7B sessions at n_ctx 2048
+    // that fit on an 80 GB card
+    static constexpr int kMaxBatch = 64;
+    // One decode step of n (2..kMaxBatch) distinct contexts of one group; the weights stream once.  Column i is fed ids[i] (< 0: the context's
     // on-device greedy id) at position n_past[i]; afterwards each context holds what its own decode_step would have left (logits,
     // arg-max, DeviceState) and ids_out[i] = its new arg-max.  Synchronous.  The caller validates (distinct, one group, ranges).
+    // n <= 8: per-op matvecs at NT = n; more: the layers in 8-column matvec chunks, or from kWideGemmMin (llama.cu) columns on a
+    // pf_ready_ model the tensor-core pass of eval_rows_batch with one row per column.
     static void decode_batch(LlamaDevice *const *ctx, int n, const int32_t *ids, const int *n_past, int32_t *ids_out);
-    // The queued prompt rows of n (1..8) distinct contexts of one group in shared passes over the weights, kPrefillMax rows per pass:
+    // The queued prompt rows of n (1..kMaxBatch) distinct contexts of one group in shared passes over the weights, kPrefillMax rows per pass:
     // context i has n_rows[i] (1..kPrefillMax) rows starting at position n_past[i], ids[i][j] >= 0 a token, < 0 row -1 - ids[i][j] of
     // emb[i] (n_embd floats per row, in order of first use).  Afterwards each context holds what its own eval_rows would have left
     // (KV cache, logits, arg-max, DeviceState) and the first rows of its hidden state are its rows of the pass that evaluated its
     // last row.  Synchronous.  The caller validates (distinct, one group, rows checked when they were queued).
     static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past);
-    // `steps` sampled decode steps of n (1..8) distinct contexts of one group with no host round trip: each step samples every context's
+    // `steps` sampled decode steps of n (1..kMaxBatch) distinct contexts of one group with no host round trip: each step samples every context's
     // current logits on the device (llama_sample.cuh; p.temp <= 0: the greedy id) into its DeviceState, then runs the decode step (n = 1:
     // the context's own graph or megakernel; n >= 2: the batch graph, every column fed its DeviceState::tokens[0]).  rng[i] holds context
     // i's mt19937 state (624 words and the position) on entry and on return, and with p.mirostat 1 / 2 mu[i] its mirostat μ (mu may be
@@ -212,7 +217,7 @@ private:
     // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
     // returns the stream the steps run on
     static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
-                                       smp::SampleArgs &a);
+                                       smp::SampleArgsN<kMaxBatch> &a);
     static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
     static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
                               cudaStream_t s);

@@ -240,11 +240,14 @@ struct SampleCtx {
     unsigned long long *keys;    // [pow2 >= n_vocab] sort keys; the discrete distribution's cumulative doubles afterwards
     int *id; float *logit, *p, *aux;   // [n_vocab] candidates (id, logit, probability); tail_free's d2 / typical's terms
 };
-struct SampleArgs {
-    SampleCtx c[8];
+// a sampling launch's arguments, one column per CTA; the table is passed by value, so its capacity N is part of the kernel's parameters
+template <int N> struct SampleArgsN {
+    SampleCtx c[N];
     int n_vocab, step, top_k;
     float temp, top_p, tfs_z, typical_p;
 };
+struct SampleArgs : SampleArgsN<8> {};                               // the kernels of 1..8 contexts
+using SampleArgsWide = SampleArgsN<LlamaDevice::kMaxBatch>;          // the wide kernels of 9..kMaxBatch contexts
 
 // float -> key that orders like the float (-0 as +0, so that equal logits are equal keys), and back
 __device__ __forceinline__ unsigned ord_key(float v) {
@@ -392,7 +395,7 @@ template <class Drawn> __device__ __forceinline__ void draw(const SampleCtx &c, 
 // Sampler::sample does and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in
 // tokens[0] (greedy = true; the generator is not read).  Otherwise the generator is written back after fed returns.
 // ---------------------------------------------------------------------------------------------------------------------------------
-template <class Fed> __device__ __forceinline__ void sample_body(const SampleArgs &a, const SampleCtx &c, Fed fed) {
+template <class A, class Fed> __device__ __forceinline__ void sample_body(const A &a, const SampleCtx &c, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
     __shared__ MtState mt;
     __shared__ unsigned hist[256];
@@ -542,8 +545,8 @@ struct MirostatArgs { int mode; float tau, eta; };   // mode 1 or 2
 // a context's μ: right after its generator in its SamplerScratch (llama.cu), so that one copy moves both
 __device__ __forceinline__ MirostatState &mirostat_state(const SampleCtx &c) { return *(MirostatState *)(c.mt + 1); }
 
-template <class Fed>
-__device__ __forceinline__ void mirostat_body(const SampleArgs &a, const MirostatArgs &ma, const SampleCtx &c, MirostatState &ms, Fed fed) {
+template <class A, class Fed>
+__device__ __forceinline__ void mirostat_body(const A &a, const MirostatArgs &ma, const SampleCtx &c, MirostatState &ms, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
     __shared__ MtState mt;
     __shared__ int sh_n;
@@ -603,7 +606,7 @@ __device__ __forceinline__ void mirostat_body(const SampleArgs &a, const Mirosta
 }
 
 // the id a step feeds: into tokens[0] (the greedy id is already there) and ids[step]; a batched column moves to its next position
-__device__ __forceinline__ void feed(const SampleArgs &a, const SampleCtx &c, int id, bool greedy) {
+template <class A> __device__ __forceinline__ void feed(const A &a, const SampleCtx &c, int id, bool greedy) {
     if (!greedy) c.state->tokens[0] = id;
     c.ids[a.step] = id;
     if (c.slot) c.slot->n_past = c.n_past0 + a.step;
@@ -611,18 +614,22 @@ __device__ __forceinline__ void feed(const SampleArgs &a, const SampleCtx &c, in
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits, writes the id into tokens[0] and
-// ids[step], and moves a batched column to its next position.
+// ids[step], and moves a batched column to its next position.  The *_wide_kernel variants take the kMaxBatch-column table (n > 8) and
+// share the body, so every column computes what it computes in the 8-column kernels.
 // ---------------------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) {
+template <class A> __device__ __forceinline__ void sample_step(const A &a) {
     const SampleCtx &c = a.c[blockIdx.x];
     sample_body(a, c, [&](int id, bool greedy) { feed(a, c, id, greedy); });
 }
-
-// sample_kernel with the mirostat step
-__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a, const MirostatArgs m) {
+template <class A> __device__ __forceinline__ void sample_mirostat_step(const A &a, const MirostatArgs &m) {
     const SampleCtx &c = a.c[blockIdx.x];
     mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { feed(a, c, id, greedy); });
 }
+__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) { sample_step(a); }
+__global__ void __launch_bounds__(kThreads) sample_wide_kernel(const SampleArgsWide a) { sample_step(a); }
+// sample_kernel with the mirostat step
+__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a, const MirostatArgs m) { sample_mirostat_step(a, m); }
+__global__ void __launch_bounds__(kThreads) sample_mirostat_wide_kernel(const SampleArgsWide a, const MirostatArgs m) { sample_mirostat_step(a, m); }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // stop on the reply's text (minigpt4_b200_sample_until; host side LlamaDevice::sample_until): the reference's chat loop
@@ -663,18 +670,21 @@ __device__ __forceinline__ bool reply_take(ReplyState &r, TokenTable t, int id) 
     return stop;
 }
 
-struct StopArgs {
-    ReplyState *r[8];
-    float *snap[8];   // [n_vocab] each context's logits after its last step
+template <int N> struct StopArgsN {
+    ReplyState *r[N];
+    float *snap[N];   // [n_vocab] each context's logits after its last step
     TokenTable tab;
 };
+struct StopArgs : StopArgsN<8> {};
+using StopArgsWide = StopArgsN<LlamaDevice::kMaxBatch>;
+static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) + sizeof(MirostatArgs) <= 32764, "the widest kernel's parameters fit the 32 764-byte limit");
 
 // one step of sample_kernel that stops each context on its reply's text.  A stopped context does not draw (its generator stays); at
 // the next step it saves its logits and DeviceState, which the host restores at the end of the call, and later steps only keep its
 // batched column moving, so the decode work that still runs for it writes K/V above its final position.
 // the start of a step of the stopping kernels (sh_state: a __shared__ int of the kernel): false for a context that has stopped (it saves
 // its snapshot once and keeps its column moving), true for one that samples
-__device__ __forceinline__ bool until_running(const SampleArgs &a, const StopArgs &s, const SampleCtx &c, ReplyState &r, int &sh_state) {
+template <class A, class S> __device__ __forceinline__ bool until_running(const A &a, const S &s, const SampleCtx &c, ReplyState &r, int &sh_state) {
     if (threadIdx.x == 0) sh_state = r.done;   // (read once: thread 0 writes r.done when it feeds)
     __syncthreads();
     const int done = sh_state;
@@ -690,7 +700,7 @@ __device__ __forceinline__ bool until_running(const SampleArgs &a, const StopArg
     return true;
 }
 // the id a step of the stopping kernels feeds, and the stop check on it
-__device__ __forceinline__ void until_feed(const SampleArgs &a, const StopArgs &s, const SampleCtx &c, ReplyState &r, int id, bool greedy) {
+template <class A, class S> __device__ __forceinline__ void until_feed(const A &a, const S &s, const SampleCtx &c, ReplyState &r, int id, bool greedy) {
     feed(a, c, id, greedy);
     r.n_fed = a.step + 1;
     if (reply_take(r, s.tab, id)) r.done = 1;
@@ -703,9 +713,23 @@ __global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs
     if (!until_running(a, s, c, r, sh_state)) return;
     sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
+__global__ void __launch_bounds__(kThreads) sample_until_wide_kernel(const SampleArgsWide a, const StopArgsWide s) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (!until_running(a, s, c, r, sh_state)) return;
+    sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+}
 
 // sample_until_kernel with the mirostat step
 __global__ void __launch_bounds__(kThreads) sample_until_mirostat_kernel(const SampleArgs a, const StopArgs s, const MirostatArgs m) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (!until_running(a, s, c, r, sh_state)) return;
+    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+}
+__global__ void __launch_bounds__(kThreads) sample_until_mirostat_wide_kernel(const SampleArgsWide a, const StopArgsWide s, const MirostatArgs m) {
     const SampleCtx &c = a.c[blockIdx.x];
     ReplyState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;

@@ -107,8 +107,19 @@ __global__ void prepare_sessions_kernel(const SessionSlot *slots, int B, DeviceS
     }
 }
 
+// prepare_sessions_kernel for a step of more than 8 columns (DeviceState::tokens holds 8): column t's token goes to ids[t], which
+// embed_rows_kernel gathers; block >= B threads
+__global__ void prepare_wide_kernel(const SessionSlot *slots, int B, int *ids) {
+    const int t = threadIdx.x;
+    if (t < B) {
+        const SessionSlot &s = slots[t];
+        ids[t] = s.id >= 0 ? s.id : s.state->tokens[0];
+        s.state->argmax_key = 0ull;
+    }
+}
+
 // after the step: every context's DeviceState is what its own decode step leaves (finalize_kernel): n_past + 1, the new arg-max
-// as argmax_id and as the next token, the key reset; ids_out[t] = column t's arg-max
+// as argmax_id and as the next token, the key reset; ids_out[t] = column t's arg-max; block >= B threads
 __global__ void finalize_sessions_kernel(const SessionSlot *slots, int B, int *ids_out) {
     const int t = threadIdx.x;
     if (t < B) {
@@ -149,7 +160,8 @@ __global__ void __launch_bounds__(256) qkv_rows_kernel(const float *__restrict__
 
 struct RowList { int r[8]; };   // rows of a pass, by value
 
-// the last row of each context that ends in this pass -> contiguous rows for the logits matvec; grid = n rows
+// the last row of each context that ends in this pass -> contiguous rows for the logits matvec; grid = n rows (<= 8: the contexts that
+// end in one pass are finished 8 at a time)
 __global__ void gather_rows_kernel(const float *__restrict__ x, const RowList rows, int E, float *__restrict__ out) {
     const float *src = x + (size_t)rows.r[blockIdx.x] * E;
     for (int i = threadIdx.x; i < E; i += blockDim.x) out[(size_t)blockIdx.x * E + i] = src[i];

@@ -336,7 +336,7 @@ class B200:
         return (C.c_void_p * max(1, len(ctxs)))(*[c.ptr for c in ctxs])
 
     def decode_batch(self, ctxs, ids=None) -> np.ndarray:
-        """one decode step of every context in `ctxs` (1..8 of one group; weights streamed once); ids[i] < 0 or ids None: each context's
+        """one decode step of every context in `ctxs` (1..64 of one group; weights streamed once); ids[i] < 0 or ids None: each context's
         own greedy id.  Returns the new greedy ids."""
         n = len(ctxs)
         a = np.full(n, -1, np.int32) if ids is None else np.ascontiguousarray(ids, np.int32)
@@ -345,7 +345,7 @@ class B200:
         return out[:n]
 
     def flush_batch(self, ctxs) -> None:
-        """evaluate the queued prompt rows of every context in `ctxs` (1..8 of one group) in shared passes over the weights"""
+        """evaluate the queued prompt rows of every context in `ctxs` (1..64 of one group) in shared passes over the weights"""
         self._chk(self.L.minigpt4_b200_flush_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), len(ctxs)))
 
     def end_chat_batch(self, ctxs, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
@@ -361,7 +361,7 @@ class B200:
 
     def sample_steps(self, ctxs, steps: int, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0,
                      typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0) -> tuple[np.ndarray, float]:
-        """`steps` device-sampled decode steps of every context in `ctxs` (1..8 of one group) with no host round trip in between;
+        """`steps` device-sampled decode steps of every context in `ctxs` (1..64 of one group) with no host round trip in between;
         returns the fed ids [steps, n] and the device ms of the steps.  mirostat 1 / 2: minigpt4_b200_sample_steps_mirostat (top_k ..
         typical_p do not apply)"""
         n = len(ctxs)
@@ -377,7 +377,7 @@ class B200:
     def sample_until(self, ctxs, max_steps: int, stop: str | bytes | None = None, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
                      tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0,
                      mirostat_eta: float = 1.0) -> tuple[list[list[int]], list[bool], float]:
-        """device-sampled steps of every context in `ctxs` (1..8 of one group), each until its reply ends with `stop` (None: "###"; "": never)
+        """device-sampled steps of every context in `ctxs` (1..64 of one group), each until its reply ends with `stop` (None: "###"; "": never)
         or max_steps; returns each context's fed ids, whether the stop text ended it, and the device ms.  mirostat 1 / 2:
         minigpt4_b200_sample_until_mirostat"""
         n = len(ctxs)
