@@ -79,6 +79,29 @@ MINIGPT4_API int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n
  * Synchronous.  NULL or duplicate contexts, contexts of different groups or n outside 1..64 return the FailedToAddString error
  * code (8) and change no context. */
 MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n);
+/* How likely is a known continuation: the log-probability of every id of it, for n (1..64) distinct contexts of one group in shared
+ * passes over the weights.  ids holds the contexts' token ids back to back, n_ids[i] >= 1 of them for context i; logprob_out and
+ * rank_out have the layout of ids, logits_out (may be NULL) one n_vocab row per id in the same order.  Queued prompt pieces are
+ * evaluated first, as in minigpt4_b200_decode_batch; then context i's ids are evaluated at positions n_past .. n_past + n_ids[i] - 1
+ * in passes of at most 512 rows (a context's rows may be split across two passes).  For entry j of context i:
+ *   logprob_out[j] = log p(ids[j] | the conversation so far and ids[0 .. j-1]): for j = 0 from the context's logits before the call,
+ *     for j >= 1 from the logits of row j - 1 of this call.  With n_past = 0 there are no logits before the call: entry 0 is NaN, its
+ *     rank -1.  With m the row's largest logit, lp = (float)((z_t - m) - log sum exp((double)z - m)), the sum in double.
+ *   rank_out[j] (may be NULL) = the ids with a larger logit plus those with an equal logit and a lower id (the device sampler's tie
+ *     rule); rank 0: the greedy step would have picked ids[j].
+ *   logits_out row j = the logits of the row of ids[j] (those that predict ids[j + 1]), bit for bit the logits the context would
+ *     hold after evaluating its ids up to j.
+ * keep = 1: afterwards each context is where minigpt4_b200_eval_tokens(ids) + flush leaves it (n_past, logits, greedy id, device
+ * state, minigpt4_b200_get_hidden as for flush_batch; the reply tail is cleared).  keep = 0: afterwards each context is exactly as it
+ * was (n_past, logits, greedy id, device state, hidden rows, reply tail, generator and mirostat μ); the call only writes K / V rows at
+ * positions >= n_past, which the next evaluated token overwrites before anything reads them, so the K continuations of one prompt are
+ * K calls on one context with nothing to undo.  The group's first call allocates 512 rows of logits (counted in
+ * minigpt4_b200_session_info's shared bytes: 65.5 MB at n_vocab 32000).  Synchronous.
+ * NULL ctxs / ids / n_ids / logprob_out, NULL or duplicate contexts, contexts of different groups, n outside 1..64, n_ids[i] < 1, an
+ * id outside the vocabulary, n_past + n_ids[i] > n_ctx, keep outside 0..1 or a tensor-parallel context return the FailedToAddString
+ * error code (8) and change no context, before any device work. */
+MINIGPT4_API int minigpt4_b200_score_tokens(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, const int32_t *n_ids, int keep,
+                                            float *logprob_out, int32_t *rank_out, float *logits_out);
 /* minigpt4_end_chat on each context in turn (each samples from its own logits with its own sampler; greedy uses the device
  * arg-max; tokens[i] = the sampled token's text), then the n sampled ids are fed in one minigpt4_b200_decode_batch step.
  * The batch is validated before any sampling. */

@@ -224,6 +224,10 @@ int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32
     return Engine::decode_batch(reinterpret_cast<Engine *const *>(ctxs), n, ids, ids_out);
 }
 int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n) { return Engine::flush_batch(reinterpret_cast<Engine *const *>(ctxs), n); }
+int minigpt4_b200_score_tokens(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, const int32_t *n_ids, int keep, float *logprob_out,
+                               int32_t *rank_out, float *logits_out) {
+    return Engine::score_tokens(reinterpret_cast<Engine *const *>(ctxs), n, ids, n_ids, keep, logprob_out, rank_out, logits_out);
+}
 int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p, float tfs_z,
                                  float typical_p, int32_t /*repeat_last_n*/, float /*repeat_penalty*/, float /*alpha_presence*/,
                                  float /*alpha_frequency*/, int mirostat, float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {

@@ -212,6 +212,34 @@ Error Engine::flush_batch(Engine *const *e, int n) {
     if (!group_valid(e, n, "flush_batch")) return ErrFailedToAddString;
     return flush_group(e, n) ? ErrNone : ErrFailedToAddString;
 }
+Error Engine::score_tokens(Engine *const *e, int n, const int32_t *ids, const int32_t *n_ids, int keep, float *logprob, int32_t *rank, float *logits) {
+    if (!ids || !n_ids || !logprob || !group_valid(e, n, "score_tokens")) return ErrFailedToAddString;
+    if (keep != 0 && keep != 1) { MG4_ERR("score_tokens: keep %d (0 or 1)", keep); return ErrFailedToAddString; }
+    const int n_vocab = e[0]->llm_->dims().n_vocab;
+    size_t off[LlamaDevice::kMaxBatch];
+    size_t total = 0;
+    for (int i = 0; i < n; ++i) {
+        if (e[i]->tp.world > 1) { MG4_ERR("score_tokens: context %d is tensor-parallel", i); return ErrFailedToAddString; }
+        const int n_ctx = e[i]->llm_->dims().n_ctx;
+        if (n_ids[i] < 1) { MG4_ERR("score_tokens: context %d: %d ids", i, n_ids[i]); return ErrFailedToAddString; }
+        if (n_ids[i] > n_ctx - e[i]->n_past_) { MG4_ERR("score_tokens: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, n_ids[i], n_ctx); return ErrFailedToAddString; }
+        off[i] = total;
+        total += (size_t)n_ids[i];
+    }
+    for (size_t t = 0; t < total; ++t)
+        if (ids[t] < 0 || ids[t] >= n_vocab) { MG4_ERR("score_tokens: token id %d out of range", ids[t]); return ErrFailedToAddString; }
+    if (!flush_group(e, n)) return ErrFailedToAddString;
+    LlamaDevice *L[LlamaDevice::kMaxBatch]; const int32_t *id[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch];
+    float *lp[LlamaDevice::kMaxBatch], *lg[LlamaDevice::kMaxBatch]; int32_t *rk[LlamaDevice::kMaxBatch];
+    for (int i = 0; i < n; ++i) {
+        L[i] = e[i]->llm_.get(); id[i] = ids + off[i]; np[i] = e[i]->n_past_; lp[i] = logprob + off[i];
+        rk[i] = rank ? rank + off[i] : nullptr; lg[i] = logits ? logits + off[i] * (size_t)n_vocab : nullptr;
+    }
+    LlamaDevice::score_rows(L, n, id, n_ids, np, keep == 1, lp, rank ? rk : nullptr, logits ? lg : nullptr);
+    if (keep)
+        for (int i = 0; i < n; ++i) { e[i]->n_past_ += n_ids[i]; e[i]->reply_clear(); }
+    return ErrNone;
+}
 // the queues of a validated batch: one context with queued rows is its own flush(), several share the passes of eval_rows_batch
 bool Engine::flush_group(Engine *const *e, int n) {
     Engine *q[LlamaDevice::kMaxBatch]; int m = 0;

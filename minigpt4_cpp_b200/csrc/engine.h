@@ -39,6 +39,10 @@ public:
     Error reply_stop(const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at);
     // the queued prompt rows of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)
     static Error flush_batch(Engine *const *e, int n);
+    // log-probability, rank and (logits non-NULL) logits of every id of a known continuation of n (1..64, LlamaDevice::kMaxBatch) distinct
+    // contexts of one group, in shared passes over the weights (see minigpt4_b200_score_tokens); keep: the ids stay evaluated, as
+    // b200_eval_tokens + flush leaves them; otherwise every context is left as it was.  All or nothing
+    static Error score_tokens(Engine *const *e, int n, const int32_t *ids, const int32_t *n_ids, int keep, float *logprob, int32_t *rank, float *logits);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
     static constexpr int kEncodeLanes = 8;
     Error encode_images(const ::MiniGPT4Image *images, size_t n, ::MiniGPT4Embedding *out, float *total_ms);   // batched: concurrent lanes

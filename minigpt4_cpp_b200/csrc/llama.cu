@@ -4,6 +4,7 @@
 #include "llama_prefill.cuh"
 #include "llama_sessions.cuh"
 #include "llama_sample.cuh"
+#include "llama_score.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -46,12 +47,18 @@ struct LlamaGroup {
     cudaGraphExec_t graph[kMaxBatch + 1] = {};
     int graph_kernels[kMaxBatch + 1] = {};
     smp::TokenTable tokens{};      // every id's text for sample_until's stop rule (built by the group's first call)
+    // score_rows (built by the group's first call): every row's logits of a pass, the DeviceState their matvecs' arg-max atomics land in
+    // (never read), and the scored entries of a pass (kPrefillMax rows + the first entry of each context) with their results
+    float *score_logits = nullptr;
+    DeviceState *score_state = nullptr;
+    k::ScoreRow *score_rows = nullptr, *h_score_rows = nullptr;
+    k::ScoreOut *score_out = nullptr, *h_score_out = nullptr;
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
         for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)tok, (void *)rows, (void *)slots, (void *)ids,
-                        (void *)tokens.off, (void *)tokens.bytes})
+                        (void *)tokens.off, (void *)tokens.bytes, (void *)score_logits, (void *)score_state, (void *)score_rows, (void *)score_out})
             if (p) cudaFree(p);
-        for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids}) if (p) cudaFreeHost(p);
+        for (void *p : {(void *)h_rows, (void *)h_slots, (void *)h_ids, (void *)h_score_rows, (void *)h_score_out}) if (p) cudaFreeHost(p);
         if (stream) cudaStreamDestroy(stream);
     }
 };
@@ -937,27 +944,58 @@ void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids,
 // contexts in order; row t carries its own position and its context's caches in the row table, and record_layers runs the pass with it.
 // Contexts whose last row is in the pass get their logits, arg-max and DeviceState through the context table, as the batched decode
 // step does.  Every row is quantised and reduced on its own, so each context gets the bits of its own eval_rows.
+// A scoring pass (score_rows) points each row's logits at its row of the group's scratch instead: after the layers every row's logits
+// are computed in 8-row chunks straight from the pass's rows, the entries whose logits are in this pass are scored, and the results and
+// requested logits rows go to the host.  The context tail runs only with score->keep.
 // ------------------------------------------------------------------------------------------------
-void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past) {
+struct ScoreCall {
+    bool keep;
+    float *const *logprob;    // [n] entries of each context
+    int32_t *const *rank;     // [n] or null
+    float *const *logits;     // [n] rows of n_vocab of each context, or null
+};
+
+void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past,
+                                  const ScoreCall *score) {
     LlamaDevice &L0 = *c[0];
     LlamaGroup &G = *L0.group_;
     for (int i = 0; i < n; ++i) c[i]->sync();   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
     if (!G.x) L0.build_group_workspace();
+    if (score && !G.score_logits) L0.build_score_scratch();
     const int E = L0.d_.n_embd, S = kPrefillMax;
+    const size_t V = (size_t)L0.d_.n_vocab;
     cudaStream_t s = G.stream;
     std::vector<int32_t> pid((size_t)S);
+    std::vector<int> ent_ctx, ent_j;   // scoring: each entry's context and index, in the order of the pass's entry table
     int ci = 0, cj = 0;   // next row: row cj of context ci
     while (ci < n) {
         // ---- the pass: rows, their slots and ids; embedding rows of each context are a contiguous run of its emb[] (queued in order)
-        int rows = 0, n_emb = 0, nf = 0;
+        int rows = 0, n_emb = 0, nf = 0, nr = 0;
         int last[kMaxBatch], fin_ctx[kMaxBatch], fin_first[kMaxBatch];
+        int run_ctx[kMaxBatch], run_j[kMaxBatch], run_row[kMaxBatch], run_n[kMaxBatch];   // scoring: each context's rows in this pass
+        ent_ctx.clear(); ent_j.clear();
         for (; ci < n && rows < S; ++ci, cj = 0) {
             const int take = std::min(n_rows[ci] - cj, S - rows);
             LlamaDevice &X = *c[ci];
             int k0 = -1, k1 = -1;
             for (int j = 0; j < take; ++j) {
                 const int id = ids[ci][cj + j], r = rows + j;
-                G.h_rows[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+                if (!score) G.h_rows[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
+                else {
+                    G.h_rows[r] = SessionSlot{n_past[ci] + cj + j, 0, X.kcache_, X.vcache_, G.score_logits + (size_t)r * V, G.score_state};
+                    const int jj = cj + j;
+                    if (jj == 0 && n_past[ci] > 0) {   // entry 0: the logits the context holds now (read before any tail of this call)
+                        G.h_score_rows[ent_ctx.size()] = k::ScoreRow{X.logits_, id, 0};
+                        ent_ctx.push_back(ci); ent_j.push_back(0);
+                    } else if (jj == 0) {
+                        score->logprob[ci][0] = NAN;
+                        if (score->rank) score->rank[ci][0] = -1;
+                    }
+                    if (jj + 1 < n_rows[ci]) {         // entry jj + 1: this row's logits
+                        G.h_score_rows[ent_ctx.size()] = k::ScoreRow{G.score_logits + (size_t)r * V, ids[ci][jj + 1], 0};
+                        ent_ctx.push_back(ci); ent_j.push_back(jj + 1);
+                    }
+                }
                 if (id >= 0) pid[(size_t)r] = id;
                 else {
                     const int k = -1 - id;
@@ -970,21 +1008,43 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
                 CUDA_CHECK(cudaMemcpyAsync(L0.embd_in_ + (size_t)n_emb * E, emb[ci] + (size_t)k0 * E, (size_t)(k1 - k0 + 1) * E * 4, cudaMemcpyHostToDevice, s));
                 n_emb += k1 - k0 + 1;
             }
+            run_ctx[nr] = ci; run_j[nr] = cj; run_row[nr] = rows; run_n[nr] = take; ++nr;
             rows += take; cj += take;
             if (cj < n_rows[ci]) break;   // the context continues in the next pass
             G.h_slots[nf] = SessionSlot{n_past[ci] + n_rows[ci] - 1, 0, X.kcache_, X.vcache_, X.logits_, X.state_};
             last[nf] = rows - 1; fin_ctx[nf] = ci; fin_first[nf] = rows - take;
             ++nf;
         }
+        const bool tail = nf && (!score || score->keep);
         CUDA_CHECK(cudaMemcpyAsync(G.rows, G.h_rows, (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(L0.tok_ids_, pid.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s));
-        if (nf) CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)nf * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+        if (tail) CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)nf * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
         embed_rows_kernel<<<rows, 256, 0, s>>>(L0.tok_type_, (const unsigned char *)L0.tok_raw_, gg_row_bytes(L0.tok_type_, (size_t)E), E, L0.tok_ids_, L0.embd_in_, G.x);
         ++L0.launches_;
         L0.record_layers(Pass{rows, G.x, G.q, G.att, G.act, G.qact, G.state, G.rows, L0.pf_ready_ && rows >= 2, s, &L0.launches_});
 
+        // ---- scoring: every row's logits into the scratch, the entries of this pass, results and logits rows to the host
+        const int ne = (int)ent_ctx.size();
+        if (score) {
+            for (int t0 = 0; t0 < rows; t0 += 8) {
+                MatvecArgs o = mv_args(L0.output_, std::min(8, rows - t0), G.state, G.qact, L0.tab_silu_);
+                o.x = G.x + (size_t)t0 * E; o.x_stride = E; o.norm_w = L0.final_norm_; o.epi = EPI_LOGITS; o.n_valid = (int)V;
+                launch_matvec(o, L0.sm_count_, s, &L0.launches_, G.rows + t0, 0);
+            }
+            if (ne) {
+                CUDA_CHECK(cudaMemcpyAsync(G.score_rows, G.h_score_rows, (size_t)ne * sizeof(k::ScoreRow), cudaMemcpyHostToDevice, s));
+                score_rows_kernel<<<ne, 256, 0, s>>>(G.score_rows, (int)V, G.score_out);
+                CUDA_CHECK(cudaGetLastError()); ++L0.launches_;
+                CUDA_CHECK(cudaMemcpyAsync(G.h_score_out, G.score_out, (size_t)ne * sizeof(k::ScoreOut), cudaMemcpyDeviceToHost, s));
+            }
+            if (score->logits)
+                for (int u = 0; u < nr; ++u)
+                    CUDA_CHECK(cudaMemcpyAsync(score->logits[run_ctx[u]] + (size_t)run_j[u] * V, G.score_logits + (size_t)run_row[u] * V,
+                                               (size_t)run_n[u] * V * 4, cudaMemcpyDeviceToHost, s));
+        }
+
         // ---- contexts that end in this pass, 8 at a time: logits + arg-max of their last row, DeviceState; then hidden rows, pinned arg-max
-        if (nf) {
+        if (tail) {
             for (int f0 = 0; f0 < nf; f0 += 8) {
                 const int m = std::min(8, nf - f0);
                 RowList lr{};
@@ -1004,8 +1064,31 @@ void LlamaDevice::eval_rows_batch(LlamaDevice *const *c, int n, const int32_t *c
             }
         }
         CUDA_CHECK(cudaStreamSynchronize(s));   // (the pinned tables and the shared workspace are reused by the next pass)
-        for (int f = 0; f < nf; ++f) *c[fin_ctx[f]]->h_argmax_ = G.h_ids[f];
+        if (tail) for (int f = 0; f < nf; ++f) *c[fin_ctx[f]]->h_argmax_ = G.h_ids[f];
+        for (int e = 0; e < ne; ++e) {
+            score->logprob[ent_ctx[(size_t)e]][ent_j[(size_t)e]] = G.h_score_out[e].logprob;
+            if (score->rank) score->rank[ent_ctx[(size_t)e]][ent_j[(size_t)e]] = G.h_score_out[e].rank;
+        }
     }
+}
+
+void LlamaDevice::build_score_scratch() {
+    LlamaGroup &G = *group_;
+    const size_t b0 = t_dev_bytes, R = (size_t)kPrefillMax, NE = R + kMaxBatch;
+    dmalloc(&G.score_logits, R * (size_t)d_.n_vocab * 4);
+    dmalloc(&G.score_state, sizeof(DeviceState)); CUDA_CHECK(cudaMemset(G.score_state, 0, sizeof(DeviceState)));
+    dmalloc(&G.score_rows, NE * sizeof(k::ScoreRow));
+    dmalloc(&G.score_out, NE * sizeof(k::ScoreOut));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_score_rows, NE * sizeof(k::ScoreRow), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_score_out, NE * sizeof(k::ScoreOut), cudaHostAllocDefault));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    G.batch_bytes += t_dev_bytes - b0;
+}
+
+void LlamaDevice::score_rows(LlamaDevice *const *c, int n, const int32_t *const *ids, const int *n_ids, const int *n_past, bool keep,
+                             float *const *logprob, int32_t *const *rank, float *const *logits) {
+    const ScoreCall sc{keep, logprob, rank, logits};
+    eval_rows_batch(c, n, ids, n_ids, nullptr, n_past, &sc);
 }
 
 // measurement seam: average CUDA-event duration (us) of one all-reduce of a [1, n_embd] partial on the tensor-parallel path in use

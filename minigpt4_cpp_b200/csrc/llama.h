@@ -60,6 +60,7 @@ struct ReplyScratch;   // a context's stop state in sample_until: reply tail, st
 namespace smp { template <int N> struct SampleArgsN; }
 
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
+struct ScoreCall;      // the outputs of a score_rows call, which eval_rows_batch's passes fill (llama.cu)
 
 class LlamaDevice {
 public:
@@ -88,7 +89,20 @@ public:
     // emb[i] (n_embd floats per row, in order of first use).  Afterwards each context holds what its own eval_rows would have left
     // (KV cache, logits, arg-max, DeviceState) and the first rows of its hidden state are its rows of the pass that evaluated its
     // last row.  Synchronous.  The caller validates (distinct, one group, rows checked when they were queued).
-    static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past);
+    // score (score_rows): every row's logits go to the group's scoring scratch and its entries are scored; without score->keep the
+    // contexts' logits, DeviceState, arg-max and hidden rows are left as they were.
+    static void eval_rows_batch(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_rows, const float *const *emb, const int *n_past,
+                                const ScoreCall *score = nullptr);
+    // Score known ids against n (1..kMaxBatch) distinct contexts of one group: context i's n_ids[i] (>= 1) token ids are evaluated at
+    // positions n_past[i] .. in the shared passes of eval_rows_batch, and every row's logits are computed (llama_score.cuh).  Entry j of
+    // context i: logprob[i][j] = log p(ids[i][j]) under the logits before row j (j = 0: the context's current logits; NaN and rank -1 when
+    // n_past[i] = 0), rank[i][j] (rank may be null) = the ids ranked above it (larger logit, or equal logit and lower id), logits[i]
+    // (logits may be null) = n_ids[i] rows of n_vocab floats, row j the logits of row j.  keep: afterwards each context holds what
+    // eval_rows_batch of these rows leaves; otherwise the call changes nothing of a context but its K / V rows at positions >= n_past[i].
+    // The group's first call allocates the scoring scratch (kPrefillMax rows of logits, counted in shared_bytes).  Synchronous.  The
+    // caller validates (distinct, one group, ids in range, room in each context).
+    static void score_rows(LlamaDevice *const *ctx, int n, const int32_t *const *ids, const int *n_ids, const int *n_past, bool keep,
+                           float *const *logprob, int32_t *const *rank, float *const *logits);
     // `steps` sampled decode steps of n (1..kMaxBatch) distinct contexts of one group with no host round trip: each step samples every context's
     // current logits on the device (llama_sample.cuh; p.temp <= 0: the greedy id) into its DeviceState, then runs the decode step (n = 1:
     // the context's own graph or megakernel; n >= 2: the batch graph, every column fed its DeviceState::tokens[0]).  rng[i] holds context
@@ -225,6 +239,7 @@ private:
     void free_weights();             // by the last context of the group
     void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)
     void build_batch_graph(int B);   // decode_batch's graph for B columns, captured on the group stream
+    void build_score_scratch();      // score_rows' logits rows, entry tables and results (group-owned, at the first scoring call)
 };
 
 }  // namespace mg4

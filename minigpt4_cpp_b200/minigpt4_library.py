@@ -220,6 +220,7 @@ _EXT = {
     "minigpt4_b200_session_info": ([_CTX, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "minigpt4_b200_decode_batch": ([_VP, _I, _VP, _VP], _I),
     "minigpt4_b200_flush_batch": ([_VP, _I], _I),
+    "minigpt4_b200_score_tokens": ([_VP, _I, _VP, _VP, _I, _VP, _VP, _VP], _I),
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
@@ -347,6 +348,24 @@ class B200:
     def flush_batch(self, ctxs) -> None:
         """evaluate the queued prompt rows of every context in `ctxs` (1..64 of one group) in shared passes over the weights"""
         self._chk(self.L.minigpt4_b200_flush_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), len(ctxs)))
+
+    def score_tokens(self, ctxs, id_lists, keep: bool = False, logits: bool = False) -> list[tuple]:
+        """the log-probability and rank of every id of id_lists[i] (>= 1 ids) as a continuation of context ctxs[i] (1..64 of one group), in
+        shared passes over the weights; per context (logprob float32, rank int32[, logits float32 [n_ids, n_vocab]]).  Entry 0 is NaN with
+        rank -1 on a context at n_past 0.  keep: the ids stay evaluated (as eval_tokens + flush); otherwise every context is left as it was."""
+        n = len(ctxs)
+        lens = np.array([len(x) for x in id_lists], np.int32)
+        ids = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32).ravel() for x in id_lists]) if n else np.zeros(0, np.int32), np.int32)
+        total = max(1, int(lens.sum()))
+        lp, rk = np.empty(total, np.float32), np.empty(total, np.int32)
+        lg = np.empty((total, self.L.minigpt4_b200_n_vocab(ctxs[0].ptr)), np.float32) if logits and n else None
+        self._chk(self.L.minigpt4_b200_score_tokens(C.cast(self._ctx_array(ctxs), C.c_void_p), n, _ptr(ids), _ptr(lens), int(keep), _ptr(lp),
+                                                    _ptr(rk), _ptr(lg)))
+        out, o = [], 0
+        for k in lens.tolist():
+            out.append((lp[o:o + k], rk[o:o + k]) + ((lg[o:o + k],) if logits else ()))
+            o += k
+        return out
 
     def end_chat_batch(self, ctxs, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
                        repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 1.0, alpha_frequency: float = 1.0,
