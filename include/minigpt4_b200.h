@@ -187,6 +187,11 @@ MINIGPT4_API int minigpt4_b200_op_gemm_f16(int M, int T, int K, const void *w_f1
 MINIGPT4_API int minigpt4_b200_op_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out);
 /* q,k,v: [n][heads*dh]; out [nq][heads*dh] rounded to F16 precision */
 MINIGPT4_API int minigpt4_b200_op_attention(const float *q, const float *k, const float *v, int nq, int nk, int heads, int dh, float score_div, float *out);
+/* the LLaMA attention of the decode step and prompt passes: q F32 [rows][n_head*128], k_f16 / v_f16 F16 caches [n_ctx][n_head*128]
+ * (row t sees keys 0 .. its position; rows above are never read), out F32 [rows][n_head*128].  path 0: the single-context kernel, row t
+ * at pos[0] + t; path 1: the batched kernel, row t at pos[t].  8 (FailedToAddString) on arguments out of range, before any device work */
+MINIGPT4_API int minigpt4_b200_op_llama_attention(const float *q, const void *k_f16, const void *v_f16, int n_head, int n_ctx, int rows, const int32_t *pos,
+                                                  int path, float *out);
 
 /* out_f16[n] = the F16 operand the vision graph builds at load time from a non-F16 matrix: `raw` holds n elements as ggml blocks of
  * `ggml_type` (0 F32, 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0); values follow ggml's dequantize_row_* and are rounded to F16 */

@@ -300,6 +300,12 @@ int minigpt4_b200_op_attention(const float *q, const float *k, const float *v, i
     VisionDevice::test_attention(q, k, v, nq, nk, heads, dh, score_div, out); return 0;
 }
 
+int minigpt4_b200_op_llama_attention(const float *q, const void *k_f16, const void *v_f16, int n_head, int n_ctx, int rows, const int32_t *pos, int path,
+                                     float *out) {
+    if (!q || !k_f16 || !v_f16 || !pos || !out) return ErrFailedToAddString;
+    return LlamaDevice::test_attention(q, (const uint16_t *)k_f16, (const uint16_t *)v_f16, n_head, n_ctx, rows, pos, path, out) ? 0 : ErrFailedToAddString;
+}
+
 int minigpt4_b200_op_dequant_f16(int ggml_type, const void *raw, long n, void *out_f16) { return VisionDevice::test_dequant(ggml_type, raw, n, out_f16); }
 extern "C" long mg4_quantize_row(int gg_type, const float *x, long n, unsigned char *out);
 long minigpt4_b200_host_quantize_row(int ggml_type, const float *x, long n, void *out_blocks) { return mg4_quantize_row(ggml_type, x, n, (unsigned char *)out_blocks); }

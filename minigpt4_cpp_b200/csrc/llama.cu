@@ -299,6 +299,10 @@ void LlamaDevice::free_weights() {
 
 static inline unsigned short f2h_bits(float f) { __half h = __float2half_rn(f); unsigned short u; memcpy(&u, &h, 2); return u; }
 static inline float h2f_bits(unsigned short u) { __half h; memcpy(&h, &u, 2); return __half2float(h); }
+// ggml's fp16 lookup tables of exp and silu (ggml_init), [65536] each, indexed by the F16 bits of the argument
+static void fp16_tables(unsigned short *te, unsigned short *ts) {
+    for (int i = 0; i < 65536; ++i) { const float x = h2f_bits((unsigned short)i); te[i] = f2h_bits(expf(x)); ts[i] = f2h_bits(x / (1.0f + expf(-x))); }
+}
 
 bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     tp_ = tp;
@@ -372,7 +376,7 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     // ggml's fp16 lookup tables (ggml_init): exp and silu, computed with the host libm exactly as ggml does
     {
         std::vector<unsigned short> te(65536), ts(65536);
-        for (int i = 0; i < 65536; ++i) { const float x = h2f_bits((unsigned short)i); te[(size_t)i] = f2h_bits(expf(x)); ts[(size_t)i] = f2h_bits(x / (1.0f + expf(-x))); }
+        fp16_tables(te.data(), ts.data());
         dmalloc(&tab_exp_, 131072); CUDA_CHECK(cudaMemcpy(tab_exp_, te.data(), 131072, cudaMemcpyHostToDevice));
         dmalloc(&tab_silu_, 131072); CUDA_CHECK(cudaMemcpy(tab_silu_, ts.data(), 131072, cudaMemcpyHostToDevice));
     }
@@ -1193,6 +1197,40 @@ void LlamaDevice::test_matvec(int gg, int rows, int cols, const void *w_host, co
     cudaFree(x); cudaFree(y); cudaFree(stt); cudaFree(stg); qmat_free(m);
 }
 
+// kernel-level test hook of the decode / prompt attention: attn_kernel (path 0, row t at pos[0] + t, the single-context graphs) or
+// attn_sessions_kernel (path 1, row t at pos[t] through a slot table, the batched passes) over caller-supplied F16 caches
+bool LlamaDevice::test_attention(const float *q_host, const uint16_t *k_host, const uint16_t *v_host, int n_head, int n_ctx, int rows, const int *pos,
+                                 int path, float *out_host) {
+    if (n_head < 1 || n_head > 128 || n_ctx < 8 || n_ctx > 32768 || rows < 1 || rows > 65535 || (path != 0 && path != 1)) return false;
+    for (int t = 0; t < rows; ++t) if (pos[t] < 0 || pos[t] >= n_ctx) return false;
+    if (path == 0 && pos[0] + rows > n_ctx) return false;
+    const int E = n_head * 128;
+    const float kq_scale = 1.0f / sqrtf((float)E / (float)n_head);   // record_layers' expression
+    const size_t kv = (size_t)n_ctx * E;
+    std::vector<unsigned short> te(65536), ts(65536);
+    fp16_tables(te.data(), ts.data());
+    float *q, *out; __half *kc, *vc, *tab_exp; DeviceState *st; SessionSlot *slots;
+    CUDA_CHECK(cudaMalloc((void **)&q, (size_t)rows * E * 4)); CUDA_CHECK(cudaMalloc((void **)&out, (size_t)rows * E * 4));
+    CUDA_CHECK(cudaMalloc((void **)&kc, kv * 2)); CUDA_CHECK(cudaMalloc((void **)&vc, kv * 2)); CUDA_CHECK(cudaMalloc((void **)&tab_exp, 131072));
+    CUDA_CHECK(cudaMalloc((void **)&st, sizeof(DeviceState))); CUDA_CHECK(cudaMalloc((void **)&slots, (size_t)rows * sizeof(SessionSlot)));
+    CUDA_CHECK(cudaMemcpy(q, q_host, (size_t)rows * E * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(kc, k_host, kv * 2, cudaMemcpyHostToDevice)); CUDA_CHECK(cudaMemcpy(vc, v_host, kv * 2, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(tab_exp, te.data(), 131072, cudaMemcpyHostToDevice));
+    DeviceState h_st{}; h_st.n_past = pos[0];
+    CUDA_CHECK(cudaMemcpy(st, &h_st, sizeof(DeviceState), cudaMemcpyHostToDevice));
+    std::vector<SessionSlot> h_slots((size_t)rows);
+    for (int t = 0; t < rows; ++t) { SessionSlot &s = h_slots[(size_t)t]; s = SessionSlot{}; s.n_past = pos[t]; s.kcache = kc; s.vcache = vc; s.state = st; }
+    CUDA_CHECK(cudaMemcpy(slots, h_slots.data(), (size_t)rows * sizeof(SessionSlot), cudaMemcpyHostToDevice));
+    attn_smem(n_ctx);
+    const dim3 ag((unsigned)n_head, (unsigned)rows);
+    if (path == 1) attn_sessions_kernel<<<ag, 256, (size_t)n_ctx * 6>>>(q, slots, 0, out, E, n_ctx, kq_scale, tab_exp);
+    else attn_kernel<<<ag, 256, (size_t)n_ctx * 6>>>(q, kc, vc, out, st, E, n_ctx, kq_scale, tab_exp);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaDeviceSynchronize());
+    CUDA_CHECK(cudaMemcpy(out_host, out, (size_t)rows * E * 4, cudaMemcpyDeviceToHost));
+    for (void *p : {(void *)q, (void *)out, (void *)kc, (void *)vc, (void *)tab_exp, (void *)st, (void *)slots}) cudaFree(p);
+    return true;
+}
 
 void LlamaDevice::ensure_sampler() {
     if (smp_) return;

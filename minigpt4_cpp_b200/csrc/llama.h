@@ -159,6 +159,11 @@ public:
     // kernel-level test hook: y[n][rows] = W x (W given as raw ggml blocks on host), through the same
     // repack + matvec kernels the engine uses.
     static void test_matvec(int gg, int rows, int cols, const void *w_host, const float *x_host, int n, float *y_host);
+    // kernel-level test hook: the LLaMA attention of `rows` rows (q F32 [rows][n_head * 128]) over F16 K / V caches [n_ctx][n_head * 128]
+    // uploaded from the host, with the exp table load() builds; path 0: attn_kernel, row t at position pos[0] + t; path 1:
+    // attn_sessions_kernel through a slot table, row t at pos[t].  false (nothing launched) on arguments outside those ranges.
+    static bool test_attention(const float *q_host, const uint16_t *k_host, const uint16_t *v_host, int n_head, int n_ctx, int rows, const int *pos,
+                               int path, float *out_host);
     // sampler test hook: n_draws draws from one generator (rng: 624 words and the position) over the same n_vocab logits, as n_draws calls
     // of Sampler::sample make (p.temp > 0); kernel_ms (optional): the average CUDA-event time of one sampling launch.  With p.mirostat
     // 1 / 2, μ starts unset and mu_out (optional) takes μ after each draw (a 4-byte device copy after each launch, inside the timing).

@@ -234,6 +234,7 @@ _EXT = {
     "minigpt4_b200_op_gemm_f16": ([_I, _I, _I, _VP, _VP, _VP, _I, _VP], _I),
     "minigpt4_b200_op_layernorm": ([_VP, _I, _I, _VP, _VP, _VP], _I),
     "minigpt4_b200_op_attention": ([_VP, _VP, _VP, _I, _I, _I, _I, _F, _VP], _I),
+    "minigpt4_b200_op_llama_attention": ([_VP, _VP, _VP, _I, _I, _I, _VP, _I, _VP], _I),
     "minigpt4_b200_op_dequant_f16": ([_I, _VP, C.c_long, _VP], _I),
     "minigpt4_b200_host_quantize_row": ([_I, _VP, C.c_long, _VP], C.c_long),
     "minigpt4_b200_host_tokenize": ([_S, _S, _I, _VP, _I], _I),
@@ -560,6 +561,17 @@ class B200:
         q = np.ascontiguousarray(q, np.float32); k = np.ascontiguousarray(k, np.float32); v = np.ascontiguousarray(v, np.float32)
         out = np.empty_like(q)
         self._chk(self.L.minigpt4_b200_op_attention(_ptr(q), _ptr(k), _ptr(v), q.shape[0], k.shape[0], heads, dh, div, _ptr(out)))
+        return out
+
+    def op_llama_attention(self, q, k, v, pos, path: int) -> np.ndarray:
+        """q float32 [rows][n_head * 128], k / v float16 [n_ctx][n_head * 128]; path 0: row t at pos[0] + t (pos may be one int), path 1:
+        row t at pos[t]"""
+        q = np.ascontiguousarray(q, np.float32)
+        k = np.ascontiguousarray(k, np.float16); v = np.ascontiguousarray(v, np.float16)
+        rows = q.shape[0]
+        pos = np.full(rows, pos, np.int32) if np.ndim(pos) == 0 else np.ascontiguousarray(pos, np.int32)
+        out = np.zeros_like(q)
+        self._chk(self.L.minigpt4_b200_op_llama_attention(_ptr(q), _ptr(k), _ptr(v), k.shape[1] // 128, k.shape[0], rows, _ptr(pos), path, _ptr(out)))
         return out
 
 

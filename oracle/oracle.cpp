@@ -912,6 +912,46 @@ ORACLE_API void *oracle_llama_new(void *model, int n_ctx) {
 ORACLE_API void oracle_llama_free(void *l) { delete (Llama *)l; }
 ORACLE_API void oracle_llama_set_nhead(void *l, int n_head) { Llama *L = (Llama *)l; L->n_head = n_head; L->hd = L->n_embd / n_head; }
 
+// one head of one row of LLaMA attention over keys 0 .. nvis - 1 of an F16 cache with row stride E (kr / vr point at the head's first
+// column); q is rounded to F16 and the soft-max probabilities too (ggml semantics).
+// canonical orders = csrc/llama_kernels.cuh attention_head: 16 lanes x 8 dims per key then a 16-lane butterfly;
+// soft-max sum: 256 strided double partials + block_sum_256; P.V: 16 key groups (key mod 16), combined by a pairwise tree
+static void attention_row(const float *q, const f16_t *kr, const f16_t *vr, int E, int nvis, int hd, float kq_scale, float *out) {
+    std::vector<f16_t> qh(hd), ph(nvis); std::vector<float> pr(nvis);
+    for (int d = 0; d < hd; ++d) qh[d] = f2h(q[d]);
+    for (int t = 0; t < nvis; ++t) {
+        const f16_t *k = &kr[(size_t)t * E];
+        float lane[16];
+        for (int l = 0; l < 16; ++l) { float sacc = 0.f; for (int e = 0; e < 8; ++e) sacc = fmaf(h2f(k[l * 8 + e]), h2f(qh[l * 8 + e]), sacc); lane[l] = sacc; }
+        pr[t] = butterfly(lane, 16) * kq_scale;
+    }
+    float mx = -INFINITY; for (int t = 0; t < nvis; ++t) mx = fmaxf(mx, pr[t]);
+    double part[256];
+    for (int tt = 0; tt < 256; ++tt) { double sacc = 0; for (int t = tt; t < nvis; t += 256) { const float e = h2f(g_tab_exp[f2h(pr[t] - mx)]); pr[t] = e; sacc += (double)e; } part[tt] = sacc; }
+    const float inv = (float)(1.0 / block_sum_256(part));
+    for (int t = 0; t < nvis; ++t) ph[t] = f2h(pr[t] * inv);
+    for (int d = 0; d < hd; ++d) {
+        float g16[16];
+        for (int g = 0; g < 16; ++g) g16[g] = 0.f;
+        for (int t = 0; t < nvis; ++t) g16[t & 15] = fmaf(h2f(vr[(size_t)t * E + d]), h2f(ph[t]), g16[t & 15]);
+        for (int st = 1; st < 16; st <<= 1) for (int g = 0; g < 16; g += 2 * st) g16[g] = g16[g] + g16[g + st];  // pairwise tree
+        out[d] = g16[0];
+    }
+}
+
+// the attention op of the language graph by itself: q F32 [rows][n_head * 128], k / v F16 [n_ctx][n_head * 128], row t at position pos[t]
+// (it sees keys 0 .. pos[t]); out F32 [rows][n_head * 128].  Returns 1 on a position outside the cache.
+ORACLE_API int oracle_llama_attention(const float *q, const f16_t *k, const f16_t *v, int n_head, int n_ctx, int rows, const int *pos, int n_threads, float *out) {
+    for (int t = 0; t < rows; ++t) if (pos[t] < 0 || pos[t] >= n_ctx) return 1;
+    if (n_threads > 0) omp_set_num_threads(n_threads);
+    const int hd = 128, E = n_head * hd;
+    const float kq_scale = 1.0f / sqrtf((float)E / n_head);
+#pragma omp parallel for schedule(dynamic) collapse(2)
+    for (int h = 0; h < n_head; ++h) for (int t = 0; t < rows; ++t)
+        attention_row(&q[(size_t)t * E + h * hd], k + h * hd, v + h * hd, E, pos[t] + 1, hd, kq_scale, &out[(size_t)t * E + h * hd]);
+    return 0;
+}
+
 // tokens != NULL -> llama_eval; else embd (F32 [N][n_embd]) -> llama_eval_embd.  Keeps last row's logits.
 // all_logits (optional): F32 [N][n_vocab] for every row (test aid; the reference keeps only the last).
 ORACLE_API int oracle_llama_eval(void *l, const int32_t *tokens, const float *embd, int N, int n_past, int n_threads, float *logits_out, float *hidden_tap, int tap_layer) {
@@ -941,33 +981,9 @@ ORACLE_API int oracle_llama_eval(void *l, const int32_t *tokens, const float *em
         }
         f16_t *kc = &L->kc[(size_t)il * C * E], *vc = &L->vc[(size_t)il * C * E];
         for (int i = 0; i < N; ++i) for (int e = 0; e < E; ++e) { kc[(size_t)(n_past + i) * E + e] = f2h(k[(size_t)i * E + e]); vc[(size_t)(n_past + i) * E + e] = f2h(vv[(size_t)i * E + e]); }
-        const int nkv = n_past + N;
 #pragma omp parallel for schedule(dynamic) collapse(2)
-        for (int h = 0; h < H; ++h) for (int i = 0; i < N; ++i) {
-            // canonical orders = csrc/llama_kernels.cuh attn_kernel: 16 lanes x 8 dims per key then a 16-lane butterfly;
-            // soft-max sum: 256 strided double partials + block_sum_256; P.V: 16 key groups (key mod 16), combined by a pairwise tree
-            std::vector<f16_t> qh(hd), ph(nkv); std::vector<float> pr(nkv);
-            for (int d = 0; d < hd; ++d) qh[d] = f2h(q[(size_t)i * E + h * hd + d]);
-            const int nvis = n_past + i + 1;  // keys visible to this row (ggml_diag_mask_inf masks the rest to -inf -> 0)
-            for (int t = 0; t < nvis; ++t) {
-                const f16_t *kr = &kc[(size_t)t * E + h * hd];
-                float lane[16];
-                for (int l = 0; l < 16; ++l) { float sacc = 0.f; for (int e = 0; e < 8; ++e) sacc = fmaf(h2f(kr[l * 8 + e]), h2f(qh[l * 8 + e]), sacc); lane[l] = sacc; }
-                pr[t] = butterfly(lane, 16) * kq_scale;
-            }
-            float mx = -INFINITY; for (int t = 0; t < nvis; ++t) mx = fmaxf(mx, pr[t]);
-            double part[256];
-            for (int tt = 0; tt < 256; ++tt) { double sacc = 0; for (int t = tt; t < nvis; t += 256) { const float e = h2f(g_tab_exp[f2h(pr[t] - mx)]); pr[t] = e; sacc += (double)e; } part[tt] = sacc; }
-            const float inv = (float)(1.0 / block_sum_256(part));
-            for (int t = 0; t < nvis; ++t) ph[t] = f2h(pr[t] * inv);
-            for (int d = 0; d < hd; ++d) {
-                float g16[16];
-                for (int g = 0; g < 16; ++g) g16[g] = 0.f;
-                for (int t = 0; t < nvis; ++t) g16[t & 15] = fmaf(h2f(vc[(size_t)t * E + h * hd + d]), h2f(ph[t]), g16[t & 15]);
-                for (int st = 1; st < 16; st <<= 1) for (int g = 0; g < 16; g += 2 * st) g16[g] = g16[g] + g16[g + st];  // pairwise tree
-                att[(size_t)i * E + h * hd + d] = g16[0];
-            }
-        }
+        for (int h = 0; h < H; ++h) for (int i = 0; i < N; ++i)  // row i sees keys 0 .. n_past + i (ggml_diag_mask_inf masks the rest to -inf -> 0)
+            attention_row(&q[(size_t)i * E + h * hd], kc + h * hd, vc + h * hd, E, n_past + i + 1, hd, kq_scale, &att[(size_t)i * E + h * hd]);
         mul_mat(T(m, p + "attention.wo.weight"), att.data(), N, cur.data(), true);
         for (size_t i = 0; i < (size_t)N * E; ++i) inp[i] = cur[i] + inp[i];  // inpFF
         op_rms_norm_mul(inp.data(), cur.data(), E, N, F(m, p + "ffn_norm.weight"));

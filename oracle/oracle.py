@@ -68,6 +68,7 @@ def lib() -> ctypes.CDLL:
         L.oracle_llama_new.restype = vp
         L.oracle_llama_free.argtypes = [vp]
         L.oracle_llama_eval.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, i32]
+        L.oracle_llama_attention.argtypes = [vp, vp, vp, i32, i32, i32, vp, i32, vp]
         L.oracle_llama_n_vocab.argtypes = [vp]
         L.oracle_llama_n_embd.argtypes = [vp]
         L.oracle_mul_mat.argtypes = [i32, i64, i64, vp, vp, i32, vp]
@@ -364,6 +365,18 @@ def mul_mat(gtype: int, w_raw: np.ndarray, rows: int, cols: int, x: np.ndarray) 
     w_raw = np.ascontiguousarray(w_raw)
     lib().oracle_mul_mat(gtype, rows, cols, _p(w_raw), _p(x), x.shape[0], _p(y))
     return y
+
+
+def llama_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, pos) -> np.ndarray:
+    """the language graph's attention op: q float32 [rows][n_head * 128], k / v float16 [n_ctx][n_head * 128]; row t sees keys 0 .. pos[t]"""
+    q = np.ascontiguousarray(q, np.float32)
+    k = np.ascontiguousarray(k, np.float16); v = np.ascontiguousarray(v, np.float16)
+    pos = np.ascontiguousarray(pos, np.int32).reshape(-1)
+    assert k.shape == v.shape and q.shape == (pos.size, k.shape[1]) and k.shape[1] % 128 == 0
+    out = np.zeros_like(q)
+    if lib().oracle_llama_attention(_p(q), _p(k), _p(v), k.shape[1] // 128, k.shape[0], pos.size, _p(pos), usable_cpus(), _p(out)):
+        raise ValueError("a position lies outside the cache")
+    return out
 
 
 def dequant_rows(gtype: int, w_raw: np.ndarray, rows: int, cols: int) -> np.ndarray:

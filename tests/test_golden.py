@@ -61,5 +61,6 @@ def test_independent_crosscheck_is_within_bounds():
     r = json.loads((GOLD / "crosscheck.json").read_text())
     assert r["vision_ln_vision_rel_err"] < 2e-3 and r["qformer_proj_rel_err"] < 2e-3
     assert r["llama_f16_logits_rel_err"] < 2e-3 and r["llama_f16_argmax_equal"]
+    assert r["llama_f16_long_logits_rel_err"] < 2e-3 and r["llama_f16_long_argmax_equal"]   # 2048 tokens: positions to 2047
     assert r["llama_q4_1_logits_rel_err"] < 2e-2 and r["llama_q4_1_argmax_equal"]  # Q8 activation quantisation is deliberate
     assert r["vision_missing_keys"] == [] and r["qformer_missing_keys"] == []

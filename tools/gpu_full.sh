@@ -6,7 +6,7 @@ mkdir -p "$OUT"
 run() { name=$1; shift; t=$1; shift; echo "=== $name"; timeout -k 5 $t "$@" > "$OUT/$name.log" 2>&1; rc=$?; echo "exit $rc"; tail -n ${TAILN:-12} "$OUT/$name.log"; return $rc; }
 nvidia-smi --query-gpu=name,power.limit,clocks.max.sm --format=csv > "$OUT/gpu.csv"
 TAILN=6 run canary6 300 python tools/canary.py || exit 1
-TAILN=8 run pytest_gpu 900 python -m pytest tests -m gpu -q -p no:cacheprovider
+TAILN=8 run pytest_gpu 1200 python -m pytest tests -m gpu -q -p no:cacheprovider
 TAILN=3 run prefill_plain 300 python tools/prof_prefill.py
 TAILN=3 run bench 600 python bench.py
 TAILN=3 run bench_reference 600 python bench.py --impl reference --steps 2 --warmup 1

@@ -26,6 +26,7 @@ from oracle import oracle as orc  # noqa: E402
 GOLD = ROOT / "tests" / "golden"
 TEXTS = ["Human: <Img>", "</Img> ", "### Assistant:", "what is this?", "héllo wörld ✓", "Give the following image: <Img>ImageContent</Img>."]
 TOKENS = [1, 266, 61, 35, 63, 316, 65, 17, 900, 511, 3, 258, 700]
+LONG_TOKENS = 2048   # the long cross-check: the F16 model over a whole n_ctx 2048 context
 
 VISION_SPEC = dict(n_blocks=2, n_qformer_layers=2, n_embd_llm=4096)
 LLAMA_SPECS = {
@@ -151,7 +152,7 @@ def crosscheck_transformers(d: Path) -> dict:
             return w.view(H, E // H // 2, 2, E).transpose(1, 2).reshape(E, E)
 
         lc = LlamaConfig(vocab_size=spec.n_vocab, hidden_size=E, intermediate_size=spec.n_ff, num_hidden_layers=spec.n_layer, num_attention_heads=H,
-                         num_key_value_heads=H, rms_norm_eps=1e-6, rope_theta=10000.0, max_position_embeddings=256, tie_word_embeddings=False, attention_bias=False)
+                         num_key_value_heads=H, rms_norm_eps=1e-6, rope_theta=10000.0, max_position_embeddings=LONG_TOKENS, tie_word_embeddings=False, attention_bias=False)
         lm = LlamaForCausalLM(lc).eval().float()
         lsd = {"model.embed_tokens.weight": W("tok_embeddings.weight"), "model.norm.weight": W("norm.weight"), "lm_head.weight": W("output.weight")}
         for i in range(spec.n_layer):
@@ -168,6 +169,13 @@ def crosscheck_transformers(d: Path) -> dict:
         e.eval_tokens(TOKENS)
         res[f"llama_{name}_logits_rel_err"] = float(np.abs(hf_logits - e.logits).max() / np.abs(hf_logits).max())
         res[f"llama_{name}_argmax_equal"] = bool(int(np.argmax(hf_logits)) == int(np.argmax(e.logits)))
+        if name == "f16":   # a whole 2048-token context: RoPE, attention and the soft-max sum up to the last position
+            ids = np.random.default_rng(LONG_TOKENS).integers(3, spec.n_vocab, size=LONG_TOKENS)
+            hf_logits = lm(torch.from_numpy(ids)[None]).logits[0, -1].numpy()
+            e = orc.OracleEngine(None, str(p), n_ctx=LONG_TOKENS)
+            e.eval_tokens(ids.tolist())
+            res["llama_f16_long_logits_rel_err"] = float(np.abs(hf_logits - e.logits).max() / np.abs(hf_logits).max())
+            res["llama_f16_long_argmax_equal"] = bool(int(np.argmax(hf_logits)) == int(np.argmax(e.logits)))
     return res
 
 
