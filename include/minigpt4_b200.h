@@ -102,6 +102,37 @@ MINIGPT4_API int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n)
  * error code (8) and change no context, before any device work. */
 MINIGPT4_API int minigpt4_b200_score_tokens(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, const int32_t *n_ids, int keep,
                                             float *logprob_out, int32_t *rank_out, float *logits_out);
+/* Copy the conversation of src into n (1..64) distinct other contexts of its group, so that several sessions continue one shared prefix
+ * (a system prompt, an image turn, best-of-N replies) without evaluating it again.  src's queued prompt pieces are evaluated first, by
+ * its own flush.  Afterwards every destination has src's conversation: n_past, K / V rows 0 .. n_past - 1 bit for bit, logits, greedy
+ * id, device state and the reply tail that minigpt4_b200_sample_until's stop rule reads; its queued pieces are discarded.  Its rows at
+ * positions >= n_past are left as they were: no kernel reads a key above a row's position, and the next evaluated row overwrites them.
+ * Each destination keeps its own sampler (generator and mirostat μ), so copies into sessions of different seeds draw different replies.
+ * The rows of minigpt4_b200_get_hidden are not carried.  src is left exactly as its flush left it.  The call first waits for the steps
+ * still running on every context involved (minigpt4_end_chat returns with its step running); it is synchronous and allocates nothing,
+ * so minigpt4_b200_session_info's bytes do not change.  One kernel launch reads each source row once and writes it to every destination.
+ * NULL src / dsts, n outside 1..64, NULL or duplicate destinations, src among them, a destination of another group or a tensor-parallel
+ * context return the FailedToAddString error code (8) before any device work, with no context changed (src's queue not evaluated).
+ * The _timed form also returns the CUDA-event time of the copy kernel (kernel_ms may be NULL). */
+MINIGPT4_API int minigpt4_b200_session_copy(struct MiniGPT4Context *src, struct MiniGPT4Context **dsts, int n);
+MINIGPT4_API int minigpt4_b200_session_copy_timed(struct MiniGPT4Context *src, struct MiniGPT4Context **dsts, int n, float *kernel_ms);
+/* Save a conversation to host memory and restore it, in this process or another, into any context whose model has the same fingerprint.
+ * state_size: the bytes state_save writes now (n_past counts the queued prompt rows; nothing is evaluated); -1 for NULL or a
+ * tensor-parallel ctx.  state_save: evaluates ctx's queue, then writes the state to buf and *written (may be NULL) = its size; cap below
+ * the size returns 8 and writes nothing (and evaluates nothing).  state_load: replaces ctx's conversation as minigpt4_b200_session_copy
+ * does (its sampler is kept, its queue discarded, its rows above n_past untouched); the state may come from any group, provided
+ * n_past <= ctx's n_ctx.  The K / V rows move with one copy per layer plane between buf and the cache, bound by the host link.
+ * The state is little-endian, 144 header bytes:
+ *   0 "MG4STATE"; 8 uint32 version 1; 12 int32 n_vocab, n_embd, n_head, n_layer, n_ff; 32 uint64 fingerprint of the model (FNV-1a 64
+ *   over the LLaMA tensor table, name, type and shape in name order, and the first 4096 bytes of each tensor's data); 40 int32 n_past;
+ *   44 int32 reply tail length (0..32); 48 the reply tail, 32 bytes; 80 the 64-byte device state (its n_past is the header's);
+ *   then 144: n_vocab float32 logits; then K[n_layer][n_past][n_embd] and V[n_layer][n_past][n_embd] as float16.
+ * state_load returns 8 and changes nothing, before any device work, for NULL arguments, a size shorter than the header or other than
+ * the header implies, a bad magic or version, other dimensions or fingerprint, n_past above ctx's n_ctx, a device state n_past that
+ * disagrees with the header or a reply tail over 32 bytes. */
+MINIGPT4_API long long minigpt4_b200_state_size(struct MiniGPT4Context *ctx);
+MINIGPT4_API int minigpt4_b200_state_save(struct MiniGPT4Context *ctx, void *buf, long long cap, long long *written);
+MINIGPT4_API int minigpt4_b200_state_load(struct MiniGPT4Context *ctx, const void *buf, long long size);
 /* minigpt4_end_chat on each context in turn (each samples from its own logits with its own sampler; greedy uses the device
  * arg-max; tokens[i] = the sampled token's text), then the n sampled ids are fed in one minigpt4_b200_decode_batch step.
  * The batch is validated before any sampling. */

@@ -228,6 +228,19 @@ int minigpt4_b200_score_tokens(struct MiniGPT4Context **ctxs, int n, const int32
                                int32_t *rank_out, float *logits_out) {
     return Engine::score_tokens(reinterpret_cast<Engine *const *>(ctxs), n, ids, n_ids, keep, logprob_out, rank_out, logits_out);
 }
+int minigpt4_b200_session_copy(struct MiniGPT4Context *src, struct MiniGPT4Context **dsts, int n) {
+    return minigpt4_b200_session_copy_timed(src, dsts, n, nullptr);
+}
+int minigpt4_b200_session_copy_timed(struct MiniGPT4Context *src, struct MiniGPT4Context **dsts, int n, float *kernel_ms) {
+    return Engine::session_copy(E(src), reinterpret_cast<Engine *const *>(dsts), n, kernel_ms);
+}
+long long minigpt4_b200_state_size(struct MiniGPT4Context *ctx) { return ctx ? E(ctx)->state_size() : -1; }
+int minigpt4_b200_state_save(struct MiniGPT4Context *ctx, void *buf, long long cap, long long *written) {
+    return ctx ? E(ctx)->state_save(buf, cap, written) : ErrFailedToAddString;
+}
+int minigpt4_b200_state_load(struct MiniGPT4Context *ctx, const void *buf, long long size) {
+    return ctx ? E(ctx)->state_load(buf, size) : ErrFailedToAddString;
+}
 int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p, float tfs_z,
                                  float typical_p, int32_t /*repeat_last_n*/, float /*repeat_penalty*/, float /*alpha_presence*/,
                                  float /*alpha_frequency*/, int mirostat, float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {

@@ -1,6 +1,7 @@
 // engine.cpp — see engine.h.
 #include "engine.h"
 #include "../../include/minigpt4.h"
+#include <stddef.h>
 #include <string.h>
 #include <algorithm>
 #include <exception>
@@ -240,6 +241,92 @@ Error Engine::score_tokens(Engine *const *e, int n, const int32_t *ids, const in
         for (int i = 0; i < n; ++i) { e[i]->n_past_ += n_ids[i]; e[i]->reply_clear(); }
     return ErrNone;
 }
+Error Engine::session_copy(Engine *src, Engine *const *dsts, int n, float *kernel_ms) {
+    if (!src || !dsts) { MG4_ERR("session_copy: NULL source or destinations"); return ErrFailedToAddString; }
+    if (n < 1 || n > LlamaDevice::kMaxBatch) { MG4_ERR("session_copy: %d destinations (1 .. %d)", n, LlamaDevice::kMaxBatch); return ErrFailedToAddString; }
+    if (src->tp.world > 1) { MG4_ERR("session_copy: the source is tensor-parallel"); return ErrFailedToAddString; }
+    for (int i = 0; i < n; ++i) {
+        if (!dsts[i]) { MG4_ERR("session_copy: destination %d is NULL", i); return ErrFailedToAddString; }
+        if (dsts[i] == src) { MG4_ERR("session_copy: destination %d is the source", i); return ErrFailedToAddString; }
+        for (int j = 0; j < i; ++j) if (dsts[j] == dsts[i]) { MG4_ERR("session_copy: destination %d appears twice", i); return ErrFailedToAddString; }
+        if (dsts[i]->llm_->group() != src->llm_->group()) { MG4_ERR("session_copy: destination %d serves another model", i); return ErrFailedToAddString; }
+        if (dsts[i]->tp.world > 1) { MG4_ERR("session_copy: destination %d is tensor-parallel", i); return ErrFailedToAddString; }
+    }
+    if (!src->flush()) return ErrFailedToAddString;
+    LlamaDevice *L[LlamaDevice::kMaxBatch];
+    for (int i = 0; i < n; ++i) L[i] = dsts[i]->llm_.get();
+    const float ms = LlamaDevice::copy_state(*src->llm_, L, n, src->n_past_);
+    for (int i = 0; i < n; ++i) {
+        Engine &d = *dsts[i];
+        d.n_past_ = src->n_past_; d.pend_ids_.clear(); d.pend_emb_.clear(); d.reply_ = src->reply_;
+    }
+    if (kernel_ms) *kernel_ms = ms;
+    return ErrNone;
+}
+
+// The saved conversation (minigpt4_b200_state_save): this header, n_vocab F32 logits, then K[n_layer][n_past][n_embd] and V[...] as F16.
+// Little-endian, as the engine's x86-64 / aarch64 hosts store it; every field sits at its natural alignment, so the struct is the layout.
+namespace {
+constexpr char kStateMagic[8] = {'M', 'G', '4', 'S', 'T', 'A', 'T', 'E'};
+constexpr uint32_t kStateVersion = 1;
+struct StateHeader {
+    char magic[8];
+    uint32_t version;
+    int32_t n_vocab, n_embd, n_head, n_layer, n_ff;
+    uint64_t fingerprint;
+    int32_t n_past;
+    int32_t reply_len;
+    char reply[LlamaDevice::kStopMax];
+    DeviceState state;
+};
+static_assert(sizeof(DeviceState) == 64 && sizeof(StateHeader) == 144 && offsetof(StateHeader, state) == 80, "the documented blob layout");
+long long state_bytes(const LlamaDims &d, long long n_past) { return (long long)sizeof(StateHeader) + 4LL * d.n_vocab + 4LL * d.n_layer * n_past * d.n_embd; }
+}  // namespace
+
+long long Engine::state_size() const { return tp.world > 1 ? -1 : state_bytes(llm_->dims(), n_past_); }
+
+Error Engine::state_save(void *buf, long long cap, long long *written) {
+    if (!buf || tp.world > 1) { MG4_ERR("state_save: NULL buffer or a tensor-parallel context"); return ErrFailedToAddString; }
+    const long long need = state_size();
+    if (cap < need) { MG4_ERR("state_save: %lld bytes of room for a %lld-byte state", cap, need); return ErrFailedToAddString; }
+    if (!flush()) return ErrFailedToAddString;
+    const LlamaDims &d = llm_->dims();
+    StateHeader h;
+    memset(&h, 0, sizeof h);
+    memcpy(h.magic, kStateMagic, 8); h.version = kStateVersion;
+    h.n_vocab = d.n_vocab; h.n_embd = d.n_embd; h.n_head = d.n_head; h.n_layer = d.n_layer; h.n_ff = d.n_ff;
+    h.fingerprint = llm_->fingerprint(); h.n_past = n_past_;
+    h.reply_len = (int32_t)reply_.size(); memcpy(h.reply, reply_.data(), reply_.size());
+    unsigned char *out = (unsigned char *)buf;
+    float *logits = (float *)(out + sizeof h);
+    llm_->state_to_host(n_past_, &h.state, logits, out + sizeof h + 4 * (size_t)d.n_vocab);
+    h.state.n_past = n_past_;   // (minigpt4_reset_chat rewinds the conversation, not the device state, which the next evaluation sets)
+    memcpy(out, &h, sizeof h);
+    if (written) *written = need;
+    return ErrNone;
+}
+
+Error Engine::state_load(const void *buf, long long size) {
+    if (!buf || tp.world > 1) { MG4_ERR("state_load: NULL buffer or a tensor-parallel context"); return ErrFailedToAddString; }
+    if (size < (long long)sizeof(StateHeader)) { MG4_ERR("state_load: %lld bytes, shorter than the header", size); return ErrFailedToAddString; }
+    StateHeader h;
+    memcpy(&h, buf, sizeof h);
+    const LlamaDims &d = llm_->dims();
+    if (memcmp(h.magic, kStateMagic, 8) != 0 || h.version != kStateVersion) { MG4_ERR("state_load: not a version %u state", kStateVersion); return ErrFailedToAddString; }
+    if (h.n_vocab != d.n_vocab || h.n_embd != d.n_embd || h.n_head != d.n_head || h.n_layer != d.n_layer || h.n_ff != d.n_ff) {
+        MG4_ERR("state_load: the state was saved by a model of other dimensions"); return ErrFailedToAddString;
+    }
+    if (h.fingerprint != llm_->fingerprint()) { MG4_ERR("state_load: the state was saved by another model"); return ErrFailedToAddString; }
+    if (h.n_past < 0 || h.n_past > d.n_ctx) { MG4_ERR("state_load: n_past %d outside 0 .. n_ctx %d", h.n_past, d.n_ctx); return ErrFailedToAddString; }
+    if (size != state_bytes(d, h.n_past)) { MG4_ERR("state_load: %lld bytes, the header implies %lld", size, state_bytes(d, h.n_past)); return ErrFailedToAddString; }
+    if (h.state.n_past != h.n_past) { MG4_ERR("state_load: device state at %d, header at %d", h.state.n_past, h.n_past); return ErrFailedToAddString; }
+    if (h.reply_len < 0 || h.reply_len > LlamaDevice::kStopMax) { MG4_ERR("state_load: reply tail of %d bytes", h.reply_len); return ErrFailedToAddString; }
+    const unsigned char *in = (const unsigned char *)buf;
+    llm_->state_from_host(h.n_past, h.state, (const float *)(in + sizeof h), in + sizeof h + 4 * (size_t)d.n_vocab);
+    n_past_ = h.n_past; pend_ids_.clear(); pend_emb_.clear(); reply_.assign(h.reply, (size_t)h.reply_len);
+    return ErrNone;
+}
+
 // the queues of a validated batch: one context with queued rows is its own flush(), several share the passes of eval_rows_batch
 bool Engine::flush_group(Engine *const *e, int n) {
     Engine *q[LlamaDevice::kMaxBatch]; int m = 0;

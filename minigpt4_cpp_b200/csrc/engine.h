@@ -43,6 +43,14 @@ public:
     // contexts of one group, in shared passes over the weights (see minigpt4_b200_score_tokens); keep: the ids stay evaluated, as
     // b200_eval_tokens + flush leaves them; otherwise every context is left as it was.  All or nothing
     static Error score_tokens(Engine *const *e, int n, const int32_t *ids, const int32_t *n_ids, int keep, float *logprob, int32_t *rank, float *logits);
+    // src's conversation into n (1..64, LlamaDevice::kMaxBatch) distinct other contexts of its group (see minigpt4_b200_session_copy):
+    // src's queue is evaluated first; each destination gets n_past, K / V rows, logits, greedy id, device state and reply tail, loses its
+    // queue and keeps its sampler.  kernel_ms (may be null): the copy kernel's CUDA-event time.  All or nothing
+    static Error session_copy(Engine *src, Engine *const *dsts, int n, float *kernel_ms);
+    // save / restore the conversation through host memory (see minigpt4_b200_state_save); state_size: -1 for a tensor-parallel context
+    long long state_size() const;
+    Error state_save(void *buf, long long cap, long long *written);
+    Error state_load(const void *buf, long long size);
     Error encode_image(const ::MiniGPT4Image *image, ::MiniGPT4Embedding *out);
     static constexpr int kEncodeLanes = 8;
     Error encode_images(const ::MiniGPT4Image *images, size_t n, ::MiniGPT4Embedding *out, float *total_ms);   // batched: concurrent lanes

@@ -5,6 +5,7 @@
 #include "llama_sessions.cuh"
 #include "llama_sample.cuh"
 #include "llama_score.cuh"
+#include "llama_state.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -35,6 +36,7 @@ constexpr int kWideGemmMin = 16;
 struct LlamaGroup {
     size_t weight_bytes = 0;       // the parent's load minus its own context: weights, operand cache, tables, prefill scratch
     size_t batch_bytes = 0;
+    unsigned long long fingerprint = 0;   // LlamaDevice::fingerprint
     cudaStream_t stream = nullptr;
     float *x = nullptr, *q = nullptr, *att = nullptr, *act = nullptr;   // [kPrefillMax] rows (act also holds the qkv GEMM's [rows][3 n_embd] output)
     float *last = nullptr;         // [8] the last rows of the contexts that end in a prompt pass
@@ -304,6 +306,22 @@ static void fp16_tables(unsigned short *te, unsigned short *ts) {
     for (int i = 0; i < 65536; ++i) { const float x = h2f_bits((unsigned short)i); te[i] = f2h_bits(expf(x)); ts[i] = f2h_bits(x / (1.0f + expf(-x))); }
 }
 
+// FNV-1a 64 over the tensor table in name order (name, type, dims) and the first 4096 bytes of every tensor: two files of one spec written
+// from different weights differ, and reading it touches a few pages per tensor
+static unsigned long long model_fingerprint(const LlamaFile &f) {
+    unsigned long long h = 0xcbf29ce484222325ull;
+    auto mix = [&h](const void *p, size_t n) { const unsigned char *b = (const unsigned char *)p; for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 0x100000001b3ull; } };
+    for (const auto &kv : f.tensors) {
+        const HostTensor &t = kv.second;
+        mix(t.name.data(), t.name.size());
+        const int32_t gg = t.gg;
+        mix(&gg, 4);
+        mix(t.ne, (size_t)t.n_dims * sizeof(int64_t));
+        mix(t.data, std::min<size_t>(t.nbytes, 4096));
+    }
+    return h;
+}
+
 bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     tp_ = tp;
     const int world = tp ? tp->world : 1, rank = tp ? tp->rank : 0;
@@ -320,6 +338,7 @@ bool LlamaDevice::load(const LlamaFile &f, int n_ctx, TPLink *tp) {
     sm_count_ = prop.multiProcessorCount;
     g_max_dyn_smem = std::min<size_t>(prop.sharedMemPerBlockOptin, 220 * 1024) - 1024;
     group_ = std::make_shared<LlamaGroup>();
+    group_->fingerprint = model_fingerprint(f);
     const size_t bytes0 = t_dev_bytes;
 
     Stager st;
@@ -1093,6 +1112,68 @@ void LlamaDevice::score_rows(LlamaDevice *const *c, int n, const int32_t *const 
                              float *const *logprob, int32_t *const *rank, float *const *logits) {
     const ScoreCall sc{keep, logprob, rank, logits};
     eval_rows_batch(c, n, ids, n_ids, nullptr, n_past, &sc);
+}
+
+// ------------------------------------------------------------------------------------------------
+// conversation copies (llama_state.cuh) and save / restore through host memory
+// ------------------------------------------------------------------------------------------------
+unsigned long long LlamaDevice::fingerprint() const { return group_->fingerprint; }
+
+float LlamaDevice::copy_state(LlamaDevice &src, LlamaDevice *const *dst, int n, int n_past) {
+    // a context's own step may still be running (minigpt4_end_chat returns before it finishes): every context involved has to be idle
+    src.sync();
+    for (int i = 0; i < n; ++i) dst[i]->sync();
+    const LlamaDims &d = src.d_;
+    const long long row = (long long)src.n_embd_local_ * 2 / 16;   // 16-byte chunks of one cache row
+    CopyStateArgs a{};
+    a.k = (const uint4 *)src.kcache_; a.v = (const uint4 *)src.vcache_; a.logits = src.logits_; a.state = src.state_;
+    for (int i = 0; i < n; ++i) { a.dk[i] = (uint4 *)dst[i]->kcache_; a.dv[i] = (uint4 *)dst[i]->vcache_; a.dlogits[i] = dst[i]->logits_; a.dstate[i] = dst[i]->state_; }
+    a.plane = (long long)d.n_ctx * row; a.run = (long long)n_past * row; a.n = n; a.n_layer = d.n_layer; a.n_vocab = d.n_vocab;
+    // about two waves over the 2 n_layer planes, no more blocks than a plane has chunks for (the logits row needs one block per
+    // kCopyThreads logits, which the KV rows outnumber from a few rows on)
+    static int per_sm = 0;
+    if (!per_sm) CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, copy_state_kernel, kCopyThreads, 0));
+    const long long per_plane = std::max(1LL, 2LL * per_sm * src.sm_count_ / (2 * d.n_layer));
+    const long long need = std::max((a.run + kCopyThreads - 1) / kCopyThreads, (long long)(d.n_vocab + kCopyThreads - 1) / kCopyThreads);
+    const dim3 grid((unsigned)std::max(1LL, std::min(per_plane, need)), (unsigned)(2 * d.n_layer + 1));
+    CUDA_CHECK(cudaEventRecord(src.ev0_, src.stream_));
+    copy_state_kernel<<<grid, kCopyThreads, 0, src.stream_>>>(a);
+    CUDA_CHECK(cudaGetLastError()); ++src.launches_;
+    CUDA_CHECK(cudaEventRecord(src.ev1_, src.stream_));
+    CUDA_CHECK(cudaStreamSynchronize(src.stream_));
+    for (int i = 0; i < n; ++i) *dst[i]->h_argmax_ = *src.h_argmax_;
+    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, src.ev0_, src.ev1_));
+    return ms;
+}
+
+void LlamaDevice::state_to_host(int n_past, DeviceState *st, float *logits, void *kv) {
+    sync();
+    const size_t run = (size_t)n_past * n_embd_local_ * 2, plane = (size_t)d_.n_ctx * n_embd_local_;
+    CUDA_CHECK(cudaMemcpyAsync(st, state_, sizeof(DeviceState), cudaMemcpyDeviceToHost, stream_));
+    CUDA_CHECK(cudaMemcpyAsync(logits, logits_, (size_t)d_.n_vocab * 4, cudaMemcpyDeviceToHost, stream_));
+    unsigned char *out = (unsigned char *)kv;
+    if (run)
+        for (int p = 0; p < 2 * d_.n_layer; ++p) {
+            const __half *c = (p < d_.n_layer ? kcache_ : vcache_) + (size_t)(p % d_.n_layer) * plane;
+            CUDA_CHECK(cudaMemcpyAsync(out + (size_t)p * run, c, run, cudaMemcpyDeviceToHost, stream_));
+        }
+    CUDA_CHECK(cudaStreamSynchronize(stream_));
+}
+
+void LlamaDevice::state_from_host(int n_past, const DeviceState &st, const float *logits, const void *kv) {
+    sync();
+    const size_t run = (size_t)n_past * n_embd_local_ * 2, plane = (size_t)d_.n_ctx * n_embd_local_;
+    *h_state_ = st;
+    CUDA_CHECK(cudaMemcpyAsync(state_, h_state_, sizeof(DeviceState), cudaMemcpyHostToDevice, stream_));
+    CUDA_CHECK(cudaMemcpyAsync(logits_, logits, (size_t)d_.n_vocab * 4, cudaMemcpyHostToDevice, stream_));
+    const unsigned char *in = (const unsigned char *)kv;
+    if (run)
+        for (int p = 0; p < 2 * d_.n_layer; ++p) {
+            __half *c = (p < d_.n_layer ? kcache_ : vcache_) + (size_t)(p % d_.n_layer) * plane;
+            CUDA_CHECK(cudaMemcpyAsync(c, in + (size_t)p * run, run, cudaMemcpyHostToDevice, stream_));
+        }
+    CUDA_CHECK(cudaStreamSynchronize(stream_));
+    *h_argmax_ = st.argmax_id;
 }
 
 // measurement seam: average CUDA-event duration (us) of one all-reduce of a [1, n_embd] partial on the tensor-parallel path in use

@@ -121,6 +121,18 @@ public:
     static constexpr int kStopMax = 32;   // longest stop text
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                               MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped);
+    // Copy src's conversation into n (1..kMaxBatch) distinct other contexts of its group (llama_state.cuh): K / V rows 0 .. n_past - 1,
+    // logits, DeviceState and the pinned greedy id, in one launch that reads the source once.  Rows >= n_past of a destination are left
+    // as they were; its sampler, reply state and hidden rows are not touched.  Waits for every context's stream first; synchronous.
+    // Returns the CUDA-event time of the kernel (ms).  The caller validates (distinct, one group, src not among dst, src's queue evaluated).
+    static float copy_state(LlamaDevice &src, LlamaDevice *const *dst, int n, int n_past);
+    // FNV-1a 64 over the LLaMA tensor table (name, type, shape, in name order) and the first 4096 bytes of each tensor, computed at load
+    // and shared by the group: tells a saved state which model wrote it
+    unsigned long long fingerprint() const;
+    // this context's conversation to / from host memory, synchronous: the DeviceState, n_vocab logits, then K[n_layer][n_past][n_embd] and
+    // V[...] as F16 (kv: 2 n_layer n_past n_embd halves), one cudaMemcpyAsync per plane; from_host also sets the pinned greedy id
+    void state_to_host(int n_past, DeviceState *st, float *logits, void *kv);
+    void state_from_host(int n_past, const DeviceState &st, const float *logits, const void *kv);
     // the group's device table of every id's text (off: n_vocab + 1 offsets into bytes), counted in shared_bytes
     bool has_token_table() const;
     void set_token_table(const std::vector<int> &off, const std::string &bytes);

@@ -221,6 +221,11 @@ _EXT = {
     "minigpt4_b200_decode_batch": ([_VP, _I, _VP, _VP], _I),
     "minigpt4_b200_flush_batch": ([_VP, _I], _I),
     "minigpt4_b200_score_tokens": ([_VP, _I, _VP, _VP, _I, _VP, _VP, _VP], _I),
+    "minigpt4_b200_session_copy": ([_CTX, _VP, _I], _I),
+    "minigpt4_b200_session_copy_timed": ([_CTX, _VP, _I, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_state_size": ([_CTX], C.c_longlong),
+    "minigpt4_b200_state_save": ([_CTX, _VP, C.c_longlong, C.POINTER(C.c_longlong)], _I),
+    "minigpt4_b200_state_load": ([_CTX, _VP, C.c_longlong], _I),
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
@@ -367,6 +372,27 @@ class B200:
             out.append((lp[o:o + k], rk[o:o + k]) + ((lg[o:o + k],) if logits else ()))
             o += k
         return out
+
+    def session_copy(self, src, dsts) -> float:
+        """copy src's conversation (n_past, K / V rows, logits, greedy id, device state, reply tail) into every context in `dsts` (1..64 other
+        contexts of src's group), each keeping its own sampler; src's queue is evaluated first.  Returns the copy kernel's device ms."""
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_session_copy_timed(src.ptr, C.cast(self._ctx_array(dsts), C.c_void_p), len(dsts), C.byref(ms)))
+        return ms.value
+
+    def state_save(self, ctx) -> bytes:
+        """ctx's conversation as the state blob of minigpt4_b200_state_save (its queue is evaluated first)"""
+        size = self.L.minigpt4_b200_state_size(ctx.ptr)
+        assert size >= 0, "minigpt4_b200_state_size failed"
+        buf = np.empty(size, np.uint8)
+        written = C.c_longlong(0)
+        self._chk(self.L.minigpt4_b200_state_save(ctx.ptr, _ptr(buf), size, C.byref(written)))
+        return buf[:written.value].tobytes()
+
+    def state_load(self, ctx, data: bytes) -> None:
+        """replace ctx's conversation by a saved one (its sampler is kept, its queue discarded)"""
+        a = np.frombuffer(data, np.uint8)
+        self._chk(self.L.minigpt4_b200_state_load(ctx.ptr, _ptr(a), a.size))
 
     def end_chat_batch(self, ctxs, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
                        repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 1.0, alpha_frequency: float = 1.0,
