@@ -213,11 +213,38 @@ MINIGPT4_API int minigpt4_b200_mega_trace(struct MiniGPT4Context *ctx, long long
 /* kernel-level seams (each runs the production kernel on cuda:current and returns to host) -------------- */
 /* y[n][rows] = W . x  with W given as raw ggml blocks of `ggml_type` (2 Q4_0, 3 Q4_1, 13 Q5_K, 14 Q6_K, 1 F16) */
 MINIGPT4_API int minigpt4_b200_op_matvec(int ggml_type, int rows, int cols, const void *w_blocks, const float *x, int n, float *y);
-/* out[T][M] = epi(bias + X[T][K] . W[M][K]^T), F16 operands; epi 0 = bias, 2 = bias+GELU(fp16 LUT) rounded to F16 */
-MINIGPT4_API int minigpt4_b200_op_gemm_f16(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, float *out);
-MINIGPT4_API int minigpt4_b200_op_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out);
-/* q,k,v: [n][heads*dh]; out [nq][heads*dh] rounded to F16 precision */
-MINIGPT4_API int minigpt4_b200_op_attention(const float *q, const float *k, const float *v, int nq, int nk, int heads, int dh, float score_div, float *out);
+/* Vision kernel seams.  Each runs one production kernel with the launch configuration the vision graph gives it, and returns 8
+ * (FailedToAddString) for arguments the kernel cannot take, before any device work.
+ * out = epi(X[T][K] . W[M][K]^T) through the wgmma GEMM, F16 operands, the plan (token tile, token split, split-K) built as at load time.
+ * epi 0: bias + acc; 1: (bias + acc) * qscale on features < qscale_rows, bias + acc above; 2: GELU (fp16 LUT) of bias + acc, F16 out;
+ * 3: aux[t] + (bias + acc) (aux = resid [T][M]; in_place: the pre-filled rows of `out` are the residual, as when the vision graph runs
+ * without split-K); 4: out row t + 1 = (0 + bias + acc) + aux[t + 1] (aux = pos [T + 1][M]; row 0 is left alone).
+ * tsplit: split the tokens of T > 128 over CTAs (the default; 0 as with MINIGPT4_B200_VISION_TSPLIT=0).  ksplit 1..4 (epi 3 only): when the
+ * plan splits K (tsplit, T > 128), grid.z slices of raw sums (bias on slice 0) go to the leading slices of `out`.
+ * out: [ksplit][T + 1 + (epi == 4)][M] (F16 for epi 2, F32 otherwise), pre-filled by the caller and returned whole, so the row past the last
+ * one written is a guard row.  plan_out (may be NULL): {token tile, grid.y, grid.z, k-blocks per slice}.
+ * Out of range: M % 128, K % 64, T outside 1..272, epi outside 0..4, ksplit outside 1..4 or > 1 with epi != 3, a missing aux. */
+MINIGPT4_API int minigpt4_b200_op_gemm_f16(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, const float *aux,
+                                           float qscale, int qscale_rows, int ksplit, int tsplit, int in_place, void *out, int32_t *plan_out);
+/* LayerNorm (eps 1e-5) of rows x [rows][n] with weight w and bias b (may be NULL); out32 F32 and / or out16 F16 [rows][n] (either may be
+ * NULL, not both).  n outside 1..1536 is out of range. */
+MINIGPT4_API int minigpt4_b200_op_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out32, void *out16);
+/* the LayerNorm that follows a split-K residual GEMM: x [rows][n] (in / out) becomes ((x + parts[0]) + parts[1]) + ... (slice p at element
+ * p * part_stride, part_stride >= rows * n), and out16 = F16 LayerNorm of it */
+MINIGPT4_API int minigpt4_b200_op_layernorm_fold(float *x, int rows, int n, const float *w, const float *b, const float *parts, int n_parts,
+                                                 long long part_stride, void *out16);
+/* attention over `heads` heads of dh (64 or 88): q, k, v at element offsets q_off / k_off / v_off of buf[n_buf] with row pitches ldq / ldkv
+ * (multiples of 4), scores / score_div, fp16-LUT softmax; q_per_cta queries per CTA (0: ceil(nq / 4)).  out: [nq + 1][ld_out] pre-filled by
+ * the caller and returned whole: rows < nq, columns < heads * dh get the F16-rounded context, row nq is a guard row.  Out of range: nk
+ * outside 1..288 or past what shared memory holds (dh 88: 268 keys), dh not 64 / 88, spans outside buf. */
+MINIGPT4_API int minigpt4_b200_op_attention(const float *buf, long long n_buf, long long q_off, int ldq, long long k_off, long long v_off, int ldkv,
+                                            int nq, int nk, int heads, int dh, float score_div, int q_per_cta, int ld_out, float *out);
+/* minigpt4_encode_image's forward on ctx's first lane, run eagerly (not as the graph) with every stage copied out once it is complete; each
+ * pointer may be NULL.  image F32 CHW [3][224][224]; embed [257][D]: patch embedding + CLS + positions; vit_blocks [n_blocks][257][D]: the
+ * residual stream after each block; ln_vision [257][D]: the F16 Q-Former operand as F32; qformer [q_layers][32][768]: the hidden states after
+ * each layer; out [32][n_embd_llm]: the embedding minigpt4_encode_image returns.  8 for a NULL ctx / image or a context without vision. */
+MINIGPT4_API int minigpt4_b200_encode_taps(struct MiniGPT4Context *ctx, const float *image, float *embed, float *vit_blocks, float *ln_vision,
+                                           float *qformer, float *out);
 /* the LLaMA attention of the decode step and prompt passes: q F32 [rows][n_head*128], k_f16 / v_f16 F16 caches [n_ctx][n_head*128]
  * (row t sees keys 0 .. its position; rows above are never read), out F32 [rows][n_head*128].  path 0: the single-context kernel, row t
  * at pos[0] + t; path 1: the batched kernel, row t at pos[t].  8 (FailedToAddString) on arguments out of range, before any device work */

@@ -305,12 +305,25 @@ int minigpt4_b200_mega_trace(struct MiniGPT4Context *ctx, long long *out, int ma
 int minigpt4_b200_op_matvec(int ggml_type, int rows, int cols, const void *w_blocks, const float *x, int n, float *y) {
     LlamaDevice::test_matvec(ggml_type, rows, cols, w_blocks, x, n, y); return 0;
 }
-int minigpt4_b200_op_gemm_f16(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, float *out) {
-    VisionDevice::test_gemm(M, T, K, w_f16, x_f16, bias, epi, out); return 0;
+int minigpt4_b200_op_gemm_f16(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, const float *aux, float qscale,
+                              int qscale_rows, int ksplit, int tsplit, int in_place, void *out, int32_t *plan_out) {
+    return VisionDevice::test_gemm(M, T, K, w_f16, x_f16, bias, epi, aux, qscale, qscale_rows, ksplit, tsplit, in_place, out, plan_out);
 }
-int minigpt4_b200_op_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out) { VisionDevice::test_layernorm(x, rows, n, w, b, out); return 0; }
-int minigpt4_b200_op_attention(const float *q, const float *k, const float *v, int nq, int nk, int heads, int dh, float score_div, float *out) {
-    VisionDevice::test_attention(q, k, v, nq, nk, heads, dh, score_div, out); return 0;
+int minigpt4_b200_op_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out32, void *out16) {
+    return VisionDevice::test_layernorm(x, rows, n, w, b, out32, out16);
+}
+int minigpt4_b200_op_layernorm_fold(float *x, int rows, int n, const float *w, const float *b, const float *parts, int n_parts, long long part_stride,
+                                    void *out16) {
+    return VisionDevice::test_layernorm_fold(x, rows, n, w, b, parts, n_parts, part_stride, out16);
+}
+int minigpt4_b200_op_attention(const float *buf, long long n_buf, long long q_off, int ldq, long long k_off, long long v_off, int ldkv, int nq, int nk,
+                               int heads, int dh, float score_div, int q_per_cta, int ld_out, float *out) {
+    return VisionDevice::test_attention(buf, n_buf, q_off, ldq, k_off, v_off, ldkv, nq, nk, heads, dh, score_div, q_per_cta, ld_out, out);
+}
+int minigpt4_b200_encode_taps(struct MiniGPT4Context *ctx, const float *image, float *embed, float *vit_blocks, float *ln_vision, float *qformer, float *out) {
+    if (!ctx || !image || !E(ctx)->has_vision()) return ErrFailedToAddString;
+    E(ctx)->vision()->encode_taps(image, embed, vit_blocks, ln_vision, qformer, out);
+    return 0;
 }
 
 int minigpt4_b200_op_llama_attention(const float *q, const void *k_f16, const void *v_f16, int n_head, int n_ctx, int rows, const int32_t *pos, int path,

@@ -31,22 +31,31 @@ public:
     void encode_begin(const float *image_host);   // asynchronous half of encode() (several lanes run concurrently) ...
     float encode_end(float *out_host);            // ... and its synchronising half
     const float *last_embedding_device() const { return proj_out_; }
-    // test taps (after encode): 1 = embeddings+pos [T][D] is not kept; 3 = ln_vision out (F16 -> F32) ; 5 = final
-    void tap_ln_vision(float *dst);       // [T][D]
-    void tap_residual(float *dst);        // ViT residual stream after the last block [T][D]
+    // The forward of encode(), run eagerly on this lane's stream (not the graph) with every stage copied to the host as it becomes complete.
+    // Each pointer may be null.  embed [T][D]: patch embedding + CLS + pos; vit_blocks [n_blocks][T][D]: the residual stream after each block;
+    // ln_vision [T][D]: the F16 Q-Former operand as F32; qformer [q_layers][32][768]: hs after each layer; out [32][n_embd_llm].
+    void encode_taps(const float *image_host, float *embed, float *vit_blocks, float *ln_vision, float *qformer, float *out);
     unsigned long long kernel_launches() const { return launches_; }
     double flops_per_image() const { return flops_; }
     size_t weight_bytes() const { return weight_bytes_; }
     cudaStream_t stream() const { return stream_; }
 
-    // kernel-level test hook: out[T][M] = bias + X[T][K] . W[M][K]^T through the wgmma GEMM (F16 operands on host)
-    static void test_gemm(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, float *out_f32);
+    // Kernel-level test seams: each runs one production kernel with the launch configuration load() / record() would give it and returns
+    // ErrFailedToAddString (8) for arguments the kernel cannot take, before any device work.
+    // out[T][M] = epi(W[M][K] . X[T][K]^T) through the wgmma GEMM; `out` is the caller's pre-filled buffer with one guard row past the last row
+    // written (see minigpt4_b200_op_gemm_f16); plan_out (may be null) = {token tile, grid.y, grid.z, k-blocks per slice}.
+    static int test_gemm(int M, int T, int K, const void *w_f16, const void *x_f16, const float *bias, int epi, const float *aux, float qscale,
+                         int qscale_rows, int ksplit, int tsplit, int in_place, void *out, int *plan_out);
     static int test_dequant(int gg_type, const void *raw, long n, void *out_f16);
-    static void test_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out);
-    static void test_attention(const float *q, const float *k, const float *v, int nq, int nk, int heads, int dh, float div, float *out);
+    static int test_layernorm(const float *x, int rows, int n, const float *w, const float *b, float *out32, void *out16);
+    static int test_layernorm_fold(float *x, int rows, int n, const float *w, const float *b, const float *parts, int n_parts, long long part_stride,
+                                   void *out16);
+    static int test_attention(const float *buf, long long n_buf, long long q_off, int ldq, long long k_off, long long v_off, int ldkv, int nq, int nk,
+                              int heads, int dh, float div, int q_per_cta, int ld_out, float *out);
 
 private:
-    void record();  // enqueue the whole forward on stream_ (captured into graph_)
+    struct Taps { float *embed, *vit_blocks, *ln_vision, *qformer, *out; };
+    void record(const Taps *taps = nullptr);  // enqueue the whole forward on stream_ (captured into graph_ without taps)
     VisionDims d_;
     std::vector<GemmPlan *> plans_;
     std::vector<void *> allocs_;

@@ -236,9 +236,11 @@ _EXT = {
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
     "minigpt4_b200_mega_trace": ([_CTX, _VP, _I], _I),
     "minigpt4_b200_op_matvec": ([_I, _I, _I, _VP, _VP, _I, _VP], _I),
-    "minigpt4_b200_op_gemm_f16": ([_I, _I, _I, _VP, _VP, _VP, _I, _VP], _I),
-    "minigpt4_b200_op_layernorm": ([_VP, _I, _I, _VP, _VP, _VP], _I),
-    "minigpt4_b200_op_attention": ([_VP, _VP, _VP, _I, _I, _I, _I, _F, _VP], _I),
+    "minigpt4_b200_op_gemm_f16": ([_I, _I, _I, _VP, _VP, _VP, _I, _VP, _F, _I, _I, _I, _I, _VP, _VP], _I),
+    "minigpt4_b200_op_layernorm": ([_VP, _I, _I, _VP, _VP, _VP, _VP], _I),
+    "minigpt4_b200_op_layernorm_fold": ([_VP, _I, _I, _VP, _VP, _VP, _I, C.c_longlong, _VP], _I),
+    "minigpt4_b200_op_attention": ([_VP, C.c_longlong, C.c_longlong, _I, C.c_longlong, C.c_longlong, _I, _I, _I, _I, _I, _F, _I, _I, _VP], _I),
+    "minigpt4_b200_encode_taps": ([_CTX, _VP, _VP, _VP, _VP, _VP, _VP], _I),
     "minigpt4_b200_op_llama_attention": ([_VP, _VP, _VP, _I, _I, _I, _VP, _I, _VP], _I),
     "minigpt4_b200_op_dequant_f16": ([_I, _VP, C.c_long, _VP], _I),
     "minigpt4_b200_host_quantize_row": ([_I, _VP, C.c_long, _VP], C.c_long),
@@ -555,20 +557,66 @@ class B200:
         self._chk(self.L.minigpt4_b200_op_matvec(gtype, rows, cols, _ptr(w), _ptr(x), x.shape[0], _ptr(y)))
         return y
 
-    def op_gemm_f16(self, w: np.ndarray, x: np.ndarray, bias: Optional[np.ndarray], epi: int = 0) -> np.ndarray:
+    def op_gemm_f16(self, w: np.ndarray, x: np.ndarray, bias: Optional[np.ndarray], epi: int = 0, aux: Optional[np.ndarray] = None,
+                    qscale: float = 1.0, qscale_rows: int = 0, ksplit: int = 1, tsplit: bool = True, in_place: bool = False,
+                    out: Optional[np.ndarray] = None, plan: bool = False):
+        """minigpt4_b200_op_gemm_f16: w float16 [M, K], x float16 [T, K].  out: the pre-filled buffer [ksplit, T + 1 + (epi == 4), M] (float16
+        for epi 2, float32 otherwise; default zeros), returned whole; plain epilogues without split-K return its first T rows (rows 1..T for
+        epi 4) as before.  plan: also return (token tile, grid.y, grid.z, k-blocks per slice)."""
         w = np.ascontiguousarray(w, np.float16); x = np.ascontiguousarray(x, np.float16)
         M, K = w.shape
         T = x.shape[0]
         b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        out = np.zeros((T, M), np.float32)
-        self._chk(self.L.minigpt4_b200_op_gemm_f16(M, T, K, _ptr(w), _ptr(x), _ptr(b), epi, _ptr(out)))
-        return out
+        a = None if aux is None else np.ascontiguousarray(aux, np.float32)
+        whole = out is not None
+        if out is None:
+            out = np.zeros((ksplit, T + 1 + (epi == 4), M), np.float16 if epi == 2 else np.float32)
+        assert out.flags.c_contiguous and out.shape == (ksplit, T + 1 + (epi == 4), M) and out.dtype == (np.float16 if epi == 2 else np.float32)
+        pl = np.zeros(4, np.int32)
+        self._chk(self.L.minigpt4_b200_op_gemm_f16(M, T, K, _ptr(w), _ptr(x), _ptr(b), epi, _ptr(a), qscale, qscale_rows, ksplit, int(tsplit),
+                                                   int(in_place), _ptr(out), _ptr(pl)))
+        res = out if whole else out[0, (1 if epi == 4 else 0):(T + 1 if epi == 4 else T)].astype(np.float32)
+        return (res, tuple(int(v) for v in pl)) if plan else res
 
-    def op_layernorm(self, x, w, b) -> np.ndarray:
-        x = np.ascontiguousarray(x, np.float32); w = np.ascontiguousarray(w, np.float32); b = np.ascontiguousarray(b, np.float32)
-        out = np.empty_like(x)
-        self._chk(self.L.minigpt4_b200_op_layernorm(_ptr(x), x.shape[0], x.shape[1], _ptr(w), _ptr(b), _ptr(out)))
-        return out
+    def op_gemm_f16_rc(self, M: int, T: int, K: int, epi: int = 0, ksplit: int = 1, aux: bool = True, in_place: bool = False) -> int:
+        """the return code of minigpt4_b200_op_gemm_f16 for a shape / configuration, with zero operands of that shape (refusals do no device work)"""
+        n = max(1, M * K), max(1, T * K)
+        w, x = np.zeros(n[0], np.float16), np.zeros(n[1], np.float16)
+        a = np.zeros(max(1, (T + 1) * M), np.float32) if aux else None
+        out = np.zeros(max(1, ksplit * (T + 2) * M), np.float32)
+        return self.L.minigpt4_b200_op_gemm_f16(M, T, K, _ptr(w), _ptr(x), None, epi, _ptr(a), 1.0, 0, ksplit, 1, int(in_place), _ptr(out), None)
+
+    def op_layernorm(self, x, w, b, f16: bool = False, f32: bool = True):
+        """float32 [rows, n] -> the F32 output, the F16 one, or (F32, F16) when both are asked for (one launch writes both)"""
+        x = np.ascontiguousarray(x, np.float32); w = np.ascontiguousarray(w, np.float32)
+        b = None if b is None else np.ascontiguousarray(b, np.float32)
+        o32 = np.empty_like(x) if f32 else None
+        o16 = np.empty(x.shape, np.float16) if f16 else None
+        self._chk(self.L.minigpt4_b200_op_layernorm(_ptr(x), x.shape[0], x.shape[1], _ptr(w), _ptr(b), _ptr(o32), _ptr(o16)))
+        return (o32, o16) if f32 and f16 else (o32 if f32 else o16)
+
+    def op_layernorm_rc(self, rows: int, n: int) -> int:
+        x = np.zeros(max(1, rows * n), np.float32); w = np.zeros(max(1, n), np.float32); o = np.zeros_like(x)
+        return self.L.minigpt4_b200_op_layernorm(_ptr(x), rows, n, _ptr(w), None, _ptr(o), None)
+
+    def op_layernorm_fold(self, x, parts, w, b) -> tuple[np.ndarray, np.ndarray]:
+        """x float32 [rows, n], parts float32 [n_parts, rows, n] -> (x + parts[0] + parts[1] + ... in slice order, F16 LayerNorm of it)"""
+        x = np.array(x, np.float32, order="C"); p = np.ascontiguousarray(parts, np.float32)
+        w = np.ascontiguousarray(w, np.float32); b = None if b is None else np.ascontiguousarray(b, np.float32)
+        o16 = np.empty(x.shape, np.float16)
+        self._chk(self.L.minigpt4_b200_op_layernorm_fold(_ptr(x), x.shape[0], x.shape[1], _ptr(w), _ptr(b), _ptr(p), p.shape[0], x.size, _ptr(o16)))
+        return x, o16
+
+    def encode_taps(self, ctx, image: np.ndarray, n_blocks: int, q_layers: int, n_embd_llm: int, d: int = 1408) -> dict:
+        """every stage of the encode of `image` on ctx (whose vision model has n_blocks ViT blocks and q_layers Q-Former layers): embed [257, d],
+        vit_blocks [n_blocks, 257, d], ln_vision [257, d], qformer [q_layers, 32, 768], out [32, n_embd_llm]"""
+        img = np.ascontiguousarray(image, np.float32)
+        r = {"embed": np.zeros((257, d), np.float32), "vit_blocks": np.zeros((n_blocks, 257, d), np.float32),
+             "ln_vision": np.zeros((257, d), np.float32), "qformer": np.zeros((q_layers, 32, 768), np.float32),
+             "out": np.zeros((32, n_embd_llm), np.float32)}
+        self._chk(self.L.minigpt4_b200_encode_taps(ctx.ptr, _ptr(img), _ptr(r["embed"]), _ptr(r["vit_blocks"]), _ptr(r["ln_vision"]),
+                                                   _ptr(r["qformer"]), _ptr(r["out"])))
+        return r
 
     def op_dequant_f16(self, gtype: int, raw: np.ndarray, n: int) -> np.ndarray:
         raw = np.ascontiguousarray(raw)
@@ -584,10 +632,29 @@ class B200:
         return out[:nb].copy()
 
     def op_attention(self, q, k, v, heads: int, dh: int, div: float) -> np.ndarray:
+        """q [nq][heads * dh], k / v [nk][heads * dh] float32 -> the attention output [nq][heads * dh] (F16 precision), ceil(nq / 4) queries per CTA"""
         q = np.ascontiguousarray(q, np.float32); k = np.ascontiguousarray(k, np.float32); v = np.ascontiguousarray(v, np.float32)
-        out = np.empty_like(q)
-        self._chk(self.L.minigpt4_b200_op_attention(_ptr(q), _ptr(k), _ptr(v), q.shape[0], k.shape[0], heads, dh, div, _ptr(out)))
+        nq, nk, ld = q.shape[0], k.shape[0], heads * dh
+        buf = np.concatenate([q.reshape(-1), k.reshape(-1), v.reshape(-1)])
+        return self.op_attention_packed(buf, 0, ld, nq * ld, (nq + nk) * ld, ld, nq, nk, heads, dh, div)[:nq]
+
+    def op_attention_packed(self, buf, q_off: int, ldq: int, k_off: int, v_off: int, ldkv: int, nq: int, nk: int, heads: int, dh: int,
+                            div: float, q_per_cta: int = 0, ld_out: Optional[int] = None, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """minigpt4_b200_op_attention over one float32 buffer with q / k / v at element offsets and row pitches (as the vision graph passes its
+        packed qkv outputs).  out: the pre-filled [nq + 1, ld_out] float32 buffer (default zeros), returned whole"""
+        buf = np.ascontiguousarray(buf, np.float32).reshape(-1)
+        ld_out = heads * dh if ld_out is None else ld_out
+        if out is None:
+            out = np.zeros((nq + 1, ld_out), np.float32)
+        assert out.flags.c_contiguous and out.shape == (nq + 1, ld_out) and out.dtype == np.float32
+        self._chk(self.L.minigpt4_b200_op_attention(_ptr(buf), buf.size, q_off, ldq, k_off, v_off, ldkv, nq, nk, heads, dh, div, q_per_cta, ld_out,
+                                                    _ptr(out)))
         return out
+
+    def op_attention_rc(self, nq: int, nk: int, heads: int, dh: int) -> int:
+        ld = heads * dh
+        buf = np.zeros((nq + 2 * nk) * ld, np.float32); out = np.zeros((nq + 1) * ld, np.float32)
+        return self.L.minigpt4_b200_op_attention(_ptr(buf), buf.size, 0, ld, nq * ld, (nq + nk) * ld, ld, nq, nk, heads, dh, 1.0, 0, ld, _ptr(out))
 
     def op_llama_attention(self, q, k, v, pos, path: int) -> np.ndarray:
         """q float32 [rows][n_head * 128], k / v float16 [n_ctx][n_head * 128]; path 0: row t at pos[0] + t (pos may be one int), path 1:

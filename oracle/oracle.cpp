@@ -764,7 +764,10 @@ static void linear(const Model *m, const std::string &prefix, const float *x, in
 // `tap`, when non-NULL, receives intermediate activations for layer-level parity tests:
 //   tap_kind 1 = embeddings after pos_embed [T][D]; 2 = after ViT block `tap_idx` [T][D];
 //   3 = ln_vision output [T][D]; 4 = Q-Former layer `tap_idx` output [32][768]
+// oracle_vit_encode_stages: one run that fills every stage at once (each pointer may be NULL): embed [T][D], vit_blocks [n_blocks][T][D],
+//   ln_vision [T][D], qformer [q_layers][32][768], and out
 // ---------------------------------------------------------------------------------------------
+struct VitStages { float *embed, *vit_blocks, *ln_vision, *qformer; };
 struct VitDims { int D, T, H, dh, nblocks, P, patch; };
 
 // NNQKVAttention::forward (minigpt4.cpp:1246-1315)
@@ -818,9 +821,7 @@ static void bert_attention(const Model *m, const std::string &pfx, const float *
     op_layernorm(dense.data(), out, HID, nq, F(m, pfx + "output.LayerNorm.weight"), F(m, pfx + "output.LayerNorm.bias"));
 }
 
-ORACLE_API int oracle_vit_encode(void *model, const float *image, float *out, int n_threads, int tap_kind, int tap_idx, float *tap) {
-    const Model *m = (const Model *)model;
-    if (n_threads > 0) omp_set_num_threads(n_threads);
+static int vit_encode(const Model *m, const float *image, float *out, int tap_kind, int tap_idx, float *tap, const VitStages &st) {
     const Tensor &pos = T(m, "visual_encoder.pos_embed");
     VitDims v; v.D = (int)pos.ne[0]; v.T = (int)pos.ne[1]; v.dh = 88; v.H = v.D / 88; v.patch = 14; v.P = 16;
     const int D = v.D, Tn = v.T, IMG = 224;
@@ -844,6 +845,7 @@ ORACLE_API int oracle_vit_encode(void *model, const float *image, float *out, in
         for (size_t i = 0; i < (size_t)Tn * D; ++i) x[i] += pe[i];
     }
     if (tap_kind == 1) { memcpy(tap, x.data(), sizeof(float) * Tn * D); return 0; }
+    if (st.embed) memcpy(st.embed, x.data(), sizeof(float) * Tn * D);
 
     std::vector<float> h1((size_t)Tn * 6144 * (D / 1408 + 1));
     for (int b = 0; b < v.nblocks; ++b) {
@@ -859,10 +861,12 @@ ORACLE_API int oracle_vit_encode(void *model, const float *image, float *out, in
         linear(m, p + "mlp.fc2", h1.data(), Tn, tmp.data());
         for (size_t i = 0; i < x.size(); ++i) x[i] += tmp[i];
         if (tap_kind == 2 && tap_idx == b) { memcpy(tap, x.data(), sizeof(float) * Tn * D); return 0; }
+        if (st.vit_blocks) memcpy(st.vit_blocks + (size_t)b * Tn * D, x.data(), sizeof(float) * Tn * D);
     }
     op_layernorm(x.data(), y.data(), D, Tn, F(m, "ln_vision.weight"), F(m, "ln_vision.bias"));
     const float *image_embeds = y.data();
     if (tap_kind == 3) { memcpy(tap, y.data(), sizeof(float) * Tn * D); return 0; }
+    if (st.ln_vision) memcpy(st.ln_vision, y.data(), sizeof(float) * Tn * D);
 
     // Q-Former (minigpt4.cpp:2203-2340, NNBertEncoderLayer :1324-1463)
     const int NQ = 32, HID = 768;
@@ -885,9 +889,19 @@ ORACLE_API int oracle_vit_encode(void *model, const float *image, float *out, in
         for (size_t i = 0; i < o.size(); ++i) o[i] += ffn_in[i];
         op_layernorm(o.data(), hs.data(), HID, NQ, F(m, p + "output_query.LayerNorm.weight"), F(m, p + "output_query.LayerNorm.bias"));
         if (tap_kind == 4 && tap_idx == l) { memcpy(tap, hs.data(), sizeof(float) * NQ * HID); return 0; }
+        if (st.qformer) memcpy(st.qformer + (size_t)l * NQ * HID, hs.data(), sizeof(float) * NQ * HID);
     }
     linear(m, "llama_proj", hs.data(), NQ, out);
     return 0;
+}
+ORACLE_API int oracle_vit_encode(void *model, const float *image, float *out, int n_threads, int tap_kind, int tap_idx, float *tap) {
+    if (n_threads > 0) omp_set_num_threads(n_threads);
+    return vit_encode((const Model *)model, image, out, tap_kind, tap_idx, tap, VitStages{nullptr, nullptr, nullptr, nullptr});
+}
+ORACLE_API int oracle_vit_encode_stages(void *model, const float *image, float *out, int n_threads, float *embed, float *vit_blocks, float *ln_vision,
+                                        float *qformer) {
+    if (n_threads > 0) omp_set_num_threads(n_threads);
+    return vit_encode((const Model *)model, image, out, 0, 0, nullptr, VitStages{embed, vit_blocks, ln_vision, qformer});
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -64,6 +64,7 @@ def lib() -> ctypes.CDLL:
         L.oracle_model_free.argtypes = [vp]
         L.oracle_model_add.argtypes = [vp, ctypes.c_char_p, i32, i32, ctypes.POINTER(i64), vp]
         L.oracle_vit_encode.argtypes = [vp, fp, fp, i32, i32, i32, fp]
+        L.oracle_vit_encode_stages.argtypes = [vp, fp, fp, i32, fp, fp, fp, fp]
         L.oracle_llama_new.argtypes = [vp, i32]
         L.oracle_llama_new.restype = vp
         L.oracle_llama_free.argtypes = [vp]
@@ -289,6 +290,8 @@ class OracleEngine:
         self.llm = None
         if minigpt4_path is not None:
             self.config, vt = read_minigpt4(minigpt4_path)
+            self._vis_names = set(vt)
+            self.vis_d = vt["visual_encoder.pos_embed"].ne[0]
             self.vis = OracleModel(vt)
             self.n_embd_llm = vt["llama_proj.weight"].ne[1]
         if llama_path is not None:
@@ -309,6 +312,25 @@ class OracleEngine:
             tap = np.zeros((257, 1408), np.float32) if tap_kind in (1, 2, 3) else np.zeros((32, 768), np.float32)
         lib().oracle_vit_encode(self.vis.h, _p(image), _p(out), self.n_threads, tap_kind, tap_idx, _p(tap) if tap is not None else None)
         return tap if tap_kind else out
+
+    def encode_image_stages(self, image: np.ndarray) -> dict:
+        """every stage of one encode_image run: embed [257, D] (patches + CLS + positions), vit_blocks [n_blocks, 257, D] (residual stream
+        after each block), ln_vision [257, D], qformer [q_layers, 32, 768] (hidden states after each layer) and out [32, n_embd_llm]"""
+        image = np.ascontiguousarray(image, np.float32).reshape(3, 224, 224)
+        D = self.vis_d
+        nb = self._count("visual_encoder.blocks.{}.norm1.weight")
+        nl = self._count("Qformer.bert.encoder.layer.{}.attention.self.query.weight")
+        r = {"embed": np.zeros((257, D), np.float32), "vit_blocks": np.zeros((nb, 257, D), np.float32), "ln_vision": np.zeros((257, D), np.float32),
+             "qformer": np.zeros((nl, 32, 768), np.float32), "out": np.zeros((32, self.n_embd_llm), np.float32)}
+        lib().oracle_vit_encode_stages(self.vis.h, _p(image), _p(r["out"]), self.n_threads, _p(r["embed"]), _p(r["vit_blocks"]), _p(r["ln_vision"]),
+                                       _p(r["qformer"]))
+        return r
+
+    def _count(self, pattern: str) -> int:
+        n = 0
+        while pattern.format(n) in self._vis_names:
+            n += 1
+        return n
 
     # -- language -------------------------------------------------------------------------
     def eval_tokens(self, ids, tap_layer: int = -1):

@@ -64,3 +64,19 @@ def test_independent_crosscheck_is_within_bounds():
     assert r["llama_f16_long_logits_rel_err"] < 2e-3 and r["llama_f16_long_argmax_equal"]   # 2048 tokens: positions to 2047
     assert r["llama_q4_1_logits_rel_err"] < 2e-2 and r["llama_q4_1_argmax_equal"]  # Q8 activation quantisation is deliberate
     assert r["vision_missing_keys"] == [] and r["qformer_missing_keys"] == []
+
+
+def test_vision_all_stages_run_equals_single_taps(orc, mg, models):
+    """encode_image_stages fills every stage in one run: each equals the single-tap run of that stage (tap kinds 1-4) and its
+    output equals the plain encode_image, bit for bit."""
+    e = orc.OracleEngine(str(models / "vision.bin"), None)
+    img = mg.synth_image(7)
+    st = e.encode_image_stages(img)
+    assert np.array_equal(st["out"], e.encode_image(img))
+    assert np.array_equal(st["embed"], e.encode_image(img, tap_kind=1))
+    assert st["vit_blocks"].shape[0] >= 1 and st["qformer"].shape[0] >= 2
+    for b in range(st["vit_blocks"].shape[0]):
+        assert np.array_equal(st["vit_blocks"][b], e.encode_image(img, tap_kind=2, tap_idx=b))
+    assert np.array_equal(st["ln_vision"], e.encode_image(img, tap_kind=3))
+    for layer in range(st["qformer"].shape[0]):
+        assert np.array_equal(st["qformer"][layer], e.encode_image(img, tap_kind=4, tap_idx=layer))
