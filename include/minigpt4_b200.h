@@ -187,6 +187,41 @@ MINIGPT4_API int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ct
                                                      int mirostat, float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out,
                                                      int32_t *stopped, float *ms_out);
 
+/* Constrained replies (DESIGN.md §4.12): sample only the ids a deterministic automaton over bytes allows.  The automaton has n_states
+ * states (1..65536), start state 0; next[s * 256 + b] is the state byte b leads to from s, or -1 to reject; accept[s] != 0 marks an
+ * accepting state.  The text of an id is the C string minigpt4_end_chat returns for it (an id whose text is empty is never allowed).
+ *   allowed(s) = every id other than 2 whose text, walked byte by byte from s, never meets -1 and ends in a live state, plus id 2 (</s>)
+ *   if s accepts.  A state is live if some sequence of allowed ids leads from it to an accepting state (computed on the ids, to a fixed
+ *   point).  An id moves the state to where its walk ends; id 2 moves it to the finished state, which allows only id 2.
+ * On a constrained context, minigpt4_end_chat / end_chat_image, minigpt4_b200_end_chat_batch, sample_steps and sample_until run the
+ * unchanged sampler chain over allowed(s) only, in id order: top_k is clamped to |allowed(s)| and temp <= 0 takes the arg-max over
+ * allowed(s), the lower id on ties.  Each fed id moves the state; sample_until also stops a constrained context after the step that
+ * feeds id 2 (stopped = 1).  decode_chain, decode_batch, the two _mirostat calls and end_chat / end_chat_batch with mirostat 1 or 2
+ * return 8 on a constrained context and change nothing; get_logits and greedy_id stay unconstrained.
+ * The state restarts where the reply tail does (system_prompt, begin_chat, begin_chat_image, reset_chat, eval_tokens, eval_embd,
+ * score_tokens with keep 1) and at state_load (the saved state carries no constraint); session_copy gives a destination with the source's
+ * constraint attached the source's state and restarts any other destination's. */
+struct MiniGPT4B200Constraint;
+/* compile against ctx's vocabulary; the device tables belong to ctx's group (counted in session_info's shared bytes).  NULL for
+ * n_states outside 1..65536, next[] outside -1..n_states-1, a start state that is not live, a tensor-parallel ctx, more than 2^31-1
+ * transitions, or device memory exhausted. */
+MINIGPT4_API struct MiniGPT4B200Constraint *minigpt4_b200_constraint_create(struct MiniGPT4Context *ctx, int n_states, const int32_t *next,
+                                                                            const uint8_t *accept);
+/* drops the handle; the tables live until no context has them attached */
+MINIGPT4_API void minigpt4_b200_constraint_free(struct MiniGPT4B200Constraint *c);
+/* attach c to ctx with its state at the start (c NULL: detach); 8 for a constraint compiled for another group */
+MINIGPT4_API int minigpt4_b200_constraint_attach(struct MiniGPT4Context *ctx, struct MiniGPT4B200Constraint *c);
+/* ctx's state (-1 once finished) and whether it is finished; 8 if no constraint is attached */
+MINIGPT4_API int minigpt4_b200_constraint_state(struct MiniGPT4Context *ctx, int *state, int *finished);
+/* allowed(state) as compiled: ids ascending (ids may be NULL) and the state each leads to (next_states may be NULL; -1: finished).
+ * Returns the count, -count if cap is short, -1 for a state that is not live or outside 0..n_states-1 (a one-id row asked with cap 0
+ * also returns -1: ask with cap >= 1). */
+MINIGPT4_API int minigpt4_b200_constraint_allowed(struct MiniGPT4B200Constraint *c, int state, int32_t *ids, int32_t *next_states, int cap);
+/* host-only seam (no GPU): the same, compiled against the vocabulary of a ggjt file; -1000000 for an unreadable file or a refused
+ * automaton */
+MINIGPT4_API int minigpt4_b200_host_constraint_allowed(const char *llm_model, int n_states, const int32_t *next, const uint8_t *accept, int state,
+                                                       int32_t *ids, int32_t *next_states, int cap);
+
 /* batch encode (config 5): n images -> n embeddings, same semantics per image as minigpt4_encode_image */
 MINIGPT4_API int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, IN struct MiniGPT4Images *images, OUT struct MiniGPT4Embeddings *embeddings);
 

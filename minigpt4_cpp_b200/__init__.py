@@ -3,4 +3,4 @@ minigpt4_encode_image and the LLaMA step behind llama_eval).  The compute lives 
 hand-written sm_90a CUDA); this package holds the host-side mirror of the reference's ctypes interface, the builder
 and the synthetic-weight generators."""
 from .minigpt4_library import (B200, DataType, ImageFormat, MiniGPT4ChatBot, MiniGPT4Context, MiniGPT4Embedding, MiniGPT4Image,  # noqa: F401
-                               MiniGPT4SharedLibrary, Verbosity, load_library, library_path)
+                               MiniGPT4SharedLibrary, Verbosity, choices_dfa, load_library, library_path)

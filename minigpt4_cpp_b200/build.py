@@ -12,7 +12,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 CSRC = Path(__file__).resolve().parent / "csrc"
 OUT = ROOT / "build" / "libminigpt4.so"
-SOURCES = ["llama.cu", "vision.cu", "api.cpp", "engine.cpp", "formats.cpp", "text.cpp", "tp.cpp", "quantize.cpp", "image.cpp", "jpeg.cpp"]
+SOURCES = ["llama.cu", "vision.cu", "api.cpp", "engine.cpp", "formats.cpp", "text.cpp", "constraint.cpp", "tp.cpp", "quantize.cpp", "image.cpp", "jpeg.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false / -ffp-contract=off: no implicit FMA contraction — float expressions evaluate exactly as written so the
 # language path is bit-identical to the CPU oracle's canonical reduction order (see oracle/oracle.cpp header)

@@ -20,7 +20,24 @@ bool path_exists(const char *p) { struct stat st; return p && stat(p, &st) == 0;
 const char *kSystemPrompt = "Give the following image: <Img>ImageContent</Img>. You will be able to see the image once I provide it to you. Please answer my questions.###";
 const char *kEosTokenSuffix = "##";
 const char *kEosSuffix = "###";
+
+// allowed(state) as the ABI reports it: the finished state's index as -1
+int allowed_of(const Constraint &c, int state, int32_t *ids, int32_t *next_states, int cap) {
+    if (state < 0 || state >= c.n_states) return -1;
+    const int m = c.row_size(state);
+    if (m == 0) return -1;   // a state that is not live
+    if (cap < m) return -m;
+    const int32_t *r = c.row(state);
+    for (int j = 0; j < m; ++j) {
+        if (ids) ids[j] = r[2 * j];
+        if (next_states) next_states[j] = r[2 * j + 1] == c.finished() ? -1 : r[2 * j + 1];
+    }
+    return m;
+}
 }  // namespace
+
+// a constraint handle: one reference to the compiled tables (constraint.h); each attached context holds another
+struct MiniGPT4B200Constraint { std::shared_ptr<Constraint> c; };
 
 extern "C" {
 
@@ -105,11 +122,12 @@ int minigpt4_end_chat_image(struct MiniGPT4Context *ctx, const char **token, siz
                             int32_t /*repeat_last_n*/, float /*repeat_penalty*/, float /*alpha_presence*/, float /*alpha_frequency*/, int mirostat,
                             float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {
     Engine *e = E(ctx);
+    if (e->constraint() && (mirostat == 1 || mirostat == 2)) { MG4_ERR("end_chat: mirostat on a constrained context"); return ErrFailedToAddString; }
     SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     const int32_t id = e->sample_token(sp);
     *token = e->id_to_token(id);
     e->add_tokens({id});  // the reference ignores this return value too (minigpt4.cpp:2715)
-    e->reply_take(*token);
+    e->reply_take_id(id);
     return ErrNone;
 }
 
@@ -199,6 +217,7 @@ int minigpt4_b200_get_hidden(struct MiniGPT4Context *ctx, float *out, int n_rows
 const char *minigpt4_b200_token_text(struct MiniGPT4Context *ctx, int32_t id) { return E(ctx)->id_to_token(id); }
 int minigpt4_b200_decode_chain(struct MiniGPT4Context *ctx, int steps, int32_t *ids_out, float *ms_out) {
     Engine *e = E(ctx);
+    if (e->constraint()) { MG4_ERR("decode_chain: a constrained context"); return ErrFailedToAddString; }
     if (!e->flush()) return ErrFailedToAddString;
     const float ms = e->llm().decode_chain(steps, e->n_past(), ids_out);
     if (ms < 0) return ErrFailedToAddString;
@@ -221,6 +240,8 @@ int minigpt4_b200_session_info(struct MiniGPT4Context *ctx, int *n_contexts, dou
     return 0;
 }
 int minigpt4_b200_decode_batch(struct MiniGPT4Context **ctxs, int n, const int32_t *ids, int32_t *ids_out) {
+    for (int i = 0; ctxs && i < n && i < LlamaDevice::kMaxBatch; ++i)
+        if (ctxs[i] && E(ctxs[i])->constraint()) { MG4_ERR("decode_batch: context %d is constrained", i); return ErrFailedToAddString; }
     return Engine::decode_batch(reinterpret_cast<Engine *const *>(ctxs), n, ids, ids_out);
 }
 int minigpt4_b200_flush_batch(struct MiniGPT4Context **ctxs, int n) { return Engine::flush_batch(reinterpret_cast<Engine *const *>(ctxs), n); }
@@ -269,6 +290,38 @@ int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, in
     if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop,
                                 SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, ids_out, n_out, stopped, ms_out);
+}
+struct MiniGPT4B200Constraint *minigpt4_b200_constraint_create(struct MiniGPT4Context *ctx, int n_states, const int32_t *next, const uint8_t *accept) {
+    if (!ctx) return nullptr;
+    std::shared_ptr<Constraint> c = E(ctx)->make_constraint(n_states, next, accept);
+    return c ? new MiniGPT4B200Constraint{c} : nullptr;
+}
+void minigpt4_b200_constraint_free(struct MiniGPT4B200Constraint *c) { delete c; }
+int minigpt4_b200_constraint_attach(struct MiniGPT4Context *ctx, struct MiniGPT4B200Constraint *c) {
+    if (!ctx) return ErrFailedToAddString;
+    return E(ctx)->constraint_attach(c ? c->c : nullptr) ? 0 : ErrFailedToAddString;
+}
+int minigpt4_b200_constraint_state(struct MiniGPT4Context *ctx, int *state, int *finished) {
+    if (!ctx || !E(ctx)->constraint()) return ErrFailedToAddString;
+    const Engine &e = *E(ctx);
+    const bool fin = e.constraint_state() == e.constraint()->finished();
+    if (state) *state = fin ? -1 : e.constraint_state();
+    if (finished) *finished = fin ? 1 : 0;
+    return 0;
+}
+int minigpt4_b200_constraint_allowed(struct MiniGPT4B200Constraint *c, int state, int32_t *ids, int32_t *next_states, int cap) {
+    return c ? allowed_of(*c->c, state, ids, next_states, cap) : -1;
+}
+int minigpt4_b200_host_constraint_allowed(const char *llm_model, int n_states, const int32_t *next, const uint8_t *accept, int state, int32_t *ids,
+                                          int32_t *next_states, int cap) {
+    LlamaFile f;
+    if (!f.load(llm_model)) return -1000000;
+    std::vector<std::string> texts(f.vocab.size());
+    for (size_t id = 0; id < texts.size(); ++id) texts[id] = id == 2 ? "</s>" : f.vocab[id].text.c_str();   // (Engine::id_to_token)
+    Constraint c;
+    std::string why;
+    if (!compile_constraint(texts, n_states, next, accept, c, &why)) return -1000000;
+    return allowed_of(c, state, ids, next_states, cap);
 }
 int minigpt4_b200_encode_images(struct MiniGPT4Context *ctx, struct MiniGPT4Images *images, struct MiniGPT4Embeddings *embeddings) {
     if (embeddings->n_embeddings < images->n_images) return ErrImageSize;

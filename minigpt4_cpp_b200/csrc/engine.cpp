@@ -10,6 +10,9 @@ namespace mg4 {
 
 TPConfig g_tp_config;
 
+// where a constraint's pairs start in its device table (in ints): after the n_states + 2 offsets, at an 8-byte boundary
+static size_t constraint_pairs_at(const Constraint &c) { return (c.off.size() + 1) / 2 * 2; }
+
 Engine::~Engine() {
     llm_.reset();
     vis_lanes_.reset();   // (lanes borrow the first lane's weights)
@@ -120,11 +123,12 @@ Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t 
 }
 Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p) {
     if (!tokens || !batch_valid(e, n, nullptr)) return ErrFailedToAddString;   // (before any sampler draws)
+    if ((p.mirostat == 1 || p.mirostat == 2) && any_constrained(e, n)) { MG4_ERR("end_chat_batch: mirostat on a constrained context"); return ErrFailedToAddString; }
     if (!flush_group(e, n)) return ErrFailedToAddString;   // so that each sample_token finds its queue empty
     int32_t ids[LlamaDevice::kMaxBatch], out[LlamaDevice::kMaxBatch];
     for (int i = 0; i < n; ++i) { ids[i] = e[i]->sample_token(p); tokens[i] = e[i]->id_to_token(ids[i]); }
     const Error err = decode_batch(e, n, ids, out);
-    for (int i = 0; i < n; ++i) e[i]->reply_take(tokens[i]);
+    for (int i = 0; i < n; ++i) e[i]->reply_take_id(ids[i]);
     return err;
 }
 // a sampler's generator and mirostat μ, to and from the device sampler's form
@@ -141,9 +145,24 @@ static void set_sampler_state(Sampler &s, const SamplingArgs &p, const uint32_t 
     if (p.mirostat) s.set_mu(mu.mu, init);
 }
 
+bool Engine::any_constrained(Engine *const *e, int n) {
+    for (int i = 0; i < n; ++i) if (e[i]->cons_) return true;
+    return false;
+}
+void Engine::sample_constraints(Engine *const *e, int n, SampleConstraint *out) {
+    for (int i = 0; i < n; ++i) {
+        out[i] = SampleConstraint{};
+        const Constraint *c = e[i]->cons_.get();
+        if (!c) continue;
+        const int *off = (const int *)c->dev->dev;
+        out[i] = SampleConstraint{off, (const int2 *)(off + constraint_pairs_at(*c)), e[i]->cons_state_};
+    }
+}
+
 Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out) {
     if (!ids_out || !group_valid(e, n, "sample_steps")) return ErrFailedToAddString;
     if (steps < 1) { MG4_ERR("sample_steps: %d steps", steps); return ErrFailedToAddString; }
+    if (p.mirostat && any_constrained(e, n)) { MG4_ERR("sample_steps: mirostat on a constrained context"); return ErrFailedToAddString; }
     for (int i = 0; i < n; ++i) {
         if (e[i]->tp.world > 1) { MG4_ERR("sample_steps: context %d is tensor-parallel", i); return ErrFailedToAddString; }
         const int n_ctx = e[i]->llm_->dims().n_ctx;
@@ -154,11 +173,13 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
     std::vector<uint32_t> rng_words((size_t)n * 625);   // (625 words a generator: 160 KB at kMaxBatch, off the stack)
     uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); }
-    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out);
+    SampleConstraint cons[LlamaDevice::kMaxBatch];
+    sample_constraints(e, n, cons);
+    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out, cons);
     for (int i = 0; i < n; ++i) {
         set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += steps;
-        for (int t = 0; t < steps; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
+        for (int t = 0; t < steps; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
     }
     if (ms_out) *ms_out = ms;
     return ErrNone;
@@ -169,6 +190,7 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     if (max_steps < 1) { MG4_ERR("sample_until: %d steps", max_steps); return ErrFailedToAddString; }
     const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
     if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("sample_until: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
+    if (p.mirostat && any_constrained(e, n)) { MG4_ERR("sample_until: mirostat on a constrained context"); return ErrFailedToAddString; }
     for (int i = 0; i < n; ++i) {
         if (e[i]->tp.world > 1) { MG4_ERR("sample_until: context %d is tensor-parallel", i); return ErrFailedToAddString; }
         const int n_ctx = e[i]->llm_->dims().n_ctx;
@@ -180,11 +202,13 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     std::vector<uint32_t> rng_words((size_t)n * 625);
     uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
-    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped);
+    SampleConstraint cons[LlamaDevice::kMaxBatch];
+    sample_constraints(e, n, cons);
+    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons);
     for (int i = 0; i < n; ++i) {
         set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += n_out[i];
-        for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take(e[i]->id_to_token(ids_out[(size_t)t * n + i]));
+        for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
     }
     if (ms_out) *ms_out = ms;
     return ErrNone;
@@ -259,6 +283,7 @@ Error Engine::session_copy(Engine *src, Engine *const *dsts, int n, float *kerne
     for (int i = 0; i < n; ++i) {
         Engine &d = *dsts[i];
         d.n_past_ = src->n_past_; d.pend_ids_.clear(); d.pend_emb_.clear(); d.reply_ = src->reply_;
+        d.cons_state_ = d.cons_ && d.cons_ == src->cons_ ? src->cons_state_ : 0;   // the source's state means nothing to another constraint
     }
     if (kernel_ms) *kernel_ms = ms;
     return ErrNone;
@@ -324,6 +349,7 @@ Error Engine::state_load(const void *buf, long long size) {
     const unsigned char *in = (const unsigned char *)buf;
     llm_->state_from_host(h.n_past, h.state, (const float *)(in + sizeof h), in + sizeof h + 4 * (size_t)d.n_vocab);
     n_past_ = h.n_past; pend_ids_.clear(); pend_emb_.clear(); reply_.assign(h.reply, (size_t)h.reply_len);
+    cons_state_ = 0;   // (the blob carries no constraint state)
     return ErrNone;
 }
 
@@ -449,9 +475,49 @@ bool Engine::flush() {
 
 int32_t Engine::sample_token(const SamplingParams &p) {
     flush();
+    if (cons_) {   // the chain over the allowed ids (greedy too: the arg-max among them, not the device's over every id)
+        llm_->logits_to_host(logits_.data());
+        const int m = cons_->row_size(cons_state_);
+        const int32_t *row = cons_->row(cons_state_);
+        std::vector<int32_t> ids((size_t)m);
+        for (int j = 0; j < m; ++j) ids[(size_t)j] = row[2 * j];
+        return sampler_->sample_allowed(logits_.data(), ids.data(), m, p);
+    }
     if (p.temp <= 0) return llm_->argmax();  // greedy: arg-max was computed on device with the logits
     llm_->logits_to_host(logits_.data());
     return sampler_->sample(logits_.data(), (int)logits_.size(), p);
+}
+
+std::vector<std::string> Engine::token_texts() const {
+    std::vector<std::string> t((size_t)llm_->dims().n_vocab);
+    for (size_t id = 0; id < t.size(); ++id) t[id] = id_to_token((int32_t)id);
+    return t;
+}
+std::shared_ptr<Constraint> Engine::make_constraint(int n_states, const int32_t *next, const uint8_t *accept) {
+    if (tp.world > 1) { MG4_ERR("constraint_create: a tensor-parallel context"); return nullptr; }
+    std::shared_ptr<Constraint> c = std::make_shared<Constraint>();
+    std::string why;
+    try {
+        if (!compile_constraint(token_texts(), n_states, next, accept, *c, &why)) { MG4_ERR("constraint_create: %s", why.c_str()); return nullptr; }
+        // on the device: off, then the pairs from an 8-byte boundary
+        const size_t at = constraint_pairs_at(*c);
+        std::vector<int32_t> buf(at + c->pairs.size(), 0);
+        std::copy(c->off.begin(), c->off.end(), buf.begin());
+        std::copy(c->pairs.begin(), c->pairs.end(), buf.begin() + (ptrdiff_t)at);
+        c->dev = llm_->upload_table(buf.data(), buf.size() * 4);
+    } catch (const std::exception &ex) {   // (host memory exhausted by a huge table)
+        MG4_ERR("constraint_create: %s", ex.what());
+        return nullptr;
+    }
+    if (!c->dev) { MG4_ERR("constraint_create: device memory exhausted"); return nullptr; }
+    c->group = llm_->group();
+    return c;
+}
+bool Engine::constraint_attach(const std::shared_ptr<Constraint> &c) {
+    if (c && c->group != llm_->group()) { MG4_ERR("constraint_attach: the constraint was compiled for another model"); return false; }
+    cons_ = c;
+    cons_state_ = 0;
+    return true;
 }
 const char *Engine::id_to_token(int32_t id) const {  // minigpt4.cpp:2485-2497
     if (id == 2) return "</s>";

@@ -2,6 +2,7 @@
 // (minigpt4.cpp:1740-2522: init, encode_image, add_tokens, add_strings, add_embedding, sample_token,
 // id_to_token, reset) with a device-resident vision graph and LLaMA step instead of ggml/llama.cpp.
 #pragma once
+#include "constraint.h"
 #include "llama.h"
 #include "text.h"
 #include "tp.h"
@@ -59,11 +60,23 @@ public:
     Error add_embedding(const float *rows, int n_rows);
     int32_t sample_token(const SamplingParams &p);
     const char *id_to_token(int32_t id) const;
-    void reset() { n_past_ = 0; pend_ids_.clear(); pend_emb_.clear(); reply_.clear(); }
+    void reset() { n_past_ = 0; pend_ids_.clear(); pend_emb_.clear(); reply_clear(); }
     // the current reply's last LlamaDevice::kStopMax bytes (the reference's `chat` of a turn): a new turn or prompt clears it, every
-    // fed id's text extends it, so a reply streamed over several sample_until calls stops where one call would
-    void reply_clear() { reply_.clear(); }
+    // fed id's text extends it, so a reply streamed over several sample_until calls stops where one call would.  The attached
+    // constraint's state restarts and advances with it.
+    void reply_clear() { reply_.clear(); cons_state_ = 0; }
     void reply_take(const char *text);
+    void reply_take_id(int32_t id) { reply_take(id_to_token(id)); if (cons_) cons_state_ = cons_->next(cons_state_, id); }
+
+    // constrained replies (minigpt4_b200_constraint_*): compile an automaton against this context's vocabulary, its tables on the device
+    // counted in the group's shared bytes; null (and the reason logged) on bad input, a tensor-parallel context or exhausted device memory
+    std::shared_ptr<Constraint> make_constraint(int n_states, const int32_t *next, const uint8_t *accept);
+    // attach c (null: detach) with its state at the start; false for a constraint of another group
+    bool constraint_attach(const std::shared_ptr<Constraint> &c);
+    const Constraint *constraint() const { return cons_.get(); }
+    int constraint_state() const { return cons_state_; }
+    // the texts of every id, as minigpt4_end_chat returns them (the constraint compiler's vocabulary)
+    std::vector<std::string> token_texts() const;
     bool flush();                     // evaluate the queued prompt rows (see add_tokens)
     static constexpr int kMaxPending = LlamaDevice::kPrefillMax;
 
@@ -81,6 +94,8 @@ private:
     static bool group_valid(Engine *const *e, int n, const char *what);   // 1..LlamaDevice::kMaxBatch distinct non-NULL contexts of one group
     static bool batch_valid(Engine *const *e, int n, const int32_t *ids);
     static bool flush_group(Engine *const *e, int n);
+    static bool any_constrained(Engine *const *e, int n);
+    static void sample_constraints(Engine *const *e, int n, SampleConstraint *out);   // each context's tables and state for a sampling call
     // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)
     std::shared_ptr<VisionFile> vfile_;
     std::shared_ptr<VisionDevice> vis_;
@@ -94,6 +109,8 @@ private:
     std::vector<float> pend_emb_;
     int pend_base_ = 0;               // position of the first queued row
     std::string reply_;
+    std::shared_ptr<Constraint> cons_;   // the attached constraint (shared with the handle and other contexts) and its state here
+    int cons_state_ = 0;
     void ensure_token_table();          // the group's device table of id_to_token (sample_until's stop rule)
     int n_batch_ = 512;
 };

@@ -71,11 +71,13 @@ struct SamplerScratch {
     void *dev = nullptr;
     smp::MtState *mt = nullptr;
     MirostatState *mu = nullptr;   // right after the generator (smp::mirostat_state), in the padding before the ids
+    int *cons = nullptr;           // the constraint's state (smp::ConsCol::state), after μ
     int *ids = nullptr, *id = nullptr;
     unsigned long long *keys = nullptr;
     float *logit = nullptr, *p = nullptr, *aux = nullptr;
-    uint32_t *h_rng = nullptr;   // [625] pinned, then h_mu
+    uint32_t *h_rng = nullptr;   // [625] pinned, then h_mu, then h_cons
     MirostatState *h_mu = nullptr;
+    int *h_cons = nullptr;
     int32_t *h_ids = nullptr;    // [n_ids] pinned
     size_t bytes = 0;
     SamplerScratch(int n_vocab, int n_ids) {
@@ -84,11 +86,14 @@ struct SamplerScratch {
         bytes = o_id + 4 * V * 4;
         CUDA_CHECK(cudaMalloc(&dev, bytes));
         unsigned char *b = (unsigned char *)dev;
-        static_assert(sizeof(smp::MtState) == 625 * 4 && sizeof(smp::MtState) + sizeof(MirostatState) <= (sizeof(smp::MtState) + 255) / 256 * 256, "μ fits before the ids");
+        static_assert(sizeof(smp::MtState) == 625 * 4 && sizeof(smp::MtState) + sizeof(MirostatState) + 4 <= (sizeof(smp::MtState) + 255) / 256 * 256,
+                      "μ and the constraint's state fit before the ids");
         mt = (smp::MtState *)b; mu = (MirostatState *)(b + sizeof(smp::MtState)); ids = (int *)(b + o_ids); keys = (unsigned long long *)(b + o_keys);
+        cons = (int *)(mu + 1);
         id = (int *)(b + o_id); logit = (float *)(b + o_id + V * 4); p = (float *)(b + o_id + 2 * V * 4); aux = (float *)(b + o_id + 3 * V * 4);
-        CUDA_CHECK(cudaHostAlloc((void **)&h_rng, 625 * 4 + sizeof(MirostatState), cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_rng, 625 * 4 + sizeof(MirostatState) + 4, cudaHostAllocDefault));
         h_mu = (MirostatState *)(h_rng + 625);
+        h_cons = (int *)(h_mu + 1);
         CUDA_CHECK(cudaHostAlloc((void **)&h_ids, (size_t)n_ids * 4, cudaHostAllocDefault));
     }
     ~SamplerScratch() { if (dev) cudaFree(dev); if (h_rng) cudaFreeHost(h_rng); if (h_ids) cudaFreeHost(h_ids); }
@@ -1342,7 +1347,17 @@ static smp::StopArgs narrow(const smp::StopArgsWide &w) {
     return s;
 }
 // one sampling step of n contexts in one launch (grid n): the 8-column kernels up to 8 contexts, the wide ones above
-static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArgs &p, const smp::MirostatArgs &m, cudaStream_t s) {
+// k (may be null): the constrained twins, which take every column's constraint table
+static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArgs &p, const smp::MirostatArgs &m, cudaStream_t s,
+                          const smp::ConsArgsWide *k = nullptr) {
+    if (k) {
+        if (n <= 8) {
+            smp::ConsArgs k8{};
+            memcpy(k8.c, k->c, sizeof(k8.c));
+            smp::sample_cons_kernel<<<n, smp::kThreads, 0, s>>>(narrow(a), k8);
+        } else smp::sample_cons_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, *k);
+        return;
+    }
     if (n <= 8) {
         const smp::SampleArgs a8 = narrow(a);
         if (p.mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, m);
@@ -1351,7 +1366,15 @@ static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArg
     else smp::sample_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
 }
 static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArgsWide &sa, int n, const SamplingArgs &p, const smp::MirostatArgs &m,
-                                cudaStream_t s) {
+                                cudaStream_t s, const smp::ConsArgsWide *k = nullptr) {
+    if (k) {
+        if (n <= 8) {
+            smp::ConsArgs k8{};
+            memcpy(k8.c, k->c, sizeof(k8.c));
+            smp::sample_until_cons_kernel<<<n, smp::kThreads, 0, s>>>(narrow(a), narrow(sa), k8);
+        } else smp::sample_until_cons_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, *k);
+        return;
+    }
     if (n <= 8) {
         const smp::SampleArgs a8 = narrow(a);
         const smp::StopArgs s8 = narrow(sa);
@@ -1364,7 +1387,7 @@ static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArg
 static size_t sampler_state_bytes(const SamplingArgs &p) { return 625 * 4 + (p.mirostat ? sizeof(MirostatState) : 0); }
 
 cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
-                                         smp::SampleArgsWide &a) {
+                                         smp::SampleArgsWide &a, const SampleConstraint *cons, smp::ConsArgsWide *k) {
     LlamaDevice &L0 = *c[0];
     a = sample_args(p, L0.d_.n_vocab);
     cudaStream_t s = L0.stream_;
@@ -1384,6 +1407,12 @@ cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int
             memcpy(L.smp_->h_rng, rng[i], 625 * 4);
             if (p.mirostat) *L.smp_->h_mu = mu[i];
             CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, sampler_state_bytes(p), cudaMemcpyHostToDevice, s));
+        }
+        if (k) k->c[i] = smp::ConsCol{nullptr, nullptr, nullptr};
+        if (k && cons[i].off) {
+            *L.smp_->h_cons = cons[i].state;
+            CUDA_CHECK(cudaMemcpyAsync(L.smp_->cons, L.smp_->h_cons, sizeof(int), cudaMemcpyHostToDevice, s));
+            k->c[i] = smp::ConsCol{cons[i].off, cons[i].tr, L.smp_->cons};
         }
     }
     if (n >= 2) {
@@ -1433,15 +1462,22 @@ float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const S
     return ms;
 }
 
+static bool any_constrained(const SampleConstraint *cons, int n) {
+    for (int i = 0; cons && i < n; ++i) if (cons[i].off) return true;
+    return false;
+}
+
 float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                                MirostatState *mu, int32_t *ids_out) {
+                                MirostatState *mu, int32_t *ids_out, const SampleConstraint *cons) {
     smp::SampleArgsWide a;
+    smp::ConsArgsWide k;
+    const smp::ConsArgsWide *kp = any_constrained(cons, n) ? &k : nullptr;
     const smp::MirostatArgs m = mirostat_args(p);
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, kp ? &k : nullptr);
     CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
     for (int t = 0; t < steps; ++t) {
         a.step = t;
-        launch_sample(a, n, p, m, s);
+        launch_sample(a, n, p, m, s, kp);
         sampled_decode(c, n, n_past[0] + t, s);
     }
     return end_sampling(c, n, steps, p, rng, mu, ids_out, s);
@@ -1451,6 +1487,19 @@ void LlamaDevice::ensure_reply() {
     if (reply_) return;
     reply_.reset(new ReplyScratch(d_.n_vocab));
     owned_bytes_ += reply_->bytes;
+}
+SharedTable::~SharedTable() {
+    if (dev) cudaFree(dev);
+    if (std::shared_ptr<LlamaGroup> g = group.lock()) g->batch_bytes -= bytes;
+}
+std::shared_ptr<SharedTable> LlamaDevice::upload_table(const void *host, size_t bytes) {
+    void *d = nullptr;
+    if (cudaMalloc(&d, std::max<size_t>(bytes, 1)) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    CUDA_CHECK(cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice));
+    std::shared_ptr<SharedTable> t = std::make_shared<SharedTable>();
+    t->dev = d; t->bytes = bytes; t->group = group_;
+    group_->batch_bytes += bytes;
+    return t;
 }
 bool LlamaDevice::has_token_table() const { return group_->tokens.off != nullptr; }
 void LlamaDevice::set_token_table(const std::vector<int> &off, const std::string &bytes) {
@@ -1476,11 +1525,14 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
 }
 
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                                MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped) {
+                                MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
+                                const SampleConstraint *cons) {
     LlamaDevice &L0 = *c[0];
     smp::SampleArgsWide a;
+    smp::ConsArgsWide k;
+    const smp::ConsArgsWide *kp = any_constrained(cons, n) ? &k : nullptr;
     const smp::MirostatArgs m = mirostat_args(p);
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a);
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, kp ? &k : nullptr);
     smp::StopArgsWide sa{};
     sa.tab = L0.group_->tokens;
     for (int i = 0; i < n; ++i) {
@@ -1502,7 +1554,7 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         }
         for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
             a.step = issued;
-            launch_sample_until(a, sa, n, p, m, s);
+            launch_sample_until(a, sa, n, p, m, s, kp);
             sampled_decode(c, n, n_past[0] + issued, s);
         }
         for (int i = 0; i < n; ++i)

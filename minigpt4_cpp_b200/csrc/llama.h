@@ -57,9 +57,20 @@ struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; int 
 struct MirostatState { float mu[2]; int init[2]; };   // a context's mirostat μ of v1 / v2 and whether each is set (Sampler::get_mu)
 struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
 struct ReplyScratch;   // a context's stop state in sample_until: reply tail, stop text, done flag, snapshot (llama.cu, llama_sample.cuh)
-namespace smp { template <int N> struct SampleArgsN; }
+namespace smp { template <int N> struct SampleArgsN; template <int N> struct ConsArgsN; }
 
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
+// device memory for tables the contexts of a group share that may outlive its last context (constraint tables): counted in the group's
+// shared_bytes while the group lives, freed with the last reference (LlamaDevice::upload_table)
+struct SharedTable {
+    void *dev = nullptr;
+    size_t bytes = 0;
+    std::weak_ptr<LlamaGroup> group;
+    ~SharedTable();
+};
+// a context's constraint in a sampling call (constraint.h): its device tables (off null: unconstrained) and its state on entry; the
+// device moves its own copy of the state, and the host replays the fed ids through the host tables
+struct SampleConstraint { const int *off = nullptr; const int2 *tr = nullptr; int state = 0; };
 struct ScoreCall;      // the outputs of a score_rows call, which eval_rows_batch's passes fill (llama.cu)
 
 class LlamaDevice {
@@ -109,8 +120,9 @@ public:
     // i's mt19937 state (624 words and the position) on entry and on return, and with p.mirostat 1 / 2 mu[i] its mirostat μ (mu may be
     // null without mirostat); ids_out[s * n + i] is the id context i was fed at step s.
     // One synchronisation at the end; returns the device ms of the steps.  The caller validates (distinct, one group, room for steps).
+    // cons (may be null: none): context i samples over its constraint's allowed ids when cons[i].off is set (no mirostat then).
     static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                              MirostatState *mu, int32_t *ids_out);
+                              MirostatState *mu, int32_t *ids_out, const SampleConstraint *cons = nullptr);
     // sample_steps that stops each context after the step whose id's text (not exactly "##") makes its reply end with `stop` (0..32
     // bytes, "" no text stop), or after max_steps.  tail[i]: context i's reply so far (its last 32 bytes decide).  The steps are issued
     // kReplyChunk at a time; the host waits for chunk j - 1's done flags before it issues chunk j + 1 and stops issuing once every
@@ -119,8 +131,10 @@ public:
     // the group's token table (set_token_table).  One wait per chunk, none of them stalling the device; returns the device ms.
     static constexpr int kReplyChunk = 4;
     static constexpr int kStopMax = 32;   // longest stop text
+    // cons as in sample_steps; a constrained context also stops after the step that feeds id 2 (stopped[i] = 1).
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                              MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped);
+                              MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
+                              const SampleConstraint *cons = nullptr);
     // Copy src's conversation into n (1..kMaxBatch) distinct other contexts of its group (llama_state.cuh): K / V rows 0 .. n_past - 1,
     // logits, DeviceState and the pinned greedy id, in one launch that reads the source once.  Rows >= n_past of a destination are left
     // as they were; its sampler, reply state and hidden rows are not touched.  Waits for every context's stream first; synchronous.
@@ -133,6 +147,8 @@ public:
     // V[...] as F16 (kv: 2 n_layer n_past n_embd halves), one cudaMemcpyAsync per plane; from_host also sets the pinned greedy id
     void state_to_host(int n_past, DeviceState *st, float *logits, void *kv);
     void state_from_host(int n_past, const DeviceState &st, const float *logits, const void *kv);
+    // `bytes` of host memory in a new device allocation counted in the group's shared_bytes; null if device memory is exhausted
+    std::shared_ptr<SharedTable> upload_table(const void *host, size_t bytes);
     // the group's device table of every id's text (off: n_vocab + 1 offsets into bytes), counted in shared_bytes
     bool has_token_table() const;
     void set_token_table(const std::vector<int> &off, const std::string &bytes);
@@ -247,8 +263,9 @@ private:
     void ensure_reply();
     // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
     // returns the stream the steps run on
+    // cons (may be null): each constrained context's state goes to its device copy, and k takes every column's tables
     static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
-                                       smp::SampleArgsN<kMaxBatch> &a);
+                                       smp::SampleArgsN<kMaxBatch> &a, const SampleConstraint *cons = nullptr, smp::ConsArgsN<kMaxBatch> *k = nullptr);
     static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
     static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
                               cudaStream_t s);

@@ -390,10 +390,34 @@ template <class Drawn> __device__ __forceinline__ void draw(const SampleCtx &c, 
     drawn(idx);
 }
 
+// the candidates of a sampling step, in the order the host Sampler lists them: every id of the vocabulary, or a constrained column's
+// allowed ids, ascending (its state's row of the constraint table, constraint.h).  sample_body takes them from its argument type
+// (cand_*), so the kernels that sample every id instantiate it exactly as before.
+struct AllowedIds {
+    const int2 *tr;   // the row's (id, next state) pairs; null: an unconstrained column of a constrained launch, every id
+    int n;
+    __device__ __forceinline__ bool listed() const { return tr != nullptr; }
+};
+// the sampling parameters of a constrained column with its candidates
+struct ListedArgs {
+    int n_vocab, top_k;
+    float temp, top_p, tfs_z, typical_p;
+    AllowedIds src;
+};
+template <class A> struct CandTraits { static constexpr bool kListed = false; };
+template <> struct CandTraits<ListedArgs> { static constexpr bool kListed = true; };
+template <class A> __device__ __forceinline__ int cand_size(const A &a) { return a.n_vocab; }
+template <class A> __device__ __forceinline__ int cand_id(const A &, int j) { return j; }
+template <class A> __device__ __forceinline__ bool cand_listed(const A &) { return false; }
+__device__ __forceinline__ int cand_size(const ListedArgs &a) { return a.src.n; }
+__device__ __forceinline__ int cand_id(const ListedArgs &a, int j) { return a.src.tr ? a.src.tr[j].x : j; }
+__device__ __forceinline__ bool cand_listed(const ListedArgs &a) { return a.src.listed(); }
+
 // ---------------------------------------------------------------------------------------------------------------------------------
-// one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits as
-// Sampler::sample does and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in
-// tokens[0] (greedy = true; the generator is not read).  Otherwise the generator is written back after fed returns.
+// one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits over the
+// candidates of a (cand_*) as Sampler::sample (Sampler::sample_allowed for listed candidates) does and hands the id to fed(id, greedy) on thread 0.
+// temp <= 0: the greedy id the logits epilogue already left in tokens[0] (greedy = true; the generator is not read), or for listed
+// candidates their arg-max, the lower id on ties (greedy = false).  Otherwise the generator is written back after fed returns.
 // ---------------------------------------------------------------------------------------------------------------------------------
 template <class A, class Fed> __device__ __forceinline__ void sample_body(const A &a, const SampleCtx &c, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
@@ -402,18 +426,34 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     __shared__ unsigned long long sh_prefix;
     __shared__ int sh_need, sh_done, sh_n;
     __shared__ float red;
-    const int tid = threadIdx.x, n = a.n_vocab;
+    const int tid = threadIdx.x, n = cand_size(a);
     if (a.temp <= 0.f) {
+        if constexpr (CandTraits<A>::kListed) {
+            if (cand_listed(a)) {
+                if (tid == 0) sh_prefix = 0ull;
+                __syncthreads();
+                unsigned long long best = 0ull;
+                for (int j = tid; j < n; j += blockDim.x) { const int i = cand_id(a, j); best = max(best, desc_key(c.logits[i], i)); }
+                atomicMax(&sh_prefix, best);
+                __syncthreads();
+                if (tid == 0) fed(key_id(sh_prefix), false);
+                return;
+            }
+        }
         if (tid == 0) fed(c.state->tokens[0], true);
         return;
     }
     for (int i = tid; i < kMtN; i += blockDim.x) mt.x[i] = c.mt->x[i];
     if (tid == 0) mt.p = c.mt->p;
 
-    // ---- top_k: the k largest (logit desc, id asc) keys; k = top_k (<= 0: n_vocab) clamped to [1, n_vocab] as Sampler::top_k does
+    // ---- top_k: the k largest (logit desc, id asc) keys; k = top_k (<= 0: all candidates) clamped to [1, candidates] as Sampler::top_k does
     const int k = min(max(a.top_k <= 0 ? n : a.top_k, 1), n);
     if (k == n) {
-        for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i]; }
+        if constexpr (CandTraits<A>::kListed) {
+            for (int j = tid; j < n; j += blockDim.x) { const int i = cand_id(a, j); c.id[j] = i; c.logit[j] = c.logits[i]; }
+        } else {   // (written as before: the every-id kernels compile to the same code)
+            for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i]; }
+        }
     } else {
         // radix select, 8 bits at a time from the top: the threshold T with exactly k keys >= T (keys are distinct: they carry the id)
         unsigned long long mask = 0ull;
@@ -423,7 +463,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
             __syncthreads();
             const unsigned long long pre = sh_prefix;
             for (int i = tid; i < n; i += blockDim.x) {
-                const unsigned long long key = desc_key(c.logits[i], i);
+                const unsigned long long key = desc_key(c.logits[cand_id(a, i)], cand_id(a, i));
                 if ((key & mask) == pre) atomicAdd(&hist[(key >> shift) & 255], 1u);
             }
             __syncthreads();
@@ -443,8 +483,8 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
         __syncthreads();
         const unsigned long long T = sh_prefix;
         for (int i = tid; i < n; i += blockDim.x) {
-            const float v = c.logits[i];
-            if (desc_key(v, i) >= T) { const int j = atomicAdd(&sh_n, 1); c.id[j] = i; c.logit[j] = v; }
+            const float v = c.logits[cand_id(a, i)];
+            if (desc_key(v, cand_id(a, i)) >= T) { const int j = atomicAdd(&sh_n, 1); c.id[j] = cand_id(a, i); c.logit[j] = v; }
         }
     }
     __syncthreads();
@@ -735,6 +775,71 @@ __global__ void __launch_bounds__(kThreads) sample_until_mirostat_wide_kernel(co
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
     mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// constrained sampling (minigpt4_b200_constraint_*, DESIGN.md §4.12): twins of the four kernels above that take each column's constraint
+// table.  A constrained column samples over its state's allowed ids only and thread 0 moves its state after feeding; an unconstrained
+// column (off null) runs exactly what the kernels above run, so one launch takes a mix of both.
+// ---------------------------------------------------------------------------------------------------------------------------------
+struct ConsCol {
+    const int *off;      // the table's row offsets (n_states + 2; row n_states the finished state); null: unconstrained
+    const int2 *tr;      // its (id, next state) pairs
+    int *state;          // the column's state, which the host uploads before the call
+};
+template <int N> struct ConsArgsN { ConsCol c[N]; };
+struct ConsArgs : ConsArgsN<8> {};
+using ConsArgsWide = ConsArgsN<LlamaDevice::kMaxBatch>;
+static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) + sizeof(ConsArgsWide) <= 32764, "the widest constrained kernel's parameters fit the 32 764-byte limit");
+
+// the candidates of column k in its current state (read by every thread before thread 0 can write the next one)
+template <class A> __device__ __forceinline__ AllowedIds allowed_ids(const A &a, const ConsCol &k) {
+    if (!k.off) return AllowedIds{nullptr, a.n_vocab};
+    const int s = *k.state, o = k.off[s];
+    return AllowedIds{k.tr + o, k.off[s + 1] - o};
+}
+template <class A> __device__ __forceinline__ ListedArgs listed_args(const A &a, const AllowedIds &src) {
+    return ListedArgs{a.n_vocab, a.top_k, a.temp, a.top_p, a.tfs_z, a.typical_p, src};
+}
+// thread 0, after the draw: the state the fed id leads to (a binary search for it in the row)
+__device__ __forceinline__ void cons_advance(const ConsCol &k, const AllowedIds &src, int id) {
+    if (!src.listed()) return;
+    int lo = 0, hi = src.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (src.tr[mid].x < id) lo = mid + 1;
+        else hi = mid;
+    }
+    *k.state = src.tr[lo].y;
+}
+
+template <class A, class K> __device__ __forceinline__ void sample_cons_step(const A &a, const K &k) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    const ConsCol &kc = k.c[blockIdx.x];
+    const AllowedIds src = allowed_ids(a, kc);
+    sample_body(listed_args(a, src), c, [&](int id, bool greedy) { feed(a, c, id, greedy); cons_advance(kc, src, id); });
+}
+// sample_until's step on a constrained column also stops it after the step that feeds id 2 (</s>)
+template <class A, class S, class K> __device__ __forceinline__ void sample_until_cons_step(const A &a, const S &s, const K &k) {
+    const SampleCtx &c = a.c[blockIdx.x];
+    const ConsCol &kc = k.c[blockIdx.x];
+    ReplyState &r = *s.r[blockIdx.x];
+    __shared__ int sh_state;
+    if (!until_running(a, s, c, r, sh_state)) return;
+    const AllowedIds src = allowed_ids(a, kc);
+    sample_body(listed_args(a, src), c, [&](int id, bool greedy) {
+        until_feed(a, s, c, r, id, greedy);
+        cons_advance(kc, src, id);
+        if (src.listed() && id == 2) r.done = 1;
+    });
+}
+__global__ void __launch_bounds__(kThreads) sample_cons_kernel(const SampleArgs a, const ConsArgs k) { sample_cons_step(a, k); }
+__global__ void __launch_bounds__(kThreads) sample_cons_wide_kernel(const SampleArgsWide a, const ConsArgsWide k) { sample_cons_step(a, k); }
+__global__ void __launch_bounds__(kThreads) sample_until_cons_kernel(const SampleArgs a, const StopArgs s, const ConsArgs k) {
+    sample_until_cons_step(a, s, k);
+}
+__global__ void __launch_bounds__(kThreads) sample_until_cons_wide_kernel(const SampleArgsWide a, const StopArgsWide s, const ConsArgsWide k) {
+    sample_until_cons_step(a, s, k);
 }
 
 // seam: reply_take over ids[0, n) from r's tail; *stop_at = the index of the id that ends the reply, -1 if none does

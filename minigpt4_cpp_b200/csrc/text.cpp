@@ -186,12 +186,28 @@ int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingParams &
         mu_v2_ -= sp.mirostat_eta * (surprise_of(id) - sp.mirostat_tau);
         return id;
     }
+    return chain(c, k, sp);
+}
+
+int32_t Sampler::chain(std::vector<Candidate> &c, int k, const SamplingParams &sp) {
+    bool sorted = false;
     top_k(c, sorted, k, 1);
     tail_free(c, sorted, sp.tfs_z, 1);
     typical(c, sorted, sp.typical_p, 1);
     top_p(c, sorted, sp.top_p, 1);
     temperature(c, sp.temp);
     return draw(c, sorted);
+}
+
+int32_t Sampler::sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingParams &sp) {
+    if (sp.temp <= 0) {   // the first arg-max over the allowed ids, which are ascending: the lower id on ties
+        int best = 0;
+        for (int j = 1; j < n; ++j) if (logits[ids[j]] > logits[ids[best]]) best = j;
+        return ids[best];
+    }
+    std::vector<Candidate> c((size_t)n);
+    for (int j = 0; j < n; ++j) c[(size_t)j] = Candidate{ids[j], logits[ids[j]], 0.f};
+    return chain(c, sp.top_k <= 0 ? n : sp.top_k, sp);
 }
 
 }  // namespace mg4

@@ -37,6 +37,9 @@ public:
     // and penalize_nl are accepted by the ABI but never applied by the reference; same here.
     int32_t sample(const float *logits, int n_vocab, const SamplingParams &p);
     static int32_t greedy(const float *logits, int n_vocab);  // first arg-max
+    // sample over the candidates ids[0, n) only (ascending ids: a constraint's allowed ids), in that order: the chain of sample() with
+    // top_k <= 0 as n; temp <= 0: the first arg-max among them.  No mirostat.
+    int32_t sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingParams &p);
     // individual stages (exposed for unit tests)
     static void top_k(std::vector<Candidate> &c, bool &sorted, int k, size_t min_keep);
     static void softmax(std::vector<Candidate> &c, bool &sorted);
@@ -45,6 +48,8 @@ public:
     static void typical(std::vector<Candidate> &c, bool &sorted, float p, size_t min_keep);
     static void temperature(std::vector<Candidate> &c, float t);
     int32_t draw(std::vector<Candidate> &c, bool &sorted);
+    // the non-mirostat chain over the unsorted candidates c: top_k (k) -> tail_free -> typical -> top_p -> temperature -> draw
+    int32_t chain(std::vector<Candidate> &c, int k, const SamplingParams &p);
     // the generator's state through its textual representation (operator<< / >>): the 624 words, then the position in them
     void get_rng(uint32_t state[625]) const;
     void set_rng(const uint32_t state[625]);

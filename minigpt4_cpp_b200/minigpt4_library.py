@@ -231,6 +231,12 @@ _EXT = {
     "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_steps_mirostat": ([_VP, _I, _I, _F, _I, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until_mirostat": ([_VP, _I, _I, _S, _F, _I, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_constraint_create": ([_CTX, _I, _VP, _VP], _VP),
+    "minigpt4_b200_constraint_free": ([_VP], None),
+    "minigpt4_b200_constraint_attach": ([_CTX, _VP], _I),
+    "minigpt4_b200_constraint_state": ([_CTX, C.POINTER(_I), C.POINTER(_I)], _I),
+    "minigpt4_b200_constraint_allowed": ([_VP, _I, _VP, _VP, _I], _I),
+    "minigpt4_b200_host_constraint_allowed": ([_S, _I, _VP, _VP, _I, _VP, _VP, _I], _I),
     "minigpt4_b200_encode_images": ([_CTX, C.POINTER(MiniGPT4Images), C.POINTER(MiniGPT4Embeddings)], _I),
     "minigpt4_b200_stats": ([_CTX, C.POINTER(Stats)], _I),
     "minigpt4_b200_time_matvec": ([_CTX, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_double)], _I),
@@ -261,6 +267,30 @@ EXT_SYMBOLS = tuple(_EXT)
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def choices_dfa(choices: list[bytes]) -> tuple[np.ndarray, np.ndarray]:
+    """The byte automaton of "exactly one of these answers": a trie over the choices' bytes, start state 0.  Returns (next [n_states,
+    256] int32, -1 rejects; accept [n_states] uint8), the form minigpt4_b200_constraint_create takes."""
+    nxt: list[list[int]] = [[-1] * 256]
+    acc = [0]
+    for ch in choices:
+        s = 0
+        for b in bytes(ch):
+            if nxt[s][b] < 0:
+                nxt[s][b] = len(nxt)
+                nxt.append([-1] * 256)
+                acc.append(0)
+            s = nxt[s][b]
+        acc[s] = 1
+    return np.array(nxt, np.int32), np.array(acc, np.uint8)
+
+
+def _automaton(next_states, accept) -> tuple[np.ndarray, np.ndarray]:
+    nx = np.ascontiguousarray(next_states, np.int32)
+    ac = np.ascontiguousarray(accept, np.uint8)
+    assert nx.ndim == 2 and nx.shape[1] == 256 and ac.shape == (nx.shape[0],), "next [n_states, 256], accept [n_states]"
+    return nx, ac
 
 
 class B200:
@@ -441,6 +471,59 @@ class B200:
             self._chk(self.L.minigpt4_b200_sample_until(ctx, n, max_steps, st, temp, top_k, top_p, tfs_z, typical_p, _ptr(ids), _ptr(n_out),
                                                         _ptr(stopped), C.byref(ms)))
         return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
+    # constrained replies (minigpt4_b200_constraint_*): handles are plain ints (the C pointer)
+    def constraint_create(self, ctx, next_states, accept) -> int:
+        """compile the byte automaton (next [n_states, 256] int32, -1 rejects; accept [n_states]) against ctx's vocabulary; the handle"""
+        nx, ac = _automaton(next_states, accept)
+        h = self.L.minigpt4_b200_constraint_create(ctx.ptr, nx.shape[0], _ptr(nx), _ptr(ac))
+        assert h, "minigpt4_b200_constraint_create refused the automaton"
+        return h
+
+    def constraint_free(self, handle: int) -> None:
+        self.L.minigpt4_b200_constraint_free(handle)
+
+    def constraint_attach(self, ctx, handle: Optional[int]) -> None:
+        """attach the constraint (None: detach); its state starts at 0"""
+        self._chk(self.L.minigpt4_b200_constraint_attach(ctx.ptr, handle))
+
+    def constraint_state(self, ctx) -> tuple[int, bool]:
+        """(state, finished) of ctx's constraint; state is -1 once finished"""
+        st, fin = C.c_int(0), C.c_int(0)
+        self._chk(self.L.minigpt4_b200_constraint_state(ctx.ptr, C.byref(st), C.byref(fin)))
+        return st.value, bool(fin.value)
+
+    @staticmethod
+    def _allowed(call) -> Optional[tuple[np.ndarray, np.ndarray]]:
+        # room for one pair first: -1 then means a pruned state, not a short buffer
+        ids, nxt = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        n = call(_ptr(ids), _ptr(nxt), 1)
+        if n == -1:
+            return None
+        if n < 0:
+            ids, nxt = np.zeros(-n, np.int32), np.zeros(-n, np.int32)
+            n = call(_ptr(ids), _ptr(nxt), ids.size)
+            assert n == ids.size, n
+        return ids[:n], nxt[:n]
+
+    def constraint_allowed(self, handle: int, state: int) -> Optional[tuple[np.ndarray, np.ndarray]]:
+        """allowed(state) as compiled: (ids ascending, next states with -1 for finished); None for a state that is not live"""
+        return self._allowed(lambda ids, nxt, cap: self.L.minigpt4_b200_constraint_allowed(handle, state, ids, nxt, cap))
+
+    def host_constraint_allowed(self, llm_path: str, next_states, accept, state: int) -> Optional[tuple[np.ndarray, np.ndarray]]:
+        """constraint_allowed compiled on the host against the vocabulary of a ggjt file (no GPU); None for a state that is not live"""
+        nx, ac = _automaton(next_states, accept)
+        def call(ids, nxt, cap):
+            r = self.L.minigpt4_b200_host_constraint_allowed(llm_path.encode(), nx.shape[0], _ptr(nx), _ptr(ac), state, ids, nxt, cap)
+            assert r != -1000000, "unreadable file or refused automaton"
+            return r
+        return self._allowed(call)
+
+    def host_constraint_refused(self, llm_path: str, next_states, accept) -> bool:
+        """whether the host compiler refuses the automaton (next and accept taken as given)"""
+        nx = np.ascontiguousarray(next_states, np.int32).reshape(-1)
+        ac = np.ascontiguousarray(accept, np.uint8)
+        return self.L.minigpt4_b200_host_constraint_allowed(llm_path.encode(), ac.size, _ptr(nx), _ptr(ac), 0, None, None, 0) == -1000000
 
     def time_matvec(self, ctx, kind: int, reps: int = 3) -> tuple[float, float]:
         ms, nb = C.c_float(0), C.c_double(0)
@@ -724,7 +807,8 @@ class MiniGPT4ChatBot:
             yield token
 
     def generate_on_device(self, message: str, limit: int = 1024, chunk: int = 16, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
-                           tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0):
+                           tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0,
+                           constraint: Optional[int] = None):
         """generate() with the sampling and the stop check on the GPU: minigpt4_b200_sample_until (mirostat 1 / 2: _mirostat) calls of up
         to `chunk` steps, each stopping where generate()'s loop stops (the repetition arguments, which generate() passes on unused, are not
         taken).
@@ -732,13 +816,28 @@ class MiniGPT4ChatBot:
 
         One difference cannot be avoided: generate() decodes each token's bytes with errors="ignore" before it appends and checks them,
         so a piece that is not valid UTF-8 on its own drops out of its reply text, while the device compares the bytes.  The two can
-        disagree only where such a piece sits inside or next to the stop text."""
+        disagree only where such a piece sits inside or next to the stop text.
+
+        constraint: a handle of B200.constraint_create (or None): the reply is drawn from the ids the automaton allows (no mirostat) and
+        also ends after </s>, which is not yielded.  It is attached for this reply only."""
+        ext = B200(self.library)
+        if constraint is None:
+            yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
+                                                mirostat_eta)
+            return
+        ext.constraint_attach(self.ctx, constraint)
+        try:
+            yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
+                                                mirostat_eta)
+        finally:
+            ext.constraint_attach(self.ctx, None)
+
+    def _generate_on_device(self, ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta):
         if self.is_image_chat:
             self.is_image_chat = False
             self.library.minigpt4_begin_chat_image(self.ctx, self.embedding, message, self.n_threads)
         else:
             self.library.minigpt4_begin_chat(self.ctx, message, self.n_threads)
-        ext = B200(self.library)
         done = 0
         while done < limit:
             ids, stopped, _ = ext.sample_until([self.ctx], min(chunk, limit - done), None, temp, top_k, top_p, tfs_z, typical_p, mirostat,
