@@ -665,8 +665,8 @@ static void pq_build(PQMat &p, const QMat &m) {
 bool LlamaDevice::build_prefill() {
     if (getenv("MINIGPT4_B200_NO_PREFILL_GEMM")) return false;
     if (tp_ && tp_->world > 1) return false;  // (tensor-parallel ranks keep the per-op prefill path for now)
-    // (Q4 layers with Q4_K / Q5_0 / Q5_1 / Q8_0 token embeddings keep the per-op prefill path: no test covers them on the GEMM path)
-    if (!(tok_type_ == GG_F32 || tok_type_ == GG_F16 || tok_type_ == GG_Q4_0 || tok_type_ == GG_Q4_1 || tok_type_ == GG_Q5_K || tok_type_ == GG_Q6_K)) return false;
+    // (any token-embedding type the loader accepts: prompt rows are gathered by embed_rows_kernel, which decodes every one of them, on both
+    // prefill paths - tests/test_mixed_types_gpu.py)
     for (auto &L : layers_) {   // (each matrix stages its own input: mixed Q4_0 / Q4_1 layers are fine)
         if (!L.fused_qkv) return false;
         for (const QMat *m : {&L.qkv, &L.wo, &L.w13, &L.w2}) if (m->type != GG_Q4_0 && m->type != GG_Q4_1) return false;
@@ -738,6 +738,9 @@ bool LlamaDevice::build_mega() {
     const int wt = output_.type;
     if (wt != GG_Q4_0 && wt != GG_Q4_1 && wt != GG_Q5_K) return false;   // homogeneous Q4_0 / Q4_1 / Q5_K files (the reference README's q5_k download has a Q6_K output matrix: per-op path)
     for (auto &L : layers_) if (!L.fused_qkv || L.qkv.type != wt || L.wo.type != wt || L.w13.type != wt || L.w2.type != wt) return false;
+    // OP_EMBED decodes the token row with dequant_elem, which knows F32 / F16 / Q4_0 / Q4_1 / Q5_K / Q6_K only (any other type would embed
+    // zeros); Q4_K / Q5_0 / Q5_1 / Q8_0 token embeddings take the per-op graph, whose launch_embed decodes them
+    if (!(tok_type_ == GG_F32 || tok_type_ == GG_F16 || tok_type_ == GG_Q4_0 || tok_type_ == GG_Q4_1 || tok_type_ == GG_Q5_K || tok_type_ == GG_Q6_K)) return false;
     if (d_.n_embd % 256 || d_.n_ff % 32 || d_.n_embd > 1024 * mk6::kNormItems || d_.n_ff > 4 * mk6::kConsumerThreads * mk6::kPlainItems) return false;
     if (d_.head_dim != 128 || d_.n_head > sm_count_ || 7 * d_.n_layer + 3 > mk6::kMaxOps) return false;
     if (tp && (n_embd_local_ % 32 || n_ff_local_ % 32)) return false;
