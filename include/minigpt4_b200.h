@@ -187,6 +187,39 @@ MINIGPT4_API int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ct
                                                      int mirostat, float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out,
                                                      int32_t *stopped, float *ms_out);
 
+/* Beam search (DESIGN.md §4.13): the n_hyp best replies of the conversation of ctxs[0] by beam search with n_beams (1..16) beams, with no
+ * host round trip between steps.  ctxs[1 .. n_beams-1] are other contexts of its group that serve as working beams; the call overwrites
+ * their conversations.  ctxs[0]'s queued prompt pieces are evaluated first, by its own flush; n0 is then its n_past and T0 its reply tail.
+ *   Start: one live beam with no ids, score S = 0.0f, tail T0, beam index 0; H, the finished replies, holds at most n_beams entries.
+ *   Step t = 0 .. max_steps-1, for each live beam b with logits z after its ids: lp[v] = (float)((((double)z[v] - M) - log sum_u
+ *   exp((double)z[u] - M)), M = max z (the log-probabilities of minigpt4_b200_score_tokens, bit for bit); candidate (b, v) scores c =
+ *   S_b + lp[v] (a float32 add).  Candidates are ordered by c descending, then beam index ascending, then z[v] descending, then v
+ *   ascending (with one beam: the greedy order, ties included).  The first 2 n_beams candidates are walked in that order, rank r = 0, 1..:
+ *   a candidate ends its reply by minigpt4_b200_sample_until's rule (its text is not exactly "##", stop is not empty and tail_b + its
+ *   text ends with stop).  An ending candidate with r < n_beams is offered to H with final score (float)((double)c / pow(t + 1,
+ *   length_penalty)); one with r >= n_beams is dropped.  Each other candidate becomes the next live beam (S = c, beam index = the order it
+ *   is taken in) until n_beams are taken; there may be fewer.
+ *   Offering: added while |H| < n_beams; otherwise it replaces the worst entry (lowest score, the later offered on equal scores) if its
+ *   score is strictly greater.
+ *   End: after the step in which |H| reaches n_beams, or when no live beam is left; the live beams are then not offered (HF generate's
+ *   early_stopping=True).  A search that runs through step max_steps-1 offers every live beam, in beam order, with stopped 0.
+ * Outputs: the n_hyp best entries of H by final score descending, the earlier offered first on equal scores: ids_out[h * max_steps + j]
+ * (-1 padded), n_out[h] (the stopping id included), score_out[h] the final score, logprob_out[h] (may be NULL) its S, stopped[h] (may be
+ * NULL) 1 if the stop text ended it; entries beyond |H| get n_out 0 and score -INFINITY.  *ms_out (may be NULL): the CUDA-event time of
+ * the search's steps; it leaves out the copy of the conversation into ctxs[1..] at the start and, with 2 or more beams, the prompt pass
+ * that evaluates the best reply into ctxs[0] at the end (with one beam the steps feed it).
+ * Afterwards ctxs[0] is where minigpt4_b200_sample_until leaves it after feeding the best entry's ids (n_past n0 + n_out[0], K / V,
+ * logits bit for bit, greedy id, device state, reply tail), and every other context is as minigpt4_b200_session_copy of ctxs[0] before
+ * the call leaves it.  No generator or mirostat μ is touched.  n_beams = 1 gives exactly sample_until with temp 0, the same stop and
+ * max_steps.  The group's first call allocates the search state (16 KiB), 2 x 16 x n_ctx ids (256 KiB at n_ctx 2048) and one row of logits,
+ * counted in minigpt4_b200_session_info's shared bytes.
+ * NULL ctxs / ids_out / n_out / score_out, n_beams outside 1..16, NULL or duplicate contexts, contexts of different groups, max_steps < 1,
+ * n_hyp outside 1..n_beams, a stop text over 32 bytes, a non-finite length_penalty, a tensor-parallel or constrained context, an empty
+ * conversation (n_past 0, queued rows counted) or n0 + max_steps > n_ctx return 8 before any device work, with nothing changed. */
+MINIGPT4_API int minigpt4_b200_beam_search(struct MiniGPT4Context **ctxs, int n_beams, int max_steps, const char *stop, float length_penalty,
+                                           int n_hyp, int32_t *ids_out, int32_t *n_out, float *score_out, float *logprob_out, int32_t *stopped,
+                                           float *ms_out);
+
 /* Constrained replies (DESIGN.md §4.12): sample only the ids a deterministic automaton over bytes allows.  The automaton has n_states
  * states (1..65536), start state 0; next[s * 256 + b] is the state byte b leads to from s, or -1 to reject; accept[s] != 0 marks an
  * accepting state.  The text of an id is the C string minigpt4_end_chat returns for it (an id whose text is empty is never allowed).
@@ -312,6 +345,11 @@ MINIGPT4_API int minigpt4_b200_op_sample_timed(const float *logits, int n_vocab,
  * logits / ids_out / mu_out, n_vocab < 1, n_draws < 1, mirostat outside 1..2, on_device outside 0..1, or temp <= 0 on the device. */
 MINIGPT4_API int minigpt4_b200_op_sample_mirostat(const float *logits, int n_vocab, int seed, float temp, int mirostat, float mirostat_tau,
                                                   float mirostat_eta, int n_draws, int on_device, int32_t *ids_out, float *mu_out, float *kernel_ms);
+/* minigpt4_b200_beam_search's ordering through its kernels, without the stop rule: n_live (1..n_beams) beams with scores S[n_live] and
+ * logits [n_live][n_vocab], n_beams 1..16; parent_out / id_out / c_out [2 n_beams] receive the first min(2 n_beams, n_live n_vocab)
+ * candidates in order (the rest is not written).  8 for NULL arguments or out-of-range sizes. */
+MINIGPT4_API int minigpt4_b200_op_beam_rank(const float *logits, int n_live, const float *S, int n_beams, int n_vocab, int32_t *parent_out,
+                                            int32_t *id_out, float *c_out);
 MINIGPT4_API int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail,
                                              int32_t *stop_at);
 /* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with

@@ -279,6 +279,18 @@ int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_ste
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out,
                                 n_out, stopped, ms_out);
 }
+int minigpt4_b200_beam_search(struct MiniGPT4Context **ctxs, int n_beams, int max_steps, const char *stop, float length_penalty, int n_hyp,
+                              int32_t *ids_out, int32_t *n_out, float *score_out, float *logprob_out, int32_t *stopped, float *ms_out) {
+    return Engine::beam_search(reinterpret_cast<Engine *const *>(ctxs), n_beams, max_steps, stop, length_penalty, n_hyp, ids_out, n_out, score_out,
+                               logprob_out, stopped, ms_out);
+}
+int minigpt4_b200_op_beam_rank(const float *logits, int n_live, const float *S, int n_beams, int n_vocab, int32_t *parent_out, int32_t *id_out,
+                               float *c_out) {
+    if (!logits || !S || !parent_out || !id_out || !c_out || n_beams < 1 || n_beams > LlamaDevice::kMaxBeams || n_live < 1 || n_live > n_beams ||
+        n_vocab < 1)
+        return ErrFailedToAddString;
+    return LlamaDevice::test_beam_rank(logits, n_live, S, n_beams, n_vocab, parent_out, id_out, c_out) >= 0 ? 0 : ErrFailedToAddString;
+}
 int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int mirostat, float mirostat_tau,
                                         float mirostat_eta, int32_t *ids_out, float *ms_out) {
     if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;

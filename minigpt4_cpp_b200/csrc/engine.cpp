@@ -4,6 +4,7 @@
 #include <stddef.h>
 #include <string.h>
 #include <algorithm>
+#include <cmath>
 #include <exception>
 
 namespace mg4 {
@@ -210,6 +211,51 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
         e[i]->n_past_ += n_out[i];
         for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
     }
+    if (ms_out) *ms_out = ms;
+    return ErrNone;
+}
+Error Engine::beam_search(Engine *const *e, int n, int max_steps, const char *stop, float length_penalty, int n_hyp, int32_t *ids_out,
+                          int32_t *n_out, float *score_out, float *logprob_out, int32_t *stopped, float *ms_out) {
+    if (!e || !ids_out || !n_out || !score_out) { MG4_ERR("beam_search: NULL contexts or outputs"); return ErrFailedToAddString; }
+    if (n < 1 || n > LlamaDevice::kMaxBeams) { MG4_ERR("beam_search: %d beams (1 .. %d)", n, LlamaDevice::kMaxBeams); return ErrFailedToAddString; }
+    if (!group_valid(e, n, "beam_search")) return ErrFailedToAddString;
+    if (max_steps < 1) { MG4_ERR("beam_search: %d steps", max_steps); return ErrFailedToAddString; }
+    if (n_hyp < 1 || n_hyp > n) { MG4_ERR("beam_search: %d hypotheses (1 .. %d)", n_hyp, n); return ErrFailedToAddString; }
+    const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
+    if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("beam_search: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
+    if (!std::isfinite(length_penalty)) { MG4_ERR("beam_search: length_penalty is not finite"); return ErrFailedToAddString; }
+    for (int i = 0; i < n; ++i) {
+        if (e[i]->tp.world > 1) { MG4_ERR("beam_search: context %d is tensor-parallel", i); return ErrFailedToAddString; }
+        if (e[i]->cons_) { MG4_ERR("beam_search: context %d is constrained", i); return ErrFailedToAddString; }
+    }
+    Engine &c0 = *e[0];
+    const int n0 = c0.n_past_, n_ctx = c0.llm_->dims().n_ctx;
+    if (n0 == 0) { MG4_ERR("beam_search: the conversation is empty"); return ErrFailedToAddString; }
+    if (n0 + max_steps > n_ctx) { MG4_ERR("beam_search: %d + %d > n_ctx %d", n0, max_steps, n_ctx); return ErrFailedToAddString; }
+    if (!c0.flush()) return ErrFailedToAddString;
+    c0.ensure_token_table();
+    LlamaDevice *L[LlamaDevice::kMaxBeams];
+    for (int i = 0; i < n; ++i) L[i] = e[i]->llm_.get();
+    std::vector<LlamaDevice::BeamHyp> hyps;
+    const float ms = LlamaDevice::beam_search(L, n, max_steps, n0, st, c0.reply_, length_penalty, hyps);
+    for (int h = 0; h < n_hyp; ++h) {
+        const bool has = h < (int)hyps.size();
+        const int len = has ? (int)hyps[(size_t)h].ids.size() : 0;
+        for (int j = 0; j < max_steps; ++j) ids_out[(size_t)h * max_steps + j] = j < len ? hyps[(size_t)h].ids[(size_t)j] : -1;
+        n_out[h] = len;
+        score_out[h] = has ? hyps[(size_t)h].score : -INFINITY;
+        if (logprob_out) logprob_out[h] = has ? hyps[(size_t)h].logprob : -INFINITY;
+        if (stopped) stopped[h] = has ? hyps[(size_t)h].stopped : 0;
+    }
+    // the other contexts: the conversation as it was (as session_copy leaves a destination); e[0]: the best reply fed, as sample_until
+    // leaves a context that fed those ids.  One beam fed them with its own decode steps; with more, e[0]'s rows from n0 belong to
+    // several beams, and the best reply is evaluated again by the prompt pass (the bits of the decode steps)
+    const std::string tail = c0.reply_;
+    for (int i = 1; i < n; ++i) { e[i]->n_past_ = n0; e[i]->pend_ids_.clear(); e[i]->pend_emb_.clear(); e[i]->reply_ = tail; e[i]->cons_state_ = 0; }
+    const std::vector<int32_t> &best = hyps[0].ids;
+    if (n >= 2 && !c0.llm_->eval_rows(best.data(), (int)best.size(), nullptr, 0, n0)) return ErrFailedToAddString;
+    c0.n_past_ = n0 + (int)best.size();
+    for (int32_t id : best) c0.reply_take_id(id);
     if (ms_out) *ms_out = ms;
     return ErrNone;
 }

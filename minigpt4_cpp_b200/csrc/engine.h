@@ -36,6 +36,10 @@ public:
     // "###"; all or nothing
     static Error sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
                               int32_t *stopped, float *ms_out);
+    // the n_hyp best replies of e[0]'s conversation by beam search over n (1..16) contexts of its group (see minigpt4_b200_beam_search);
+    // all or nothing
+    static Error beam_search(Engine *const *e, int n, int max_steps, const char *stop, float length_penalty, int n_hyp, int32_t *ids_out,
+                             int32_t *n_out, float *score_out, float *logprob_out, int32_t *stopped, float *ms_out);
     // sample_until's text check over ids from the reply `tail` (see minigpt4_b200_op_reply_stop); -1: no id ends the reply
     Error reply_stop(const int32_t *ids, int n, const char *stop, const char *tail, int32_t *stop_at);
     // the queued prompt rows of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group in shared passes over the weights (see minigpt4_b200_flush_batch)

@@ -6,6 +6,7 @@
 #include "llama_sample.cuh"
 #include "llama_score.cuh"
 #include "llama_state.cuh"
+#include "llama_beam.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -55,8 +56,19 @@ struct LlamaGroup {
     DeviceState *score_state = nullptr;
     k::ScoreRow *score_rows = nullptr, *h_score_rows = nullptr;
     k::ScoreOut *score_out = nullptr, *h_score_out = nullptr;
+    // beam_search (built by the group's first call): the search state and its pinned mirror, each slot's ids and each hypothesis' ids
+    // ([2][kMaxBeams][n_ctx]), the first context's logits and DeviceState at the start of a call, the done flags of the last two chunks
+    beam::BeamState *beam = nullptr, *h_beam = nullptr;
+    int *beam_ids = nullptr;
+    float *beam_snap = nullptr;
+    DeviceState *beam_snap_state = nullptr;
+    int *h_beam_done = nullptr;
+    cudaEvent_t beam_ev[2] = {};
     ~LlamaGroup() {
         for (cudaGraphExec_t g : graph) if (g) cudaGraphExecDestroy(g);
+        for (void *p : {(void *)beam, (void *)beam_ids, (void *)beam_snap, (void *)beam_snap_state}) if (p) cudaFree(p);
+        for (void *p : {(void *)h_beam, (void *)h_beam_done}) if (p) cudaFreeHost(p);
+        for (cudaEvent_t e : beam_ev) if (e) cudaEventDestroy(e);
         for (void *p : {(void *)x, (void *)q, (void *)att, (void *)act, (void *)last, (void *)qact, (void *)state, (void *)tok, (void *)rows, (void *)slots, (void *)ids,
                         (void *)tokens.off, (void *)tokens.bytes, (void *)score_logits, (void *)score_state, (void *)score_rows, (void *)score_out})
             if (p) cudaFree(p);
@@ -1602,6 +1614,145 @@ int LlamaDevice::test_reply_stop(const int32_t *ids, int n, const std::string &s
     sync();
     cudaFree(d);
     return at;
+}
+
+// ------------------------------------------------------------------------------------------------
+// beam search (llama_beam.cuh): contexts c[0 .. n) are the slots; every step ranks, merges and reorders on the device, then runs the
+// decode step of every slot (n = 1: the context's own graph or megakernel, n >= 2: the batch graph with column ids -1).  The steps are
+// issued kReplyChunk at a time, as in sample_until.
+// ------------------------------------------------------------------------------------------------
+void LlamaDevice::build_beam_scratch() {
+    LlamaGroup &G = *group_;
+    const size_t b0 = t_dev_bytes;
+    dmalloc(&G.beam, sizeof(beam::BeamState));
+    dmalloc(&G.beam_ids, (size_t)2 * beam::kMaxBeams * d_.n_ctx * 4);
+    dmalloc(&G.beam_snap, (size_t)d_.n_vocab * 4);
+    dmalloc(&G.beam_snap_state, sizeof(DeviceState));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_beam, sizeof(beam::BeamState), cudaHostAllocDefault));
+    CUDA_CHECK(cudaHostAlloc((void **)&G.h_beam_done, 2 * sizeof(int), cudaHostAllocDefault));
+    for (cudaEvent_t &e : G.beam_ev) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    G.batch_bytes += t_dev_bytes - b0;
+}
+
+float LlamaDevice::beam_search(LlamaDevice *const *c, int n, int max_steps, int n0, const std::string &stop, const std::string &tail, float length_penalty,
+                               std::vector<BeamHyp> &hyps) {
+    LlamaDevice &L0 = *c[0];
+    LlamaGroup &G = *L0.group_;
+    for (int i = 0; i < n; ++i) c[i]->sync();
+    if (!G.beam) L0.build_beam_scratch();
+    const int V = L0.d_.n_vocab, stride = L0.d_.n_ctx;
+    const int32_t argmax0 = L0.argmax();
+    cudaStream_t s = L0.stream_;
+    if (n >= 2) {
+        if (!G.x) L0.build_group_workspace();
+        if (!G.graph[n]) L0.build_batch_graph(n);
+        copy_state(L0, c + 1, n - 1, n0);   // every slot starts from the conversation; its rows below n0 are not written again
+        s = G.stream;
+        CUDA_CHECK(cudaMemcpyAsync(G.beam_snap, L0.logits_, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(G.beam_snap_state, L0.state_, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
+        for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n0, -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
+        CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
+    }
+    beam::BeamState &h = *G.h_beam;
+    memset(&h, 0, sizeof h);
+    for (int i = 0; i < beam::kMaxBeams; ++i) h.beam[i] = -1;
+    h.beam[0] = 0;   // one live beam: no ids, S = 0, the reply's tail
+    reply_init(h.tail[0], stop, tail);
+    CUDA_CHECK(cudaMemcpyAsync(G.beam, G.h_beam, sizeof(beam::BeamState), cudaMemcpyHostToDevice, s));
+    beam::BeamArgs a{};
+    a.st = G.beam;
+    for (int i = 0; i < n; ++i) { a.logits[i] = c[i]->logits_; a.state[i] = c[i]->state_; }
+    a.slots = n >= 2 ? G.slots : nullptr;
+    a.ids = G.beam_ids; a.hids = G.beam_ids + (size_t)beam::kMaxBeams * stride; a.stride = stride;
+    a.n_beams = n; a.n_vocab = V; a.max_steps = max_steps; a.n0 = n0; a.length_penalty = length_penalty; a.tab = G.tokens;
+    if (n == 1) { a.snap = G.beam_snap; a.snap_state = G.beam_snap_state; }   // (with 2 or more beams they hold the start)
+    beam::ReorderArgs ra{};
+    ra.st = G.beam;
+    for (int i = 0; i < n; ++i) { ra.k[i] = (uint4 *)c[i]->kcache_; ra.v[i] = (uint4 *)c[i]->vcache_; }
+    ra.row = (long long)L0.n_embd_local_ * 2 / 16; ra.plane = (long long)L0.d_.n_ctx * ra.row; ra.n_layer = L0.d_.n_layer; ra.n0 = n0;
+    const dim3 rgrid((unsigned)std::max(1, 8 * L0.sm_count_ / (2 * L0.d_.n_layer)), (unsigned)(2 * L0.d_.n_layer));
+    CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
+    int issued = 0;
+    for (int j = 0; issued < max_steps; ++j) {
+        if (j >= 2) {   // chunk j - 2's flag; chunk j - 1 keeps the device busy meanwhile
+            CUDA_CHECK(cudaEventSynchronize(G.beam_ev[j % 2]));
+            if (G.h_beam_done[j % 2]) break;
+        }
+        for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
+            beam::beam_rank_kernel<<<n, beam::kRankThreads, 0, s>>>(a);
+            beam::beam_merge_kernel<<<1, beam::kMergeThreads, 0, s>>>(a);
+            L0.launches_ += 2;
+            if (n == 1) {
+                CUDA_CHECK(cudaGetLastError());
+                L0.decode_step(-1, n0 + issued);
+            } else {
+                beam::beam_reorder_kernel<<<rgrid, beam::kCopyThreads, 0, s>>>(ra);
+                CUDA_CHECK(cudaGetLastError());
+                CUDA_CHECK(cudaGraphLaunch(G.graph[n], s));
+                L0.launches_ += (unsigned long long)G.graph_kernels[n] + 1;
+            }
+        }
+        CUDA_CHECK(cudaMemcpyAsync(G.h_beam_done + j % 2, &G.beam->done, sizeof(int), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaEventRecord(G.beam_ev[j % 2], s));
+    }
+    CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
+    std::vector<int32_t> hid((size_t)n * stride);
+    CUDA_CHECK(cudaMemcpyAsync(G.h_beam, G.beam, sizeof(beam::BeamState), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaMemcpyAsync(hid.data(), a.hids, hid.size() * 4, cudaMemcpyDeviceToHost, s));
+    for (int i = 1; i < n; ++i) {   // the other slots go back to the conversation as it was
+        CUDA_CHECK(cudaMemcpyAsync(c[i]->logits_, G.beam_snap, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(c[i]->state_, G.beam_snap_state, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
+    }
+    if (n == 1) L0.sync_decode();
+    else CUDA_CHECK(cudaStreamSynchronize(s));
+    for (int i = 1; i < n; ++i) *c[i]->h_argmax_ = argmax0;
+    if (n == 1 && h.done == 2) {   // one beam ran steps past its reply: back to what the reply's last step left
+        CUDA_CHECK(cudaMemcpyAsync(L0.logits_, G.beam_snap, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(L0.state_, G.beam_snap_state, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
+        DeviceState snap{};
+        CUDA_CHECK(cudaMemcpyAsync(&snap, G.beam_snap_state, sizeof(DeviceState), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        *L0.h_argmax_ = snap.argmax_id;
+    }
+    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, L0.ev0_, L0.ev1_));
+    // H by final score descending, the earlier offered first on equal scores
+    std::vector<int> order((size_t)h.n_h);
+    for (int e = 0; e < h.n_h; ++e) order[(size_t)e] = e;
+    std::sort(order.begin(), order.end(), [&](int x, int y) {
+        return h.h[x].score != h.h[y].score ? h.h[x].score > h.h[y].score : h.h[x].seq < h.h[y].seq;
+    });
+    hyps.clear();
+    for (int e : order) {
+        const beam::Hyp &y = h.h[e];
+        const int32_t *p = hid.data() + (size_t)e * stride;
+        hyps.push_back(BeamHyp{std::vector<int32_t>(p, p + y.len), y.score, y.logprob, y.stopped});
+    }
+    return ms;
+}
+
+int LlamaDevice::test_beam_rank(const float *logits, int n_live, const float *S, int n_beams, int n_vocab, int32_t *parent, int32_t *id, float *c) {
+    beam::BeamState *st = nullptr;
+    float *lg = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&st, sizeof(beam::BeamState)));
+    CUDA_CHECK(cudaMalloc((void **)&lg, (size_t)n_live * n_vocab * 4));
+    std::unique_ptr<beam::BeamState> h(new beam::BeamState);
+    memset(h.get(), 0, sizeof(beam::BeamState));
+    for (int i = 0; i < beam::kMaxBeams; ++i) h->beam[i] = i < n_live ? i : -1;
+    for (int i = 0; i < n_live; ++i) h->S[i] = S[i];
+    CUDA_CHECK(cudaMemcpy(st, h.get(), sizeof(beam::BeamState), cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemcpy(lg, logits, (size_t)n_live * n_vocab * 4, cudaMemcpyHostToDevice));
+    beam::BeamArgs a{};
+    a.st = st;
+    for (int i = 0; i < n_live; ++i) a.logits[i] = lg + (size_t)i * n_vocab;
+    a.n_beams = n_beams; a.n_vocab = n_vocab; a.rank_only = 1;
+    beam::beam_rank_kernel<<<n_live, beam::kRankThreads>>>(a);
+    beam::beam_merge_kernel<<<1, beam::kMergeThreads>>>(a);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpy(h.get(), st, sizeof(beam::BeamState), cudaMemcpyDeviceToHost));
+    for (int r = 0; r < h->n_sorted; ++r) { parent[r] = h->sorted[r].beam; id[r] = h->sorted[r].id; c[r] = h->sorted[r].c; }
+    cudaFree(st); cudaFree(lg);
+    return h->n_sorted;
 }
 
 void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms,

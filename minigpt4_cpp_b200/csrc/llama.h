@@ -135,6 +135,20 @@ public:
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                               MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
                               const SampleConstraint *cons = nullptr);
+    // Beam search over n (1..kMaxBeams) distinct contexts of one group (llama_beam.cuh, DESIGN.md §4.13): c[0] holds the conversation
+    // (evaluated, n0 rows, reply `tail`), the others serve as working slots.  Runs the search of minigpt4_b200_beam_search through
+    // max_steps steps or its early end, with no host round trip between steps, and returns H in output order (score desc, earlier offered
+    // first).  Afterwards c[1..] hold c[0]'s logits, DeviceState and greedy id of the start (their K / V rows >= n0 are overwritten).  With
+    // one beam c[0] is where its decode steps left it after the reply's last id, as in sample_until; with more, c[0] holds rows of
+    // several beams, which the caller evaluates again.  The device ms cover the steps, not the copy into c[1..] at the start.  Needs the group's token table.  The group's first call allocates the search state
+    // and 2 kMaxBeams n_ctx ids (shared_bytes).  Returns the device ms.  The caller validates.
+    static constexpr int kMaxBeams = 16;
+    struct BeamHyp { std::vector<int32_t> ids; float score, logprob; int stopped; };
+    static float beam_search(LlamaDevice *const *c, int n, int max_steps, int n0, const std::string &stop, const std::string &tail, float length_penalty,
+                             std::vector<BeamHyp> &hyps);
+    // test seam: beam_rank_kernel and beam_merge_kernel's ordering over n_live host rows of logits with beam scores S; the first
+    // min(2 n_beams, candidates) candidates: parent beam, id, c.  Returns their count.
+    static int test_beam_rank(const float *logits, int n_live, const float *S, int n_beams, int n_vocab, int32_t *parent, int32_t *id, float *c);
     // Copy src's conversation into n (1..kMaxBatch) distinct other contexts of its group (llama_state.cuh): K / V rows 0 .. n_past - 1,
     // logits, DeviceState and the pinned greedy id, in one launch that reads the source once.  Rows >= n_past of a destination are left
     // as they were; its sampler, reply state and hidden rows are not touched.  Waits for every context's stream first; synchronous.
@@ -274,6 +288,7 @@ private:
     void build_group_workspace();    // the batched passes' rows, slot tables and stream (group-owned, at the first batched call)
     void build_batch_graph(int B);   // decode_batch's graph for B columns, captured on the group stream
     void build_score_scratch();      // score_rows' logits rows, entry tables and results (group-owned, at the first scoring call)
+    void build_beam_scratch();       // beam_search's state, ids and snapshot (group-owned, at the first call)
 };
 
 }  // namespace mg4

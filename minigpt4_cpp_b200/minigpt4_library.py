@@ -229,6 +229,8 @@ _EXT = {
     "minigpt4_b200_end_chat_batch": ([_VP, _I, _VP] + _SAMPLING, _I),
     "minigpt4_b200_sample_steps": ([_VP, _I, _I, _F, _I, _F, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_beam_search": ([_VP, _I, _I, _S, _F, _I, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_op_beam_rank": ([_VP, _I, _VP, _I, _I, _VP, _VP, _VP], _I),
     "minigpt4_b200_sample_steps_mirostat": ([_VP, _I, _I, _F, _I, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until_mirostat": ([_VP, _I, _I, _S, _F, _I, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_constraint_create": ([_CTX, _I, _VP, _VP], _VP),
@@ -471,6 +473,32 @@ class B200:
             self._chk(self.L.minigpt4_b200_sample_until(ctx, n, max_steps, st, temp, top_k, top_p, tfs_z, typical_p, _ptr(ids), _ptr(n_out),
                                                         _ptr(stopped), C.byref(ms)))
         return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
+    def beam_search(self, ctxs, max_steps: int, stop: str | bytes | None = None, length_penalty: float = 1.0,
+                    n_hyp: int = 1) -> tuple[list[tuple[list[int], float, float, bool]], float]:
+        """the n_hyp best replies of ctxs[0]'s conversation by beam search with len(ctxs) (1..16) beams; ctxs[1:] are other sessions of
+        its group used as working beams (their conversations are overwritten by ctxs[0]'s).  stop: None "###", "" no text stop.  Returns
+        ([(ids, final score, sum of log-probabilities, stopped), ...] best first, device ms); afterwards ctxs[0] has fed the best ids."""
+        n = len(ctxs)
+        ids = np.full((max(1, n_hyp), max(1, max_steps)), -1, np.int32)
+        n_out, stopped = np.zeros(max(1, n_hyp), np.int32), np.zeros(max(1, n_hyp), np.int32)
+        score, lp = np.zeros(max(1, n_hyp), np.float32), np.zeros(max(1, n_hyp), np.float32)
+        ms = C.c_float(0)
+        st = stop.encode() if isinstance(stop, str) else stop
+        self._chk(self.L.minigpt4_b200_beam_search(C.cast(self._ctx_array(ctxs), C.c_void_p), n, max_steps, st, length_penalty, n_hyp, _ptr(ids),
+                                                   _ptr(n_out), _ptr(score), _ptr(lp), _ptr(stopped), C.byref(ms)))
+        return [(ids[h, :n_out[h]].tolist(), float(score[h]), float(lp[h]), bool(stopped[h])) for h in range(n_hyp)], ms.value
+
+    def op_beam_rank(self, logits: np.ndarray, S: np.ndarray, n_beams: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """beam_search's candidate order through its kernels over host logits [n_live, n_vocab] and beam scores S [n_live]: the first
+        2 n_beams candidates' (parent beam, id, c)"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        s = np.ascontiguousarray(S, np.float32)
+        n_live, V = lg.shape
+        k = min(2 * n_beams, n_live * V)
+        par, ids, c = np.zeros(2 * n_beams, np.int32), np.zeros(2 * n_beams, np.int32), np.zeros(2 * n_beams, np.float32)
+        self._chk(self.L.minigpt4_b200_op_beam_rank(_ptr(lg), n_live, _ptr(s), n_beams, V, _ptr(par), _ptr(ids), _ptr(c)))
+        return par[:k], ids[:k], c[:k]
 
     # constrained replies (minigpt4_b200_constraint_*): handles are plain ints (the C pointer)
     def constraint_create(self, ctx, next_states, accept) -> int:
@@ -767,6 +795,9 @@ class MiniGPT4ChatBot:
         self._keep = None
 
     def free(self):
+        for c in getattr(self, "_beams", []):
+            self.library.minigpt4_free(c)
+        self._beams = []
         if self.ctx and self.ctx.ptr:
             self.library.minigpt4_free(self.ctx)
 
@@ -849,6 +880,36 @@ class MiniGPT4ChatBot:
                 token = ext.L.minigpt4_b200_token_text(self.ctx.ptr, t).decode("utf-8", errors="ignore")
                 if not self.library.minigpt4_contains_eos_token(token):
                     yield token
+
+    def generate_beam(self, message: str, num_beams: int = 4, limit: int = 1024, length_penalty: float = 1.0):
+        """generate() with beam search on the GPU (minigpt4_b200_beam_search): the best of num_beams (1..16) beams, deterministic.  The
+        num_beams - 1 working sessions are created on first use and kept.  Yields the best reply's tokens as generate_on_device does: no
+        "##" token, and not the token that completes "###"."""
+        ext = B200(self.library)
+        if not hasattr(self, "_beams"):
+            self._beams = []
+        while len(self._beams) < num_beams - 1:
+            self._beams.append(ext.session_create(self.ctx))
+        if self.is_image_chat:
+            self.is_image_chat = False
+            self.library.minigpt4_begin_chat_image(self.ctx, self.embedding, message, self.n_threads)
+        else:
+            self.library.minigpt4_begin_chat(self.ctx, message, self.n_threads)
+        steps = min(limit, self._room(ext))
+        if steps < 1:   # the conversation fills the context: no reply
+            return
+        hyps, _ = ext.beam_search([self.ctx] + self._beams[:num_beams - 1], steps, None, length_penalty)
+        ids, _, _, stopped = hyps[0]
+        for k, t in enumerate(ids):
+            if stopped and k == len(ids) - 1:
+                return
+            token = ext.L.minigpt4_b200_token_text(self.ctx.ptr, t).decode("utf-8", errors="ignore")
+            if not self.library.minigpt4_contains_eos_token(token):
+                yield token
+
+    def _room(self, ext) -> int:
+        """the positions left in the conversation (n_ctx - n_past, queued rows counted)"""
+        return ext.stats(self.ctx).n_ctx - ext.n_past(self.ctx)
 
     def reset_chat(self):
         self.is_image_chat = False
