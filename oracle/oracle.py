@@ -339,7 +339,7 @@ class OracleEngine:
         for i in range(0, len(ids), self.n_batch):  # add_tokens chunking minigpt4.cpp:2369-2379
             chunk = ids[i:i + self.n_batch]
             rc = lib().oracle_llama_eval(self.llm, _p(chunk), None, len(chunk), self.n_past, self.n_threads, _p(self.logits),
-                                         _p(tap) if tap is not None else None, tap_layer)
+                                         _p(tap[i:]) if tap is not None else None, tap_layer)   # (each chunk's rows at its own offset)
             if rc:
                 raise RuntimeError("FailedToAddString")
             self.n_past += len(chunk)
