@@ -186,6 +186,32 @@ MINIGPT4_API int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ct
 MINIGPT4_API int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp,
                                                      int mirostat, float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out,
                                                      int32_t *stopped, float *ms_out);
+/* Log-probabilities of a generated reply (DESIGN.md §4.14): minigpt4_b200_sample_until (mirostat 0) or minigpt4_b200_sample_until_mirostat
+ * (mirostat 1 or 2, which ignores top_k .. typical_p) that also reports, for every id it feeds, how likely that id was.
+ * Generation is unchanged: ids_out, n_out, stopped, *ms_out and the state every context is left in (n_past, K / V, logits, greedy id,
+ * device state, reply tail, generator, mirostat μ, constraint state) are exactly those of the call it stands for, and a reply streamed
+ * over several calls of either function stops at the same step.
+ * Records: entry e = s * n + i for step s of context i, s < n_out[i].  z is the logits context i held before step s: the raw model
+ * distribution (temperature 1, no top_k / tail_free / typical / top_p / mirostat cut, no constraint), as minigpt4_b200_get_logits returns it.
+ *   logprob_out[e] = (float)(((double)z[t] - M) - log sum_v exp((double)z[v] - M)), M = max z, t = ids_out[e]: the bits
+ *     minigpt4_b200_score_tokens reports for the same id after the same rows (the same sweep and reduction order).
+ *   rank_out[e] (may be NULL) = the ids ranked above t (a larger logit, or an equal logit and a lower id), as score_tokens ranks it.
+ *   top_ids_out[e * top_n + j] and top_logprob_out[e * top_n + j] (may be NULL), j < min(top_n, n_vocab): the j-th id in the order
+ *     (logit descending, id ascending) and its log-probability by the same formula.  Where rank_out[e] is 0, top_logprob_out[e * top_n]
+ *     equals logprob_out[e] bit for bit.
+ *   No entry (s >= n_out[i], also for steps the device ran past a context's stop, and j >= n_vocab): ids and ranks -1, log-probabilities NaN.
+ *   The arrays hold max_steps * n entries (top arrays: max_steps * n * top_n).
+ * Memory: a context's first call allocates its record buffer, n_ctx steps of 168 bytes (up to 20 alternatives each; 336 KiB at n_ctx
+ * 2048), counted in minigpt4_b200_session_info's owned bytes.  The records cost one extra kernel launch per step and one device-to-host
+ * copy per context at the end.
+ * Everything sample_until / sample_until_mirostat refuse, and NULL logprob_out, top_n outside 0..20, top_n > 0 with NULL top_ids_out,
+ * mirostat outside 0..2, or an empty conversation (n_past 0, queued rows counted; it has no logits to report on) return 8 before any
+ * device work, with nothing changed (queued rows are not evaluated). */
+MINIGPT4_API int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp,
+                                                     int32_t top_k, float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau,
+                                                     float mirostat_eta, int top_n, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
+                                                     float *logprob_out, int32_t *rank_out, int32_t *top_ids_out, float *top_logprob_out,
+                                                     float *ms_out);
 
 /* Beam search (DESIGN.md §4.13): the n_hyp best replies of the conversation of ctxs[0] by beam search with n_beams (1..16) beams, with no
  * host round trip between steps.  ctxs[1 .. n_beams-1] are other contexts of its group that serve as working beams; the call overwrites
@@ -350,6 +376,13 @@ MINIGPT4_API int minigpt4_b200_op_sample_mirostat(const float *logits, int n_voc
  * candidates in order (the rest is not written).  8 for NULL arguments or out-of-range sizes. */
 MINIGPT4_API int minigpt4_b200_op_beam_rank(const float *logits, int n_live, const float *S, int n_beams, int n_vocab, int32_t *parent_out,
                                             int32_t *id_out, float *c_out);
+/* minigpt4_b200_sample_until_logprobs' records through its kernel, over host rows: logits [rows][n_vocab] (rows 1..64), ids[rows] (one id
+ * per row, 0..n_vocab-1, as if each row's step had fed it), top_n 0..20.  logprob_out[rows], rank_out[rows] (may be NULL),
+ * top_ids_out / top_logprob_out (may be NULL) [rows][top_n], with the semantics and the -1 / NaN padding of sample_until_logprobs.
+ * *kernel_ms (may be NULL): the average CUDA-event time of one launch over all rows.  8 for NULL logits / ids / logprob_out, a NULL
+ * top_ids_out with top_n > 0, or out-of-range sizes or ids, before any device work. */
+MINIGPT4_API int minigpt4_b200_op_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, int top_n, float *logprob_out,
+                                           int32_t *rank_out, int32_t *top_ids_out, float *top_logprob_out, float *kernel_ms);
 MINIGPT4_API int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail,
                                              int32_t *stop_at);
 /* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with

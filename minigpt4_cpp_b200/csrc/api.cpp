@@ -303,6 +303,26 @@ int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, in
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop,
                                 SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, ids_out, n_out, stopped, ms_out);
 }
+int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
+                                        float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau, float mirostat_eta, int top_n,
+                                        int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *logprob_out, int32_t *rank_out,
+                                        int32_t *top_ids_out, float *top_logprob_out, float *ms_out) {
+    if (!ctxs) return ErrFailedToAddString;
+    // the sampling arguments of the call this one stands for
+    const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
+                                    : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
+    const LogprobRequest rec{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out};
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, p, ids_out, n_out, stopped, ms_out, &rec);
+}
+int minigpt4_b200_op_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, int top_n, float *logprob_out, int32_t *rank_out,
+                              int32_t *top_ids_out, float *top_logprob_out, float *kernel_ms) {
+    if (!logits || !ids || !logprob_out || rows < 1 || rows > LlamaDevice::kMaxBatch || n_vocab < 1 || top_n < 0 ||
+        top_n > LlamaDevice::kLogprobTop || (top_n > 0 && !top_ids_out))
+        return ErrFailedToAddString;
+    for (int r = 0; r < rows; ++r) if (ids[r] < 0 || ids[r] >= n_vocab) return ErrFailedToAddString;
+    LlamaDevice::test_logprobs(logits, rows, n_vocab, ids, LogprobRequest{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out}, kernel_ms);
+    return 0;
+}
 struct MiniGPT4B200Constraint *minigpt4_b200_constraint_create(struct MiniGPT4Context *ctx, int n_states, const int32_t *next, const uint8_t *accept) {
     if (!ctx) return nullptr;
     std::shared_ptr<Constraint> c = E(ctx)->make_constraint(n_states, next, accept);

@@ -186,8 +186,16 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
     return ErrNone;
 }
 Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                           int32_t *stopped, float *ms_out) {
+                           int32_t *stopped, float *ms_out, const LogprobRequest *rec) {
+    if (rec) {   // (arguments first: none of these reads a context)
+        if (!rec->logprob) { MG4_ERR("sample_until_logprobs: NULL logprob_out"); return ErrFailedToAddString; }
+        if (rec->top_n < 0 || rec->top_n > LlamaDevice::kLogprobTop) { MG4_ERR("sample_until_logprobs: top_n %d (0 .. %d)", rec->top_n, LlamaDevice::kLogprobTop); return ErrFailedToAddString; }
+        if (rec->top_n > 0 && !rec->top_ids) { MG4_ERR("sample_until_logprobs: NULL top_ids_out with top_n %d", rec->top_n); return ErrFailedToAddString; }
+        if (p.mirostat < 0 || p.mirostat > 2) { MG4_ERR("sample_until_logprobs: mirostat %d (0 .. 2)", p.mirostat); return ErrFailedToAddString; }
+    }
     if (!ids_out || !n_out || !group_valid(e, n, "sample_until")) return ErrFailedToAddString;
+    for (int i = 0; rec && i < n; ++i)
+        if (e[i]->n_past_ == 0) { MG4_ERR("sample_until_logprobs: context %d: the conversation is empty", i); return ErrFailedToAddString; }
     if (max_steps < 1) { MG4_ERR("sample_until: %d steps", max_steps); return ErrFailedToAddString; }
     const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
     if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("sample_until: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
@@ -205,7 +213,7 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
     SampleConstraint cons[LlamaDevice::kMaxBatch];
     sample_constraints(e, n, cons);
-    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons);
+    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons, rec);
     for (int i = 0; i < n; ++i) {
         set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += n_out[i];

@@ -34,8 +34,9 @@ public:
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
     // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
     // "###"; all or nothing
+    // rec (may be null): also each fed id's record (see minigpt4_b200_sample_until_logprobs), with its further refusals
     static Error sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                              int32_t *stopped, float *ms_out);
+                              int32_t *stopped, float *ms_out, const LogprobRequest *rec = nullptr);
     // the n_hyp best replies of e[0]'s conversation by beam search over n (1..16) contexts of its group (see minigpt4_b200_beam_search);
     // all or nothing
     static Error beam_search(Engine *const *e, int n, int max_steps, const char *stop, float length_penalty, int n_hyp, int32_t *ids_out,

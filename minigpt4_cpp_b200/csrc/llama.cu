@@ -7,11 +7,13 @@
 #include "llama_score.cuh"
 #include "llama_state.cuh"
 #include "llama_beam.cuh"
+#include "llama_logprob.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
 #include <string.h>
 #include <algorithm>
+#include <limits>
 
 namespace mg4 {
 using namespace k;
@@ -135,6 +137,21 @@ struct ReplyScratch {
         if (h_r) cudaFreeHost(h_r);
         if (h_done) cudaFreeHost(h_done);
         for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    }
+};
+
+// sample_until_logprobs' records of one context (llama_logprob.cuh): n_ctx steps on the device and their pinned mirror
+struct LogprobScratch {
+    lp::Record *rec = nullptr, *h_rec = nullptr;
+    size_t bytes = 0;
+    explicit LogprobScratch(int n_ctx) {
+        bytes = (size_t)n_ctx * sizeof(lp::Record);
+        CUDA_CHECK(cudaMalloc((void **)&rec, bytes));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_rec, bytes, cudaHostAllocDefault));
+    }
+    ~LogprobScratch() {
+        if (rec) cudaFree(rec);
+        if (h_rec) cudaFreeHost(h_rec);
     }
 };
 
@@ -307,6 +324,7 @@ LlamaDevice::~LlamaDevice() {
     if (stream_) cudaStreamDestroy(stream_);
     smp_.reset();
     reply_.reset();
+    logprob_.reset();
 }
 void LlamaDevice::free_weights() {
     for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
@@ -1503,6 +1521,11 @@ void LlamaDevice::ensure_reply() {
     reply_.reset(new ReplyScratch(d_.n_vocab));
     owned_bytes_ += reply_->bytes;
 }
+void LlamaDevice::ensure_logprob() {
+    if (logprob_) return;
+    logprob_.reset(new LogprobScratch(d_.n_ctx));
+    owned_bytes_ += logprob_->bytes;
+}
 SharedTable::~SharedTable() {
     if (dev) cudaFree(dev);
     if (std::shared_ptr<LlamaGroup> g = group.lock()) g->batch_bytes -= bytes;
@@ -1529,6 +1552,21 @@ void LlamaDevice::set_token_table(const std::vector<int> &off, const std::string
     G.batch_bytes += t_dev_bytes - b0;
 }
 
+// context i's records (steps 0 .. n_rec - 1) into the caller's layout (entry e = s * n + i); the other entries of its max_steps get -1 / NaN
+static void scatter_records(const lp::Record *r, int n_rec, int i, int n, int max_steps, const LogprobRequest &q) {
+    const float nan = std::numeric_limits<float>::quiet_NaN();
+    for (int t = 0; t < max_steps; ++t) {
+        const size_t e = (size_t)t * n + i;
+        const bool has = t < n_rec;
+        q.logprob[e] = has ? r[t].logprob : nan;
+        if (q.rank) q.rank[e] = has ? r[t].rank : -1;
+        for (int j = 0; j < q.top_n; ++j) {
+            q.top_ids[e * q.top_n + j] = has ? r[t].top_id[j] : -1;
+            if (q.top_logprob) q.top_logprob[e * q.top_n + j] = has ? r[t].top_lp[j] : nan;
+        }
+    }
+}
+
 // a context's ReplyState at the start of a call: its reply's last kStopMax bytes, the stop text, nothing fed
 static void reply_init(smp::ReplyState &r, const std::string &stop, const std::string &tail) {
     memset(&r, 0, sizeof(r));
@@ -1541,7 +1579,7 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
 
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                                 MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                                const SampleConstraint *cons) {
+                                const SampleConstraint *cons, const LogprobRequest *rec) {
     LlamaDevice &L0 = *c[0];
     smp::SampleArgsWide a;
     smp::ConsArgsWide k;
@@ -1550,13 +1588,19 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
     cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, kp ? &k : nullptr);
     smp::StopArgsWide sa{};
     sa.tab = L0.group_->tokens;
+    lp::LogprobArgs la{};
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         L.ensure_reply();
         reply_init(*L.reply_->h_r, stop, tail[i]);
         CUDA_CHECK(cudaMemcpyAsync(L.reply_->r, L.reply_->h_r, sizeof(smp::ReplyState), cudaMemcpyHostToDevice, s));
         sa.r[i] = L.reply_->r; sa.snap[i] = L.reply_->snap;
+        if (rec) {
+            L.ensure_logprob();
+            la.c[i] = lp::LogprobCol{L.logits_, L.state_, L.reply_->r, L.logprob_->rec};
+        }
     }
+    la.n_vocab = L0.d_.n_vocab; la.top_n = rec ? rec->top_n : 0;
     ReplyScratch &R0 = *L0.reply_;
     CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
     int issued = 0;
@@ -1570,6 +1614,11 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
             a.step = issued;
             launch_sample_until(a, sa, n, p, m, s, kp);
+            if (rec) {   // the logits the step sampled from, before the decode step replaces them
+                la.step = issued;
+                lp::logprob_rows_kernel<<<n, lp::kThreads, 0, s>>>(la);
+                ++L0.launches_;
+            }
             sampled_decode(c, n, n_past[0] + issued, s);
         }
         for (int i = 0; i < n; ++i)
@@ -1591,10 +1640,14 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
             CUDA_CHECK(cudaMemcpyAsync(L.state_, &L.reply_->r->snap, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
             *L.h_argmax_ = r.snap.argmax_id;
         }
+        if (rec && r.n_fed > 0)
+            CUDA_CHECK(cudaMemcpyAsync(L.logprob_->h_rec, L.logprob_->rec, (size_t)r.n_fed * sizeof(lp::Record), cudaMemcpyDeviceToHost, s));
     }
     CUDA_CHECK(cudaStreamSynchronize(s));
     for (int t = issued; t < max_steps; ++t)
         for (int i = 0; i < n; ++i) ids_out[(size_t)t * n + i] = -1;
+    if (rec)
+        for (int i = 0; i < n; ++i) scatter_records(c[i]->logprob_->h_rec, n_out[i], i, n, max_steps, *rec);
     return ms;
 }
 
@@ -1753,6 +1806,42 @@ int LlamaDevice::test_beam_rank(const float *logits, int n_live, const float *S,
     for (int r = 0; r < h->n_sorted; ++r) { parent[r] = h->sorted[r].beam; id[r] = h->sorted[r].id; c[r] = h->sorted[r].c; }
     cudaFree(st); cudaFree(lg);
     return h->n_sorted;
+}
+
+void LlamaDevice::test_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, const LogprobRequest &rec, float *kernel_ms) {
+    float *lg = nullptr;
+    DeviceState *st = nullptr;
+    lp::Record *out = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&lg, (size_t)rows * n_vocab * 4));
+    CUDA_CHECK(cudaMalloc((void **)&st, (size_t)rows * sizeof(DeviceState)));
+    CUDA_CHECK(cudaMalloc((void **)&out, (size_t)rows * sizeof(lp::Record)));
+    CUDA_CHECK(cudaMemcpy(lg, logits, (size_t)rows * n_vocab * 4, cudaMemcpyHostToDevice));
+    std::vector<DeviceState> hs((size_t)rows);
+    for (int r = 0; r < rows; ++r) { hs[(size_t)r] = DeviceState{}; hs[(size_t)r].tokens[0] = ids[r]; }
+    CUDA_CHECK(cudaMemcpy(st, hs.data(), (size_t)rows * sizeof(DeviceState), cudaMemcpyHostToDevice));
+    lp::LogprobArgs a{};
+    for (int r = 0; r < rows; ++r) a.c[r] = lp::LogprobCol{lg + (size_t)r * n_vocab, st + r, nullptr, out + r};
+    a.n_vocab = n_vocab; a.step = 0; a.top_n = rec.top_n;
+    lp::logprob_rows_kernel<<<rows, lp::kThreads>>>(a);
+    CUDA_CHECK(cudaGetLastError());
+    if (kernel_ms) {
+        constexpr int kReps = 50;
+        cudaEvent_t e0, e1;
+        CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+        CUDA_CHECK(cudaEventRecord(e0, 0));
+        for (int i = 0; i < kReps; ++i) lp::logprob_rows_kernel<<<rows, lp::kThreads>>>(a);
+        CUDA_CHECK(cudaEventRecord(e1, 0));
+        CUDA_CHECK(cudaEventSynchronize(e1));
+        float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+        *kernel_ms = ms / kReps;
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
+    }
+    std::vector<lp::Record> h((size_t)rows);
+    CUDA_CHECK(cudaMemcpy(h.data(), out, (size_t)rows * sizeof(lp::Record), cudaMemcpyDeviceToHost));
+    for (int r = 0; r < rows; ++r) scatter_records(h.data() + r, 1, 0, 1, 1, LogprobRequest{rec.top_n, rec.logprob + r, rec.rank ? rec.rank + r : nullptr,
+                                                                                  rec.top_ids ? rec.top_ids + (size_t)r * rec.top_n : nullptr,
+                                                                                  rec.top_logprob ? rec.top_logprob + (size_t)r * rec.top_n : nullptr});
+    for (void *p : {(void *)lg, (void *)st, (void *)out}) cudaFree(p);
 }
 
 void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms,

@@ -71,6 +71,10 @@ struct SharedTable {
 // a context's constraint in a sampling call (constraint.h): its device tables (off null: unconstrained) and its state on entry; the
 // device moves its own copy of the state, and the host replays the fed ids through the host tables
 struct SampleConstraint { const int *off = nullptr; const int2 *tr = nullptr; int state = 0; };
+// sample_until's record request (minigpt4_b200_sample_until_logprobs): top_n 0..kLogprobTop and the caller's arrays (rank, top_logprob may
+// be null; top_ids null only with top_n 0), laid out as that call states
+struct LogprobRequest { int top_n; float *logprob; int32_t *rank; int32_t *top_ids; float *top_logprob; };
+struct LogprobScratch; // a context's records of sample_until_logprobs and their pinned mirror (llama.cu, llama_logprob.cuh)
 struct ScoreCall;      // the outputs of a score_rows call, which eval_rows_batch's passes fill (llama.cu)
 
 class LlamaDevice {
@@ -132,9 +136,18 @@ public:
     static constexpr int kReplyChunk = 4;
     static constexpr int kStopMax = 32;   // longest stop text
     // cons as in sample_steps; a constrained context also stops after the step that feeds id 2 (stopped[i] = 1).
+    // rec (may be null: none, and no extra work is issued): every step also runs logprob_rows_kernel (llama_logprob.cuh) between its
+    // sampling launch and its decode step, and each context's first n_out[i] records come back in one copy at the end, scattered into rec's
+    // arrays (entries without a record: -1 / NaN).  A context's first such call allocates its records (kLogprobRecordBytes n_ctx,
+    // owned_bytes_).  The caller validates (n_past >= 1: there are logits to report on).
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                               MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                              const SampleConstraint *cons = nullptr);
+                              const SampleConstraint *cons = nullptr, const LogprobRequest *rec = nullptr);
+    static constexpr int kLogprobTop = 20;            // most alternatives a record holds
+    static constexpr int kLogprobRecordBytes = 168;   // one step's record: logprob, rank, kLogprobTop ids and log-probabilities
+    // test seam: logprob_rows_kernel over `rows` (1..kMaxBatch) host rows of logits, row r as a step that fed ids[r], into rec's arrays
+    // ([rows], [rows][top_n]); kernel_ms (may be null): the average CUDA-event time of one launch.  The caller validates.
+    static void test_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, const LogprobRequest &rec, float *kernel_ms);
     // Beam search over n (1..kMaxBeams) distinct contexts of one group (llama_beam.cuh, DESIGN.md §4.13): c[0] holds the conversation
     // (evaluated, n0 rows, reply `tail`), the others serve as working slots.  Runs the search of minigpt4_b200_beam_search through
     // max_steps steps or its early end, with no host round trip between steps, and returns H in output order (score desc, earlier offered
@@ -275,6 +288,8 @@ private:
     void ensure_sampler();
     std::unique_ptr<ReplyScratch> reply_;   // sample_until's stop state and snapshot, from the context's first call (owned_bytes_)
     void ensure_reply();
+    std::unique_ptr<LogprobScratch> logprob_;   // sample_until's records, from the context's first call with a request (owned_bytes_)
+    void ensure_logprob();
     // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
     // returns the stream the steps run on
     // cons (may be null): each constrained context's state goes to its device copy, and k takes every column's tables

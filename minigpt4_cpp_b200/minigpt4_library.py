@@ -233,6 +233,9 @@ _EXT = {
     "minigpt4_b200_op_beam_rank": ([_VP, _I, _VP, _I, _I, _VP, _VP, _VP], _I),
     "minigpt4_b200_sample_steps_mirostat": ([_VP, _I, _I, _F, _I, _F, _F, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until_mirostat": ([_VP, _I, _I, _S, _F, _I, _F, _F, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_sample_until_logprobs": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _I, _F, _F, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP,
+                                             C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_op_logprobs": ([_VP, _I, _I, _VP, _I, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_constraint_create": ([_CTX, _I, _VP, _VP], _VP),
     "minigpt4_b200_constraint_free": ([_VP], None),
     "minigpt4_b200_constraint_attach": ([_CTX, _VP], _I),
@@ -473,6 +476,38 @@ class B200:
             self._chk(self.L.minigpt4_b200_sample_until(ctx, n, max_steps, st, temp, top_k, top_p, tfs_z, typical_p, _ptr(ids), _ptr(n_out),
                                                         _ptr(stopped), C.byref(ms)))
         return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
+    def sample_until_logprobs(self, ctxs, max_steps: int, stop: str | bytes | None = None, top_n: int = 0, temp: float = 0.8, top_k: int = 40,
+                              top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0,
+                              mirostat_eta: float = 1.0) -> tuple[list[list[int]], list[bool], list[tuple], float]:
+        """sample_until (mirostat 1 / 2: sample_until_mirostat) with the same ids and end state, which also reports each fed id's
+        log-probability and rank under the raw logits it was drawn from, and the top_n (0..20) most likely ids there.  Returns each
+        context's fed ids, whether the stop text ended it, its records (logprob float32 [k], rank int32 [k], top ids int32 [k, top_n], top
+        log-probabilities float32 [k, top_n]; k its ids) and the device ms."""
+        n = len(ctxs)
+        shape = (max(1, max_steps), max(1, n))
+        ids, lp, rk = np.zeros(shape, np.int32), np.zeros(shape, np.float32), np.zeros(shape, np.int32)
+        tid, tlp = np.zeros(shape + (max(1, top_n),), np.int32), np.zeros(shape + (max(1, top_n),), np.float32)
+        n_out, stopped = np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.int32)
+        ms = C.c_float(0)
+        st = stop.encode() if isinstance(stop, str) else stop
+        self._chk(self.L.minigpt4_b200_sample_until_logprobs(C.cast(self._ctx_array(ctxs), C.c_void_p), n, max_steps, st, temp, top_k, top_p, tfs_z,
+                                                             typical_p, mirostat, mirostat_tau, mirostat_eta, top_n, _ptr(ids), _ptr(n_out),
+                                                             _ptr(stopped), _ptr(lp), _ptr(rk), _ptr(tid), _ptr(tlp), C.byref(ms)))
+        recs = [(lp[:k, i].copy(), rk[:k, i].copy(), tid[:k, i, :top_n].copy(), tlp[:k, i, :top_n].copy()) for i, k in enumerate(n_out[:n].tolist())]
+        return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], recs, ms.value
+
+    def op_logprobs(self, logits: np.ndarray, ids, top_n: int) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, float]:
+        """sample_until_logprobs' records through its kernel over host logits [rows, n_vocab] (rows 1..64) and one fed id per row:
+        (logprob [rows], rank [rows], top ids [rows, top_n], top log-probabilities [rows, top_n], kernel ms per launch)"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        rows, V = lg.shape
+        t = np.ascontiguousarray(ids, np.int32)
+        lp, rk = np.zeros(rows, np.float32), np.zeros(rows, np.int32)
+        tid, tlp = np.zeros((rows, max(1, top_n)), np.int32), np.zeros((rows, max(1, top_n)), np.float32)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_op_logprobs(_ptr(lg), rows, V, _ptr(t), top_n, _ptr(lp), _ptr(rk), _ptr(tid), _ptr(tlp), C.byref(ms)))
+        return lp, rk, tid[:, :top_n], tlp[:, :top_n], ms.value
 
     def beam_search(self, ctxs, max_steps: int, stop: str | bytes | None = None, length_penalty: float = 1.0,
                     n_hyp: int = 1) -> tuple[list[tuple[list[int], float, float, bool]], float]:
@@ -863,23 +898,55 @@ class MiniGPT4ChatBot:
         finally:
             ext.constraint_attach(self.ctx, None)
 
-    def _generate_on_device(self, ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta):
+    def generate_with_logprobs(self, message: str, top_n: int = 5, limit: int = 1024, chunk: int = 16, temp: float = 0.8, top_k: int = 40,
+                               top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0,
+                               mirostat_eta: float = 1.0, constraint: Optional[int] = None):
+        """generate_on_device() that yields (token, logprob, [(alt_token, alt_logprob), ...]) for exactly the tokens generate_on_device
+        yields with the same seed and arguments, through minigpt4_b200_sample_until_logprobs: the token's log-probability under the model's
+        raw distribution at that step (temperature 1, no sampling cut or constraint), and the top_n (0..20) most likely tokens there."""
+        ext = B200(self.library)
+        if constraint is None:
+            yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
+                                                mirostat_eta, top_n)
+            return
+        ext.constraint_attach(self.ctx, constraint)
+        try:
+            yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
+                                                mirostat_eta, top_n)
+        finally:
+            ext.constraint_attach(self.ctx, None)
+
+    def _generate_on_device(self, ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta,
+                            top_n=None):
+        """the reply's tokens; with top_n (not None) each as (token, logprob, alternatives)"""
         if self.is_image_chat:
             self.is_image_chat = False
             self.library.minigpt4_begin_chat_image(self.ctx, self.embedding, message, self.n_threads)
         else:
             self.library.minigpt4_begin_chat(self.ctx, message, self.n_threads)
+
+        def text(t):
+            return ext.L.minigpt4_b200_token_text(self.ctx.ptr, int(t)).decode("utf-8", errors="ignore")
         done = 0
         while done < limit:
-            ids, stopped, _ = ext.sample_until([self.ctx], min(chunk, limit - done), None, temp, top_k, top_p, tfs_z, typical_p, mirostat,
-                                               mirostat_tau, mirostat_eta)
+            steps = min(chunk, limit - done)
+            if top_n is None:
+                ids, stopped, _ = ext.sample_until([self.ctx], steps, None, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
+                                                   mirostat_eta)
+            else:
+                ids, stopped, recs, _ = ext.sample_until_logprobs([self.ctx], steps, None, top_n, temp, top_k, top_p, tfs_z, typical_p, mirostat,
+                                                                  mirostat_tau, mirostat_eta)
             done += len(ids[0])
             for k, t in enumerate(ids[0]):
                 if stopped[0] and k == len(ids[0]) - 1:
                     return
-                token = ext.L.minigpt4_b200_token_text(self.ctx.ptr, t).decode("utf-8", errors="ignore")
+                token = text(t)
                 if not self.library.minigpt4_contains_eos_token(token):
-                    yield token
+                    if top_n is None:
+                        yield token
+                    else:
+                        lp, _, tid, tlp = recs[0]
+                        yield token, float(lp[k]), [(text(a), float(b)) for a, b in zip(tid[k], tlp[k])]
 
     def generate_beam(self, message: str, num_beams: int = 4, limit: int = 1024, length_penalty: float = 1.0):
         """generate() with beam search on the GPU (minigpt4_b200_beam_search): the best of num_beams (1..16) beams, deterministic.  The
