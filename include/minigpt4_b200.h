@@ -212,6 +212,54 @@ MINIGPT4_API int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ct
                                                      float mirostat_eta, int top_n, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
                                                      float *logprob_out, int32_t *rank_out, int32_t *top_ids_out, float *top_logprob_out,
                                                      float *ms_out);
+/* Repetition, presence and frequency penalties (DESIGN.md §4.15), opt in: minigpt4_end_chat, end_chat_image, end_chat_batch, sample_steps,
+ * sample_until, beam search and the logprob calls take or ignore these arguments as the reference does, and never apply them.
+ * The semantics follow llama.cpp master-31cfbb1: llama_sample_repetition_penalty, then llama_sample_frequency_and_presence_penalties, then
+ * main.cpp's penalize_nl, applied to a copy of the logits before the unchanged sampler.
+ *   Window: the caller supplies each context's recent ids, as llama.cpp's sampling API takes last_tokens.  The window W of context i at
+ *   step s of a call is the last min(repeat_last_n, n_last[i] + s) entries of last_ids_i ++ (the ids fed to i at steps 0 .. s-1 of this
+ *   call).  Unlike llama.cpp's main, which pre-fills its ring with id 0, W holds only real ids; the engine keeps no history of its own, so
+ *   the caller decides whether prompt ids count (MiniGPT4ChatBot.generate_on_device passes the ids of the reply so far).
+ *   Penalised logits, in float32 with every operation rounded on its own (no contraction): for each id v with c = its count in W, c >= 1,
+ *   and z its raw logit,
+ *     z1 = repeat_penalty == 1 ? z : (z <= 0 ? z * repeat_penalty : z / repeat_penalty)   (IEEE division),
+ *     z' = (alpha_frequency == 0 && alpha_presence == 0) ? z1 : z1 - ((float)c * alpha_frequency + alpha_presence);
+ *   ids with c = 0 keep z, and with penalize_nl 0 and n_vocab > 13 id 13 (llama_token_nl() of that llama.cpp) keeps its raw z.  At
+ *   master-31cfbb1 main.cpp restored logits[nl] after the candidates had been copied, so there its restore had no effect; this project
+ *   implements the intended behaviour.
+ *   Sampling: a step samples z' exactly as sample_until / sample_until_mirostat sample z: the same chain, mirostat μ, generator and
+ *   constraint (allowed(s) over z'), the same tie rule (lower id); greedy (temp <= 0) takes the first arg-max of z' (over allowed(s) on a
+ *   constrained context).  No draw is added or removed.  The stop rule, max_steps, the steps run past a stop and n_out / stopped are
+ *   those of sample_until.
+ *   End state: each context ends where n_out[i] calls of minigpt4_b200_end_chat_penalized with the same arguments (last_ids there: the
+ *   history and the ids fed before) leave it: n_past and K / V, logits (the raw model logits: the buffer minigpt4_b200_get_logits reads is
+ *   never overwritten), greedy id, device state, reply tail, generator, μ and constraint state.
+ *   Neutral parameters (repeat_penalty 1 with both alphas 0, any penalize_nl; or repeat_last_n 0): ids and end state are bit-identical to
+ *   sample_until / sample_until_mirostat, and the call issues exactly their work.
+ * last_ids holds the contexts' histories one after another (context i's n_last[i] ids after those of contexts 0 .. i-1); n_last NULL means
+ * no history.  mirostat 0 samples with top_k .. typical_p, 1 or 2 with mirostat (which ignores them).  Other arguments and outputs are
+ * those of sample_until.
+ * Memory: a context's first call with penalties that are not neutral allocates its penalised row and window counts (8 n_vocab bytes) and
+ * a history buffer of n_ctx ids (4 n_ctx bytes; 264 KB at n_vocab 32000, n_ctx 2048), counted in minigpt4_b200_session_info's owned bytes;
+ * a later call whose window needs more than n_ctx history ids grows the buffer to them.  The penalties cost one kernel launch per step.
+ * Everything sample_until / sample_until_mirostat refuse, and mirostat outside 0..2, repeat_last_n < 0, a non-finite or <= 0
+ * repeat_penalty, a non-finite alpha, penalize_nl outside 0..1, n_last[i] < 0, n_last[i] > 0 with NULL last_ids or a history id outside
+ * 0..n_vocab-1 return 8 before any device work, with nothing changed (queued rows are not evaluated). */
+MINIGPT4_API int minigpt4_b200_sample_until_penalized(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp,
+                                                      int32_t top_k, float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau,
+                                                      float mirostat_eta, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
+                                                      float alpha_frequency, int penalize_nl, const int32_t *last_ids, const int32_t *n_last,
+                                                      int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out);
+/* The host twin of minigpt4_b200_sample_until_penalized: minigpt4_end_chat with the context's own host sampler run on the penalised copy of
+ * its logits, the window being the last min(repeat_last_n, n_last) of last_ids (a host loop passes the history and every id it fed
+ * since).  *token = the fed id's text, as minigpt4_end_chat returns it; *id_out (may be NULL) = the id.  The reply tail and constraint
+ * state advance as minigpt4_end_chat advances them; with neutral penalties the call is minigpt4_end_chat.  NULL ctx / token and the
+ * argument refusals of sample_until_penalized (n_last < 0, NULL last_ids with n_last > 0, a history id out of range, mirostat 1 / 2 on a
+ * constrained context) return 8 with nothing changed. */
+MINIGPT4_API int minigpt4_b200_end_chat_penalized(struct MiniGPT4Context *ctx, const char **token, float temp, int32_t top_k, float top_p,
+                                                  float tfs_z, float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
+                                                  float alpha_frequency, int penalize_nl, int mirostat, float mirostat_tau, float mirostat_eta,
+                                                  const int32_t *last_ids, int n_last, int32_t *id_out);
 
 /* Beam search (DESIGN.md §4.13): the n_hyp best replies of the conversation of ctxs[0] by beam search with n_beams (1..16) beams, with no
  * host round trip between steps.  ctxs[1 .. n_beams-1] are other contexts of its group that serve as working beams; the call overwrites
@@ -383,6 +431,14 @@ MINIGPT4_API int minigpt4_b200_op_beam_rank(const float *logits, int n_live, con
  * top_ids_out with top_n > 0, or out-of-range sizes or ids, before any device work. */
 MINIGPT4_API int minigpt4_b200_op_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, int top_n, float *logprob_out,
                                            int32_t *rank_out, int32_t *top_ids_out, float *top_logprob_out, float *kernel_ms);
+/* minigpt4_b200_sample_until_penalized's penalised logits over host rows: logits [rows][n_vocab] (rows 1..64), row r's window the last
+ * min(repeat_last_n, n_last[r]) of its history (last_ids: the rows' histories one after another; n_last NULL: none), as at step 0 of that
+ * call; out [rows][n_vocab] = z'.  on_device 1: its kernel, *kernel_ms (may be NULL) the average CUDA-event time of one launch over all
+ * rows; on_device 0: the host sampler's penalize (no GPU touched), *kernel_ms 0.  8 for NULL logits / out, out-of-range sizes, on_device
+ * outside 0..1 and the penalty refusals of sample_until_penalized, before any device work. */
+MINIGPT4_API int minigpt4_b200_op_penalize(const float *logits, int rows, int n_vocab, const int32_t *last_ids, const int32_t *n_last,
+                                           int32_t repeat_last_n, float repeat_penalty, float alpha_presence, float alpha_frequency, int penalize_nl,
+                                           int on_device, float *out, float *kernel_ms);
 MINIGPT4_API int minigpt4_b200_op_reply_stop(struct MiniGPT4Context *ctx, const int32_t *ids, int n, const char *stop, const char *tail,
                                              int32_t *stop_at);
 /* the device sampler's expf (fn 0) / logf (fn 1) over the float bit patterns lo_bits .. hi_bits (inclusive), compared bit for bit with

@@ -323,6 +323,57 @@ int minigpt4_b200_op_logprobs(const float *logits, int rows, int n_vocab, const 
     LlamaDevice::test_logprobs(logits, rows, n_vocab, ids, LogprobRequest{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out}, kernel_ms);
     return 0;
 }
+int minigpt4_b200_sample_until_penalized(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
+                                         float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau, float mirostat_eta,
+                                         int32_t repeat_last_n, float repeat_penalty, float alpha_presence, float alpha_frequency, int penalize_nl,
+                                         const int32_t *last_ids, const int32_t *n_last, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
+                                         float *ms_out) {
+    if (!ctxs) return ErrFailedToAddString;
+    // the sampling arguments of the call this one stands for
+    const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
+                                    : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
+    const PenaltyRequest pen{PenaltyParams{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl}, last_ids, n_last};
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, p, ids_out, n_out, stopped, ms_out, nullptr, &pen);
+}
+int minigpt4_b200_end_chat_penalized(struct MiniGPT4Context *ctx, const char **token, float temp, int32_t top_k, float top_p, float tfs_z,
+                                     float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence, float alpha_frequency,
+                                     int penalize_nl, int mirostat, float mirostat_tau, float mirostat_eta, const int32_t *last_ids, int n_last,
+                                     int32_t *id_out) {
+    if (!ctx) return ErrFailedToAddString;
+    const SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    return E(ctx)->end_chat_penalized(sp, PenaltyParams{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl}, last_ids, n_last,
+                                      token, id_out);
+}
+int minigpt4_b200_op_penalize(const float *logits, int rows, int n_vocab, const int32_t *last_ids, const int32_t *n_last, int32_t repeat_last_n,
+                              float repeat_penalty, float alpha_presence, float alpha_frequency, int penalize_nl, int on_device, float *out,
+                              float *kernel_ms) {
+    const PenaltyParams q{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl};
+    if (!logits || !out || rows < 1 || rows > LlamaDevice::kMaxBatch || n_vocab < 1 || (on_device != 0 && on_device != 1) ||
+        !Engine::penalty_valid(q, 0, "op_penalize"))
+        return ErrFailedToAddString;
+    std::vector<int32_t> none((size_t)rows, 0);
+    if (!n_last) n_last = none.data();
+    size_t at = 0;
+    for (int r = 0; r < rows; ++r) {
+        if (n_last[r] < 0 || (n_last[r] > 0 && !last_ids)) return ErrFailedToAddString;
+        for (int j = 0; j < n_last[r]; ++j) if (last_ids[at + j] < 0 || last_ids[at + j] >= n_vocab) return ErrFailedToAddString;
+        at += (size_t)n_last[r];
+    }
+    if (on_device) {
+        LlamaDevice::test_penalize(logits, rows, n_vocab, last_ids, n_last, q, out, kernel_ms);
+        return 0;
+    }
+    memcpy(out, logits, (size_t)rows * n_vocab * 4);
+    at = 0;
+    for (int r = 0; r < rows; ++r) {
+        const int w = std::min(repeat_last_n, n_last[r]);
+        Sampler::penalize(out + (size_t)r * n_vocab, n_vocab, last_ids + at + (n_last[r] - w), w, repeat_penalty, alpha_presence, alpha_frequency,
+                          penalize_nl);
+        at += (size_t)n_last[r];
+    }
+    if (kernel_ms) *kernel_ms = 0.f;
+    return 0;
+}
 struct MiniGPT4B200Constraint *minigpt4_b200_constraint_create(struct MiniGPT4Context *ctx, int n_states, const int32_t *next, const uint8_t *accept) {
     if (!ctx) return nullptr;
     std::shared_ptr<Constraint> c = E(ctx)->make_constraint(n_states, next, accept);

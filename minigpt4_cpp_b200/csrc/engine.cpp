@@ -186,16 +186,27 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
     return ErrNone;
 }
 Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                           int32_t *stopped, float *ms_out, const LogprobRequest *rec) {
+                           int32_t *stopped, float *ms_out, const LogprobRequest *rec, const PenaltyRequest *pen) {
     if (rec) {   // (arguments first: none of these reads a context)
         if (!rec->logprob) { MG4_ERR("sample_until_logprobs: NULL logprob_out"); return ErrFailedToAddString; }
         if (rec->top_n < 0 || rec->top_n > LlamaDevice::kLogprobTop) { MG4_ERR("sample_until_logprobs: top_n %d (0 .. %d)", rec->top_n, LlamaDevice::kLogprobTop); return ErrFailedToAddString; }
         if (rec->top_n > 0 && !rec->top_ids) { MG4_ERR("sample_until_logprobs: NULL top_ids_out with top_n %d", rec->top_n); return ErrFailedToAddString; }
         if (p.mirostat < 0 || p.mirostat > 2) { MG4_ERR("sample_until_logprobs: mirostat %d (0 .. 2)", p.mirostat); return ErrFailedToAddString; }
     }
+    if (pen && !penalty_valid(pen->q, p.mirostat, "sample_until_penalized")) return ErrFailedToAddString;
     if (!ids_out || !n_out || !group_valid(e, n, "sample_until")) return ErrFailedToAddString;
     for (int i = 0; rec && i < n; ++i)
         if (e[i]->n_past_ == 0) { MG4_ERR("sample_until_logprobs: context %d: the conversation is empty", i); return ErrFailedToAddString; }
+    if (pen) {
+        const int n_vocab = e[0]->llm_->dims().n_vocab;
+        size_t at = 0;
+        for (int i = 0; i < n; ++i) {
+            const int n_last = pen->n_last ? pen->n_last[i] : 0;
+            if (!history_valid(pen->last_ids ? pen->last_ids + at : nullptr, n_last, n_vocab, "sample_until_penalized")) return ErrFailedToAddString;
+            at += (size_t)std::max(0, n_last);
+        }
+        if (pen->q.neutral()) pen = nullptr;   // no logit changes: exactly sample_until's work
+    }
     if (max_steps < 1) { MG4_ERR("sample_until: %d steps", max_steps); return ErrFailedToAddString; }
     const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
     if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("sample_until: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
@@ -213,13 +224,54 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
     SampleConstraint cons[LlamaDevice::kMaxBatch];
     sample_constraints(e, n, cons);
-    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons, rec);
+    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons, rec, pen);
     for (int i = 0; i < n; ++i) {
         set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
         e[i]->n_past_ += n_out[i];
         for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
     }
     if (ms_out) *ms_out = ms;
+    return ErrNone;
+}
+bool Engine::penalty_valid(const PenaltyParams &q, int mirostat, const char *what) {
+    if (mirostat < 0 || mirostat > 2) { MG4_ERR("%s: mirostat %d (0 .. 2)", what, mirostat); return false; }
+    if (q.repeat_last_n < 0) { MG4_ERR("%s: repeat_last_n %d", what, q.repeat_last_n); return false; }
+    if (!std::isfinite(q.repeat_penalty) || q.repeat_penalty <= 0.f) { MG4_ERR("%s: repeat_penalty %g (finite, > 0)", what, q.repeat_penalty); return false; }
+    if (!std::isfinite(q.alpha_presence) || !std::isfinite(q.alpha_frequency)) { MG4_ERR("%s: an alpha is not finite", what); return false; }
+    if (q.penalize_nl != 0 && q.penalize_nl != 1) { MG4_ERR("%s: penalize_nl %d (0 or 1)", what, q.penalize_nl); return false; }
+    return true;
+}
+bool Engine::history_valid(const int32_t *ids, int n, int n_vocab, const char *what) {
+    if (n < 0) { MG4_ERR("%s: a history of %d ids", what, n); return false; }
+    if (n > 0 && !ids) { MG4_ERR("%s: NULL last_ids for a history of %d ids", what, n); return false; }
+    for (int j = 0; j < n; ++j) if (ids[j] < 0 || ids[j] >= n_vocab) { MG4_ERR("%s: history id %d out of range", what, ids[j]); return false; }
+    return true;
+}
+Error Engine::end_chat_penalized(const SamplingParams &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token,
+                                 int32_t *id_out) {
+    if (!token || !penalty_valid(q, p.mirostat, "end_chat_penalized")) return ErrFailedToAddString;
+    const int V = llm_->dims().n_vocab;
+    if (!history_valid(last_ids, n_last, V, "end_chat_penalized")) return ErrFailedToAddString;
+    if (cons_ && (p.mirostat == 1 || p.mirostat == 2)) { MG4_ERR("end_chat_penalized: mirostat on a constrained context"); return ErrFailedToAddString; }
+    int32_t id;
+    if (q.neutral()) id = sample_token(p);   // no logit changes: minigpt4_end_chat itself
+    else {
+        flush();
+        llm_->logits_to_host(logits_.data());
+        const int w = std::min(q.repeat_last_n, n_last);
+        Sampler::penalize(logits_.data(), V, last_ids + (n_last - w), w, q.repeat_penalty, q.alpha_presence, q.alpha_frequency, q.penalize_nl);
+        if (cons_) {   // (as sample_token: the chain over the allowed ids, greedy their first arg-max)
+            const int m = cons_->row_size(cons_state_);
+            const int32_t *row = cons_->row(cons_state_);
+            std::vector<int32_t> ids((size_t)m);
+            for (int j = 0; j < m; ++j) ids[(size_t)j] = row[2 * j];
+            id = sampler_->sample_allowed(logits_.data(), ids.data(), m, p);
+        } else id = sampler_->sample(logits_.data(), V, p);
+    }
+    *token = id_to_token(id);
+    if (id_out) *id_out = id;
+    add_tokens({id});   // (minigpt4_end_chat ignores this return value too)
+    reply_take_id(id);
     return ErrNone;
 }
 Error Engine::beam_search(Engine *const *e, int n, int max_steps, const char *stop, float length_penalty, int n_hyp, int32_t *ids_out,

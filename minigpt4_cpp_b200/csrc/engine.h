@@ -35,8 +35,13 @@ public:
     // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
     // "###"; all or nothing
     // rec (may be null): also each fed id's record (see minigpt4_b200_sample_until_logprobs), with its further refusals
+    // pen (may be null): sample from the penalised logits (see minigpt4_b200_sample_until_penalized), with its further refusals
     static Error sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                              int32_t *stopped, float *ms_out, const LogprobRequest *rec = nullptr);
+                              int32_t *stopped, float *ms_out, const LogprobRequest *rec = nullptr, const PenaltyRequest *pen = nullptr);
+    // minigpt4_end_chat with the context's host sampler over the penalised copy of its logits (see minigpt4_b200_end_chat_penalized)
+    Error end_chat_penalized(const SamplingParams &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token, int32_t *id_out);
+    // the penalty arguments that need no context (mirostat 0..2 too: the penalised calls take all three modes); what: the caller's name
+    static bool penalty_valid(const PenaltyParams &q, int mirostat, const char *what);
     // the n_hyp best replies of e[0]'s conversation by beam search over n (1..16) contexts of its group (see minigpt4_b200_beam_search);
     // all or nothing
     static Error beam_search(Engine *const *e, int n, int max_steps, const char *stop, float length_penalty, int n_hyp, int32_t *ids_out,
@@ -101,6 +106,8 @@ private:
     static bool flush_group(Engine *const *e, int n);
     static bool any_constrained(Engine *const *e, int n);
     static void sample_constraints(Engine *const *e, int n, SampleConstraint *out);   // each context's tables and state for a sampling call
+    // a history of n ids for the penalties: n >= 0, ids non-null if n > 0, every id in 0 .. n_vocab - 1
+    static bool history_valid(const int32_t *ids, int n, int n_vocab, const char *what);
     // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)
     std::shared_ptr<VisionFile> vfile_;
     std::shared_ptr<VisionDevice> vis_;

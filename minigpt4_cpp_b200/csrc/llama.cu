@@ -8,6 +8,7 @@
 #include "llama_state.cuh"
 #include "llama_beam.cuh"
 #include "llama_logprob.cuh"
+#include "llama_penalty.cuh"
 #include "tp.h"
 #include <stdlib.h>
 #include <math.h>
@@ -152,6 +153,27 @@ struct LogprobScratch {
     ~LogprobScratch() {
         if (rec) cudaFree(rec);
         if (h_rec) cudaFreeHost(h_rec);
+    }
+};
+
+// sample_until_penalized's state of one context (llama_penalty.cuh): the penalised row and the window counts (zeroed once; every launch
+// leaves them zero), then the history tail on the device and its pinned staging
+struct PenaltyScratch {
+    float *row = nullptr;
+    int *count = nullptr, *tail = nullptr, *h_tail = nullptr;
+    int cap = 0;
+    size_t bytes = 0;
+    PenaltyScratch(int n_vocab, int n_tail) : cap(n_tail) {
+        bytes = (size_t)LlamaDevice::kPenaltyBytesPerId * n_vocab + 4 * (size_t)cap;
+        CUDA_CHECK(cudaMalloc((void **)&row, bytes));
+        count = (int *)(row + n_vocab);
+        tail = count + n_vocab;
+        CUDA_CHECK(cudaMemset(count, 0, (size_t)n_vocab * 4));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_tail, std::max<size_t>(1, (size_t)cap) * 4, cudaHostAllocDefault));
+    }
+    ~PenaltyScratch() {
+        if (row) cudaFree(row);
+        if (h_tail) cudaFreeHost(h_tail);
     }
 };
 
@@ -325,6 +347,7 @@ LlamaDevice::~LlamaDevice() {
     smp_.reset();
     reply_.reset();
     logprob_.reset();
+    pen_.reset();
 }
 void LlamaDevice::free_weights() {
     for (auto &L : layers_) { qmat_free(L.qkv); qmat_free(L.wq); qmat_free(L.wk); qmat_free(L.wv); qmat_free(L.wo); qmat_free(L.w13); qmat_free(L.w2); cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
@@ -1526,6 +1549,13 @@ void LlamaDevice::ensure_logprob() {
     logprob_.reset(new LogprobScratch(d_.n_ctx));
     owned_bytes_ += logprob_->bytes;
 }
+void LlamaDevice::ensure_penalty(int n_tail) {
+    if (pen_ && pen_->cap >= n_tail) return;
+    if (pen_) owned_bytes_ -= pen_->bytes;   // (a longer history tail than any before: the scratch grows; the last call has synchronised)
+    pen_.reset();
+    pen_.reset(new PenaltyScratch(d_.n_vocab, std::max(d_.n_ctx, n_tail)));
+    owned_bytes_ += pen_->bytes;
+}
 SharedTable::~SharedTable() {
     if (dev) cudaFree(dev);
     if (std::shared_ptr<LlamaGroup> g = group.lock()) g->batch_bytes -= bytes;
@@ -1579,7 +1609,7 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
 
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                                 MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                                const SampleConstraint *cons, const LogprobRequest *rec) {
+                                const SampleConstraint *cons, const LogprobRequest *rec, const PenaltyRequest *pen) {
     LlamaDevice &L0 = *c[0];
     smp::SampleArgsWide a;
     smp::ConsArgsWide k;
@@ -1589,6 +1619,8 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
     smp::StopArgsWide sa{};
     sa.tab = L0.group_->tokens;
     lp::LogprobArgs la{};
+    pen::PenaltyArgs pa{};
+    size_t hist = 0;   // where context i's history starts in pen->last_ids
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         L.ensure_reply();
@@ -1599,8 +1631,23 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
             L.ensure_logprob();
             la.c[i] = lp::LogprobCol{L.logits_, L.state_, L.reply_->r, L.logprob_->rec};
         }
+        if (pen) {   // the history's last repeat_last_n ids go up once; the step's sampling reads the penalised row
+            const int n_last = pen->n_last ? pen->n_last[i] : 0, T = std::min(pen->q.repeat_last_n, n_last);
+            L.ensure_penalty(T);
+            if (T > 0) {
+                memcpy(L.pen_->h_tail, pen->last_ids + hist + (n_last - T), (size_t)T * 4);
+                CUDA_CHECK(cudaMemcpyAsync(L.pen_->tail, L.pen_->h_tail, (size_t)T * 4, cudaMemcpyHostToDevice, s));
+            }
+            hist += (size_t)n_last;
+            pa.c[i] = pen::PenaltyCol{L.logits_, L.pen_->row, L.pen_->count, L.pen_->tail, L.smp_->ids, L.state_, L.reply_->r, T};
+            a.c[i].logits = L.pen_->row;
+        }
     }
     la.n_vocab = L0.d_.n_vocab; la.top_n = rec ? rec->top_n : 0;
+    if (pen) {
+        pa.n_vocab = L0.d_.n_vocab; pa.repeat_last_n = pen->q.repeat_last_n; pa.penalize_nl = pen->q.penalize_nl; pa.greedy = p.temp <= 0.f;
+        pa.repeat_penalty = pen->q.repeat_penalty; pa.alpha_presence = pen->q.alpha_presence; pa.alpha_frequency = pen->q.alpha_frequency;
+    }
     ReplyScratch &R0 = *L0.reply_;
     CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
     int issued = 0;
@@ -1613,6 +1660,11 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         }
         for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
             a.step = issued;
+            if (pen) {   // the rows this step samples from
+                pa.step = issued;
+                pen::penalty_rows_kernel<<<n, pen::kThreads, 0, s>>>(pa);
+                ++L0.launches_;
+            }
             launch_sample_until(a, sa, n, p, m, s, kp);
             if (rec) {   // the logits the step sampled from, before the decode step replaces them
                 la.step = issued;
@@ -1842,6 +1894,52 @@ void LlamaDevice::test_logprobs(const float *logits, int rows, int n_vocab, cons
                                                                                   rec.top_ids ? rec.top_ids + (size_t)r * rec.top_n : nullptr,
                                                                                   rec.top_logprob ? rec.top_logprob + (size_t)r * rec.top_n : nullptr});
     for (void *p : {(void *)lg, (void *)st, (void *)out}) cudaFree(p);
+}
+
+void LlamaDevice::test_penalize(const float *logits, int rows, int n_vocab, const int32_t *last_ids, const int32_t *n_last, const PenaltyParams &q,
+                                float *out, float *kernel_ms) {
+    const size_t V = (size_t)n_vocab;
+    std::vector<int> off((size_t)rows + 1, 0), T((size_t)rows);
+    for (int r = 0; r < rows; ++r) {
+        T[(size_t)r] = std::min(q.repeat_last_n, n_last[r]);
+        off[(size_t)r + 1] = off[(size_t)r] + T[(size_t)r];
+    }
+    std::vector<int> tails((size_t)std::max(1, off[(size_t)rows]));
+    size_t h = 0;
+    for (int r = 0; r < rows; ++r) {
+        std::copy(last_ids + h + (n_last[r] - T[(size_t)r]), last_ids + h + n_last[r], tails.begin() + off[(size_t)r]);
+        h += (size_t)n_last[r];
+    }
+    float *lg = nullptr, *row = nullptr;
+    int *count = nullptr, *tail = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&lg, (size_t)rows * V * 4));
+    CUDA_CHECK(cudaMalloc((void **)&row, (size_t)rows * V * 4));
+    CUDA_CHECK(cudaMalloc((void **)&count, (size_t)rows * V * 4));
+    CUDA_CHECK(cudaMalloc((void **)&tail, tails.size() * 4));
+    CUDA_CHECK(cudaMemcpy(lg, logits, (size_t)rows * V * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(cudaMemset(count, 0, (size_t)rows * V * 4));
+    CUDA_CHECK(cudaMemcpy(tail, tails.data(), tails.size() * 4, cudaMemcpyHostToDevice));
+    pen::PenaltyArgs a{};
+    for (int r = 0; r < rows; ++r)
+        a.c[r] = pen::PenaltyCol{lg + r * V, row + r * V, count + r * V, tail + off[(size_t)r], nullptr, nullptr, nullptr, T[(size_t)r]};
+    a.n_vocab = n_vocab; a.step = 0; a.repeat_last_n = q.repeat_last_n; a.penalize_nl = q.penalize_nl; a.greedy = 0;
+    a.repeat_penalty = q.repeat_penalty; a.alpha_presence = q.alpha_presence; a.alpha_frequency = q.alpha_frequency;
+    pen::penalty_rows_kernel<<<rows, pen::kThreads>>>(a);
+    CUDA_CHECK(cudaGetLastError());
+    if (kernel_ms) {
+        constexpr int kReps = 50;
+        cudaEvent_t e0, e1;
+        CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+        CUDA_CHECK(cudaEventRecord(e0, 0));
+        for (int i = 0; i < kReps; ++i) pen::penalty_rows_kernel<<<rows, pen::kThreads>>>(a);
+        CUDA_CHECK(cudaEventRecord(e1, 0));
+        CUDA_CHECK(cudaEventSynchronize(e1));
+        float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+        *kernel_ms = ms / kReps;
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
+    }
+    CUDA_CHECK(cudaMemcpy(out, row, (size_t)rows * V * 4, cudaMemcpyDeviceToHost));
+    for (void *p : {(void *)lg, (void *)row, (void *)count, (void *)tail}) cudaFree(p);
 }
 
 void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingArgs &p, const uint32_t *rng, int n_draws, int32_t *out, float *kernel_ms,

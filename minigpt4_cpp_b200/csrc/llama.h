@@ -75,6 +75,15 @@ struct SampleConstraint { const int *off = nullptr; const int2 *tr = nullptr; in
 // be null; top_ids null only with top_n 0), laid out as that call states
 struct LogprobRequest { int top_n; float *logprob; int32_t *rank; int32_t *top_ids; float *top_logprob; };
 struct LogprobScratch; // a context's records of sample_until_logprobs and their pinned mirror (llama.cu, llama_logprob.cuh)
+// the penalties of minigpt4_b200_sample_until_penalized / end_chat_penalized (Sampler::penalize); neutral ones change no logit
+struct PenaltyParams {
+    int repeat_last_n; float repeat_penalty, alpha_presence, alpha_frequency; int penalize_nl;
+    bool neutral() const { return repeat_last_n == 0 || (repeat_penalty == 1.0f && alpha_presence == 0.0f && alpha_frequency == 0.0f); }
+};
+// sample_until's penalty request: the parameters and each context's history, context i's n_last[i] ids after those of contexts 0 .. i-1
+// in last_ids (n_last null: no history)
+struct PenaltyRequest { PenaltyParams q; const int32_t *last_ids; const int32_t *n_last; };
+struct PenaltyScratch; // a context's penalised row, window counts and history tail (llama.cu, llama_penalty.cuh)
 struct ScoreCall;      // the outputs of a score_rows call, which eval_rows_batch's passes fill (llama.cu)
 
 class LlamaDevice {
@@ -140,9 +149,19 @@ public:
     // sampling launch and its decode step, and each context's first n_out[i] records come back in one copy at the end, scattered into rec's
     // arrays (entries without a record: -1 / NaN).  A context's first such call allocates its records (kLogprobRecordBytes n_ctx,
     // owned_bytes_).  The caller validates (n_past >= 1: there are logits to report on).
+    // pen (may be null: none, and no extra work is issued): every step first runs penalty_rows_kernel (llama_penalty.cuh), which writes
+    // each context's penalised logits into its own row, and the sampling launch reads that row; the raw logits stay as the decode step
+    // left them.  A context's first such call allocates its row, counts and history tail (kPenaltyBytesPerId n_vocab + 4 n_ctx bytes,
+    // owned_bytes_; a history tail longer than n_ctx ids grows the tail).  The caller validates and passes only non-neutral penalties.
     static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                               MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                              const SampleConstraint *cons = nullptr, const LogprobRequest *rec = nullptr);
+                              const SampleConstraint *cons = nullptr, const LogprobRequest *rec = nullptr, const PenaltyRequest *pen = nullptr);
+    static constexpr int kPenaltyBytesPerId = 8;      // the penalised row (F32) and the window counts (int32), per vocabulary id
+    // test seam: penalty_rows_kernel over `rows` (1..kMaxBatch) host rows of logits, row r's window the last min(repeat_last_n, n_last[r])
+    // of its ids (rows' histories one after another in last_ids) into out [rows][n_vocab]; kernel_ms (may be null): the average
+    // CUDA-event time of one launch.  The caller validates.
+    static void test_penalize(const float *logits, int rows, int n_vocab, const int32_t *last_ids, const int32_t *n_last, const PenaltyParams &q,
+                              float *out, float *kernel_ms);
     static constexpr int kLogprobTop = 20;            // most alternatives a record holds
     static constexpr int kLogprobRecordBytes = 168;   // one step's record: logprob, rank, kLogprobTop ids and log-probabilities
     // test seam: logprob_rows_kernel over `rows` (1..kMaxBatch) host rows of logits, row r as a step that fed ids[r], into rec's arrays
@@ -290,6 +309,8 @@ private:
     void ensure_reply();
     std::unique_ptr<LogprobScratch> logprob_;   // sample_until's records, from the context's first call with a request (owned_bytes_)
     void ensure_logprob();
+    std::unique_ptr<PenaltyScratch> pen_;   // sample_until's penalised row, from the context's first call with penalties (owned_bytes_)
+    void ensure_penalty(int n_tail);        // ... with room for a history tail of n_tail ids
     // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
     // returns the stream the steps run on
     // cons (may be null): each constrained context's state goes to its device copy, and k takes every column's tables

@@ -189,6 +189,22 @@ int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingParams &
     return chain(c, k, sp);
 }
 
+void Sampler::penalize(float *logits, int n_vocab, const int32_t *ids, int n, float repeat_penalty, float alpha_presence, float alpha_frequency,
+                       int penalize_nl) {
+    std::vector<int> count((size_t)n_vocab, 0);
+    for (int j = 0; j < n; ++j) ++count[(size_t)ids[j]];
+    const bool keep_nl = !penalize_nl && n_vocab > 13;
+    for (int j = 0; j < n; ++j) {
+        const int v = ids[j];
+        const int c = count[(size_t)v];
+        if (c == 0 || (keep_nl && v == 13)) continue;   // (an id seen before in the window is done)
+        count[(size_t)v] = 0;
+        const float z = logits[v];
+        const float z1 = repeat_penalty == 1.0f ? z : (z <= 0 ? z * repeat_penalty : z / repeat_penalty);
+        logits[v] = (alpha_frequency == 0 && alpha_presence == 0) ? z1 : z1 - ((float)c * alpha_frequency + alpha_presence);
+    }
+}
+
 int32_t Sampler::chain(std::vector<Candidate> &c, int k, const SamplingParams &sp) {
     bool sorted = false;
     top_k(c, sorted, k, 1);

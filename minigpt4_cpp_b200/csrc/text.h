@@ -34,8 +34,15 @@ class Sampler {
 public:
     explicit Sampler(int seed);
     // Mirrors MiniGPT4::sample_token (reference minigpt4.cpp:2425-2483).  Repeat/presence/frequency penalties
-    // and penalize_nl are accepted by the ABI but never applied by the reference; same here.
+    // and penalize_nl are accepted by the ABI but never applied by the reference; same here (penalize() applies them on request:
+    // minigpt4_b200_end_chat_penalized / sample_until_penalized).
     int32_t sample(const float *logits, int n_vocab, const SamplingParams &p);
+    // llama.cpp's repetition penalty, then its frequency and presence penalties, then main.cpp's penalize_nl, in place over the window
+    // ids[0, n) (the caller's last repeat_last_n ids), as include/minigpt4_b200.h states them: for each id v with c >= 1 copies in the
+    // window, z1 = repeat_penalty == 1 ? z : z <= 0 ? z * repeat_penalty : z / repeat_penalty, then z1 - (c * alpha_frequency +
+    // alpha_presence) unless both alphas are 0; penalize_nl 0 with n_vocab > 13 leaves id 13 as it was.  Every operation rounds to float.
+    static void penalize(float *logits, int n_vocab, const int32_t *ids, int n, float repeat_penalty, float alpha_presence, float alpha_frequency,
+                         int penalize_nl);
     static int32_t greedy(const float *logits, int n_vocab);  // first arg-max
     // sample over the candidates ids[0, n) only (ascending ids: a constraint's allowed ids), in that order: the chain of sample() with
     // top_k <= 0 as n; temp <= 0: the first arg-max among them.  No mirostat.

@@ -236,6 +236,11 @@ _EXT = {
     "minigpt4_b200_sample_until_logprobs": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _I, _F, _F, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP,
                                              C.POINTER(C.c_float)], _I),
     "minigpt4_b200_op_logprobs": ([_VP, _I, _I, _VP, _I, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_sample_until_penalized": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _I, _F, _F, _I, _F, _F, _F, _I, _VP, _VP, _VP, _VP, _VP,
+                                              C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_end_chat_penalized": ([_CTX, C.POINTER(_S), _F, _I, _F, _F, _F, _I, _F, _F, _F, _I, _I, _F, _F, _VP, _I,
+                                          C.POINTER(C.c_int32)], _I),
+    "minigpt4_b200_op_penalize": ([_VP, _I, _I, _VP, _VP, _I, _F, _F, _F, _I, _I, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_constraint_create": ([_CTX, _I, _VP, _VP], _VP),
     "minigpt4_b200_constraint_free": ([_VP], None),
     "minigpt4_b200_constraint_attach": ([_CTX, _VP], _I),
@@ -508,6 +513,60 @@ class B200:
         ms = C.c_float(0)
         self._chk(self.L.minigpt4_b200_op_logprobs(_ptr(lg), rows, V, _ptr(t), top_n, _ptr(lp), _ptr(rk), _ptr(tid), _ptr(tlp), C.byref(ms)))
         return lp, rk, tid[:, :top_n], tlp[:, :top_n], ms.value
+
+    @staticmethod
+    def _histories(last_ids, n: int) -> tuple[np.ndarray, np.ndarray]:
+        """each context's history (a list of id lists, None: none) as minigpt4_b200_*_penalized take them: (ids one after another, counts)"""
+        lists = [[] if x is None else list(x) for x in (last_ids if last_ids is not None else [None] * n)]
+        assert len(lists) == n, "one history per context"
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32).ravel() for x in lists]) if n else np.zeros(0, np.int32), np.int32)
+        return (flat if flat.size else np.zeros(1, np.int32)), np.array([len(x) for x in lists] or [0], np.int32)
+
+    def sample_until_penalized(self, ctxs, max_steps: int, stop: str | bytes | None = None, last_ids=None, repeat_last_n: int = 64,
+                               repeat_penalty: float = 1.1, alpha_presence: float = 0.0, alpha_frequency: float = 0.0, penalize_nl: bool = True,
+                               temp: float = 0.8, top_k: int = 40, top_p: float = 0.9, tfs_z: float = 1.0, typical_p: float = 1.0,
+                               mirostat: int = 0, mirostat_tau: float = 5.0,
+                               mirostat_eta: float = 1.0) -> tuple[list[list[int]], list[bool], float]:
+        """sample_until (mirostat 1 / 2: sample_until_mirostat) that samples every step from the logits after llama.cpp's repetition,
+        frequency and presence penalties over the last repeat_last_n ids of last_ids[i] (context i's history; None: none) and the ids the
+        call has fed.  The defaults are llama.cpp main's.  Returns each context's fed ids, whether the stop text ended it, and the device ms."""
+        n = len(ctxs)
+        ids = np.zeros((max(1, max_steps), max(1, n)), np.int32)
+        n_out, stopped = np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.int32)
+        hist, n_last = self._histories(last_ids, n)
+        ms = C.c_float(0)
+        st = stop.encode() if isinstance(stop, str) else stop
+        self._chk(self.L.minigpt4_b200_sample_until_penalized(C.cast(self._ctx_array(ctxs), C.c_void_p), n, max_steps, st, temp, top_k, top_p,
+                                                              tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta, repeat_last_n, repeat_penalty,
+                                                              alpha_presence, alpha_frequency, int(penalize_nl), _ptr(hist), _ptr(n_last),
+                                                              _ptr(ids), _ptr(n_out), _ptr(stopped), C.byref(ms)))
+        return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
+    def end_chat_penalized(self, ctx, last_ids=None, repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 0.0,
+                           alpha_frequency: float = 0.0, penalize_nl: bool = True, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
+                           tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0,
+                           mirostat_eta: float = 1.0) -> tuple[str, int]:
+        """minigpt4_end_chat with ctx's host sampler over its logits after the penalties of sample_until_penalized, the window being the last
+        repeat_last_n ids of last_ids; returns the fed token's text and id"""
+        hist = np.ascontiguousarray(last_ids if last_ids is not None else [], np.int32)
+        tok, tid = C.c_char_p(), C.c_int32(0)
+        self._chk(self.L.minigpt4_b200_end_chat_penalized(ctx.ptr, C.byref(tok), temp, top_k, top_p, tfs_z, typical_p, repeat_last_n, repeat_penalty,
+                                                          alpha_presence, alpha_frequency, int(penalize_nl), mirostat, mirostat_tau, mirostat_eta,
+                                                          _ptr(hist if hist.size else np.zeros(1, np.int32)), hist.size, C.byref(tid)))
+        return tok.value.decode("utf-8", errors="ignore"), tid.value
+
+    def op_penalize(self, logits: np.ndarray, last_ids=None, repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 0.0,
+                    alpha_frequency: float = 0.0, penalize_nl: bool = True, on_device: bool = True) -> tuple[np.ndarray, float]:
+        """sample_until_penalized's penalised logits over host rows [rows, n_vocab] (rows 1..64), row r's window the last repeat_last_n ids
+        of last_ids[r], through its kernel or (on_device False) the host sampler's penalize: (penalised rows, kernel ms per launch)"""
+        lg = np.ascontiguousarray(logits, np.float32)
+        rows, V = lg.shape
+        hist, n_last = self._histories(last_ids, rows)
+        out = np.zeros_like(lg)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_op_penalize(_ptr(lg), rows, V, _ptr(hist), _ptr(n_last), repeat_last_n, repeat_penalty, alpha_presence,
+                                                   alpha_frequency, int(penalize_nl), int(on_device), _ptr(out), C.byref(ms)))
+        return out, ms.value
 
     def beam_search(self, ctxs, max_steps: int, stop: str | bytes | None = None, length_penalty: float = 1.0,
                     n_hyp: int = 1) -> tuple[list[tuple[list[int], float, float, bool]], float]:
@@ -874,11 +933,17 @@ class MiniGPT4ChatBot:
 
     def generate_on_device(self, message: str, limit: int = 1024, chunk: int = 16, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
                            tfs_z: float = 1.0, typical_p: float = 1.0, mirostat: int = 0, mirostat_tau: float = 5.0, mirostat_eta: float = 1.0,
-                           constraint: Optional[int] = None):
+                           constraint: Optional[int] = None, repeat_last_n: int = 64, repeat_penalty: float = 1.0, alpha_presence: float = 0.0,
+                           alpha_frequency: float = 0.0, penalize_nl: int = 1):
         """generate() with the sampling and the stop check on the GPU: minigpt4_b200_sample_until (mirostat 1 / 2: _mirostat) calls of up
-        to `chunk` steps, each stopping where generate()'s loop stops (the repetition arguments, which generate() passes on unused, are not
-        taken).
+        to `chunk` steps, each stopping where generate()'s loop stops.
         Yields what generate() yields for the same seed: no "##" token, and not the token that completes "###".
+
+        The repetition arguments default to neutral values (repeat_penalty 1.0, alphas 0.0), and then the calls above are issued exactly,
+        as generate() ignores them.  Otherwise every chunk is a minigpt4_b200_sample_until_penalized call whose history is the ids of this
+        reply from the earlier chunks, so the penalties see the last repeat_last_n ids of the reply and a chunked reply equals one call; it
+        yields what a loop of minigpt4_b200_end_chat_penalized over the same history yields (repeat_penalty 1.1 is the reference web UI's
+        slider default, which generate() does not apply).
 
         One difference cannot be avoided: generate() decodes each token's bytes with errors="ignore" before it appends and checks them,
         so a piece that is not valid UTF-8 on its own drops out of its reply text, while the device compares the bytes.  The two can
@@ -887,14 +952,18 @@ class MiniGPT4ChatBot:
         constraint: a handle of B200.constraint_create (or None): the reply is drawn from the ids the automaton allows (no mirostat) and
         also ends after </s>, which is not yielded.  It is attached for this reply only."""
         ext = B200(self.library)
+        pen = None
+        if repeat_last_n != 0 and (repeat_penalty != 1.0 or alpha_presence != 0.0 or alpha_frequency != 0.0):
+            pen = dict(repeat_last_n=repeat_last_n, repeat_penalty=repeat_penalty, alpha_presence=alpha_presence, alpha_frequency=alpha_frequency,
+                       penalize_nl=penalize_nl)
         if constraint is None:
             yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
-                                                mirostat_eta)
+                                                mirostat_eta, pen=pen)
             return
         ext.constraint_attach(self.ctx, constraint)
         try:
             yield from self._generate_on_device(ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
-                                                mirostat_eta)
+                                                mirostat_eta, pen=pen)
         finally:
             ext.constraint_attach(self.ctx, None)
 
@@ -917,8 +986,9 @@ class MiniGPT4ChatBot:
             ext.constraint_attach(self.ctx, None)
 
     def _generate_on_device(self, ext, message, limit, chunk, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta,
-                            top_n=None):
-        """the reply's tokens; with top_n (not None) each as (token, logprob, alternatives)"""
+                            top_n=None, pen=None):
+        """the reply's tokens; with top_n (not None) each as (token, logprob, alternatives); pen (not None): the penalty arguments of
+        sample_until_penalized, the reply's ids so far as the history"""
         if self.is_image_chat:
             self.is_image_chat = False
             self.library.minigpt4_begin_chat_image(self.ctx, self.embedding, message, self.n_threads)
@@ -928,9 +998,15 @@ class MiniGPT4ChatBot:
         def text(t):
             return ext.L.minigpt4_b200_token_text(self.ctx.ptr, int(t)).decode("utf-8", errors="ignore")
         done = 0
+        reply = []
         while done < limit:
             steps = min(chunk, limit - done)
-            if top_n is None:
+            if pen is not None:
+                ids, stopped, _ = ext.sample_until_penalized([self.ctx], steps, None, [reply], temp=temp, top_k=top_k, top_p=top_p, tfs_z=tfs_z,
+                                                             typical_p=typical_p, mirostat=mirostat, mirostat_tau=mirostat_tau,
+                                                             mirostat_eta=mirostat_eta, **pen)
+                reply += ids[0]
+            elif top_n is None:
                 ids, stopped, _ = ext.sample_until([self.ctx], steps, None, temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau,
                                                    mirostat_eta)
             else:
