@@ -166,8 +166,9 @@ MINIGPT4_API int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n
  * (1..max_steps); stopped[i] (may be NULL) = 1 if the stop text ended it, 0 if max_steps did; *ms_out (may be NULL) the CUDA-event time.
  * Afterwards context i is where n_out[i] calls of minigpt4_end_chat (n = 1) or end_chat_batch (n >= 2) with these parameters leave it:
  * n_past, logits, greedy id and generator.  A context that stops early is not changed by the steps the others still run.
- * The host checks the stop flags every 4 steps without stalling the device, so up to 7 steps run past the last stop; their K/V writes
- * lie above each context's final position, where its next token overwrites them.  The first call of a group builds a device table of
+ * The host checks the stop flags every 4 steps without stalling the device, so up to 7 steps run past the last stop; with n = 1 their
+ * K/V writes lie above the context's final position, where its next token overwrites them, and with n >= 2 a stopped context's column
+ * is parked on its last id and position, rewriting the same K/V bits.  The first call of a group builds a device table of
  * every id's text (counted in minigpt4_b200_session_info's shared bytes); each context's first call allocates its stop state and a
  * snapshot of its logits (owned bytes).
  * NULL ctxs / ids_out / n_out, NULL or duplicate contexts, contexts of different groups, n outside 1..64, max_steps < 1, a stop text
@@ -250,6 +251,51 @@ MINIGPT4_API int minigpt4_b200_sample_until_penalized(struct MiniGPT4Context **c
                                                       float mirostat_eta, int32_t repeat_last_n, float repeat_penalty, float alpha_presence,
                                                       float alpha_frequency, int penalize_nl, const int32_t *last_ids, const int32_t *n_last,
                                                       int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out);
+/* Per-conversation settings in one batched reply call (DESIGN.md §4.16): context i of minigpt4_b200_generate_batch runs with params[i].
+ * Layout (80 bytes on LP64; every field at its natural alignment, no padding):
+ *   offset  0 size, 4 max_steps, 8 stop, 16 temp, 20 top_k, 24 top_p, 28 tfs_z, 32 typical_p, 36 mirostat, 40 mirostat_tau,
+ *   44 mirostat_eta, 48 repeat_last_n, 52 repeat_penalty, 56 alpha_presence, 60 alpha_frequency, 64 penalize_nl, 68 n_last, 72 last_ids. */
+struct MiniGPT4B200GenParams {
+    int32_t size;            /* sizeof(struct MiniGPT4B200GenParams); any other value is refused */
+    int32_t max_steps;       /* this context's budget, >= 1; n_past + max_steps <= n_ctx is required of this context only */
+    const char *stop;        /* NULL "###", "" no text stop, at most 32 bytes */
+    float temp;              /* <= 0: greedy */
+    int32_t top_k;           /* mirostat 0: the chain of minigpt4_end_chat */
+    float top_p, tfs_z, typical_p;
+    int32_t mirostat;        /* 0 the chain; 1 / 2 mirostat, which ignores top_k .. typical_p */
+    float mirostat_tau, mirostat_eta;
+    int32_t repeat_last_n;   /* the penalties of minigpt4_b200_sample_until_penalized; neutral ones (repeat_penalty 1 with both alphas 0, */
+    float repeat_penalty;    /* or repeat_last_n 0) cost nothing */
+    float alpha_presence, alpha_frequency;
+    int32_t penalize_nl;
+    int32_t n_last;          /* the penalty history: n_last ids at last_ids (may be 0 / NULL) */
+    const int32_t *last_ids;
+};
+/* One reply call over n (1..64) contexts of one group where every context has its own sampler, penalties, stop text and budget.
+ * Context i ends exactly where it would end if it ran alone (n = 1) with params[i] through the call those settings select:
+ * minigpt4_b200_sample_until (mirostat 0, neutral penalties), sample_until_mirostat (mirostat 1 / 2, neutral penalties),
+ * sample_until_penalized (penalties that are not neutral), or with records sample_until_logprobs: the ids, n_out, stopped, n_past and
+ * K / V rows 0..n_past-1, logits, greedy id, device state, reply tail, generator, mirostat μ and constraint state, bit for bit.  The one
+ * combination no single call has, penalties with records, reports records of the raw logits, as sample_until_logprobs defines them.
+ *   Steps: each step samples in one launch per kind of context present (the chain with greedy and constrained contexts; mirostat), then
+ *   runs one batched decode step for all n.  The call runs at most S = max max_steps steps and ends once every context is done.  A
+ *   context whose reply ended is parked: later steps feed its last id again at that id's own position, which rewrites the same K / V
+ *   bits, so nothing is written beyond its final n_past and a budget that ends at n_ctx is safe while others run on.
+ *   ids_out[s * n + i] (S * n entries) = the id context i was fed at step s, -1 after its last step; n_out[i] its ids (1..max_steps);
+ *   stopped[i] (may be NULL) = 1 if its stop text (or </s> on a constrained context) ended it, 0 if its budget did; *ms_out (may be
+ *   NULL) the CUDA-event time.
+ *   Records: logprob_out NULL means none (top_n must then be 0); otherwise every context gets them, laid out as sample_until_logprobs
+ *   lays them out with max_steps = S, and every context needs n_past >= 1.
+ * Memory: only what the single calls allocate (stop state and snapshot; records; the penalty scratch of a context with penalties that are
+ * not neutral), counted in minigpt4_b200_session_info's owned bytes.
+ * Refusals, each checked per context, return 8 before any device work with nothing changed (queued rows are not evaluated): NULL ctxs /
+ * params / ids_out / n_out, n outside 1..64, NULL, duplicate or tensor-parallel contexts, contexts of different groups, a size other
+ * than sizeof(struct MiniGPT4B200GenParams), max_steps < 1, n_past + max_steps > n_ctx for that context, a stop text over 32 bytes,
+ * mirostat outside 0..2, mirostat on a constrained context, the penalty and history refusals of sample_until_penalized, and with
+ * records top_n outside 0..20, top_n > 0 with NULL top_ids_out or an empty conversation; without records top_n other than 0. */
+MINIGPT4_API int minigpt4_b200_generate_batch(struct MiniGPT4Context **ctxs, int n, const struct MiniGPT4B200GenParams *params, int top_n,
+                                              int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *logprob_out, int32_t *rank_out,
+                                              int32_t *top_ids_out, float *top_logprob_out, float *ms_out);
 /* The host twin of minigpt4_b200_sample_until_penalized: minigpt4_end_chat with the context's own host sampler run on the penalised copy of
  * its logits, the window being the last min(repeat_last_n, n_last) of last_ids (a host loop passes the history and every id it fed
  * since).  *token = the fed id's text, as minigpt4_end_chat returns it; *id_out (may be NULL) = the id.  The reply tail and constraint

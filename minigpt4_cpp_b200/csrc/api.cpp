@@ -3,6 +3,7 @@
 #include "../../include/minigpt4_b200.h"
 #include "engine.h"
 #include "image.h"
+#include <stddef.h>
 #include <string.h>
 #include <sys/stat.h>
 #include <exception>
@@ -273,11 +274,17 @@ int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, 
     if (!ctxs) return ErrFailedToAddString;
     return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out, ms_out);
 }
+// the settings of one context of a uniform reply call: the same for every context (n clamped: Engine::sample_until refuses n outside
+// 1 .. kMaxBatch before it reads them), neutral penalties unless set afterwards
+static std::vector<UntilArgs> uniform_until(int n, int max_steps, const char *stop, const SamplingArgs &p) {
+    const UntilArgs u{p, max_steps, stop ? stop : "###", PenaltyParams{0, 1.f, 0.f, 0.f, 1}, nullptr, 0};   // (NULL stop: the reference's EOS_SUFFIX)
+    return std::vector<UntilArgs>((size_t)std::max(1, std::min(n, LlamaDevice::kMaxBatch)), u);
+}
 int minigpt4_b200_sample_until(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k, float top_p,
                                float tfs_z, float typical_p, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out) {
     if (!ctxs) return ErrFailedToAddString;
-    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p}, ids_out,
-                                n_out, stopped, ms_out);
+    const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, SamplingArgs{temp, top_k, top_p, tfs_z, typical_p});
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out);
 }
 int minigpt4_b200_beam_search(struct MiniGPT4Context **ctxs, int n_beams, int max_steps, const char *stop, float length_penalty, int n_hyp,
                               int32_t *ids_out, int32_t *n_out, float *score_out, float *logprob_out, int32_t *stopped, float *ms_out) {
@@ -300,8 +307,8 @@ int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ctxs, int n, in
 int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int mirostat,
                                         float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out) {
     if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
-    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop,
-                                SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, ids_out, n_out, stopped, ms_out);
+    const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta});
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out);
 }
 int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
                                         float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau, float mirostat_eta, int top_n,
@@ -312,7 +319,8 @@ int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, in
     const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
                                     : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
     const LogprobRequest rec{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out};
-    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, p, ids_out, n_out, stopped, ms_out, &rec);
+    const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, p);
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out, &rec, "sample_until_logprobs");
 }
 int minigpt4_b200_op_logprobs(const float *logits, int rows, int n_vocab, const int32_t *ids, int top_n, float *logprob_out, int32_t *rank_out,
                               int32_t *top_ids_out, float *top_logprob_out, float *kernel_ms) {
@@ -332,8 +340,39 @@ int minigpt4_b200_sample_until_penalized(struct MiniGPT4Context **ctxs, int n, i
     // the sampling arguments of the call this one stands for
     const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
                                     : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
-    const PenaltyRequest pen{PenaltyParams{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl}, last_ids, n_last};
-    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, max_steps, stop, p, ids_out, n_out, stopped, ms_out, nullptr, &pen);
+    std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, p);
+    size_t at = 0;   // context i's history: its n_last[i] ids after those of contexts 0 .. i-1
+    for (int i = 0; i < (int)u.size() && i < n; ++i) {
+        u[(size_t)i].q = PenaltyParams{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl};
+        u[(size_t)i].n_last = n_last ? n_last[i] : 0;
+        u[(size_t)i].last_ids = last_ids ? last_ids + at : nullptr;
+        at += (size_t)std::max(0, u[(size_t)i].n_last);
+    }
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out, nullptr, "sample_until_penalized");
+}
+static_assert(sizeof(MiniGPT4B200GenParams) == 80 && offsetof(MiniGPT4B200GenParams, stop) == 8 && offsetof(MiniGPT4B200GenParams, penalize_nl) == 64 &&
+                  offsetof(MiniGPT4B200GenParams, last_ids) == 72, "the layout include/minigpt4_b200.h states");
+int minigpt4_b200_generate_batch(struct MiniGPT4Context **ctxs, int n, const struct MiniGPT4B200GenParams *params, int top_n, int32_t *ids_out,
+                                 int32_t *n_out, int32_t *stopped, float *logprob_out, int32_t *rank_out, int32_t *top_ids_out, float *top_logprob_out,
+                                 float *ms_out) {
+    if (!ctxs || !params) { MG4_ERR("generate_batch: NULL contexts or params"); return ErrFailedToAddString; }
+    if (n < 1 || n > LlamaDevice::kMaxBatch) { MG4_ERR("generate_batch: %d contexts (1 .. %d)", n, LlamaDevice::kMaxBatch); return ErrFailedToAddString; }
+    if (!logprob_out && top_n != 0) { MG4_ERR("generate_batch: top_n %d without records", top_n); return ErrFailedToAddString; }
+    std::vector<UntilArgs> u((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const MiniGPT4B200GenParams &g = params[i];
+        if (g.size != (int32_t)sizeof(MiniGPT4B200GenParams)) {
+            MG4_ERR("generate_batch: params[%d].size %d (%zu)", i, g.size, sizeof(MiniGPT4B200GenParams)); return ErrFailedToAddString;
+        }
+        // mirostat 1 / 2 ignores top_k .. typical_p, as sample_until_mirostat does
+        const SamplingArgs p = g.mirostat ? SamplingArgs{g.temp, 0, 1.f, 1.f, 1.f, g.mirostat, g.mirostat_tau, g.mirostat_eta}
+                                          : SamplingArgs{g.temp, g.top_k, g.top_p, g.tfs_z, g.typical_p};
+        u[(size_t)i] = UntilArgs{p, g.max_steps, g.stop ? g.stop : "###",
+                                 PenaltyParams{g.repeat_last_n, g.repeat_penalty, g.alpha_presence, g.alpha_frequency, g.penalize_nl}, g.last_ids, g.n_last};
+    }
+    const LogprobRequest rec{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out};
+    return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out, logprob_out ? &rec : nullptr,
+                                "generate_batch");
 }
 int minigpt4_b200_end_chat_penalized(struct MiniGPT4Context *ctx, const char **token, float temp, int32_t top_k, float top_p, float tfs_z,
                                      float typical_p, int32_t repeat_last_n, float repeat_penalty, float alpha_presence, float alpha_frequency,

@@ -185,36 +185,28 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
     if (ms_out) *ms_out = ms;
     return ErrNone;
 }
-Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                           int32_t *stopped, float *ms_out, const LogprobRequest *rec, const PenaltyRequest *pen) {
+Error Engine::sample_until(Engine *const *e, int n, const UntilArgs *u, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out,
+                           const LogprobRequest *rec, const char *what) {
     if (rec) {   // (arguments first: none of these reads a context)
-        if (!rec->logprob) { MG4_ERR("sample_until_logprobs: NULL logprob_out"); return ErrFailedToAddString; }
-        if (rec->top_n < 0 || rec->top_n > LlamaDevice::kLogprobTop) { MG4_ERR("sample_until_logprobs: top_n %d (0 .. %d)", rec->top_n, LlamaDevice::kLogprobTop); return ErrFailedToAddString; }
-        if (rec->top_n > 0 && !rec->top_ids) { MG4_ERR("sample_until_logprobs: NULL top_ids_out with top_n %d", rec->top_n); return ErrFailedToAddString; }
-        if (p.mirostat < 0 || p.mirostat > 2) { MG4_ERR("sample_until_logprobs: mirostat %d (0 .. 2)", p.mirostat); return ErrFailedToAddString; }
+        if (!rec->logprob) { MG4_ERR("%s: NULL logprob_out", what); return ErrFailedToAddString; }
+        if (rec->top_n < 0 || rec->top_n > LlamaDevice::kLogprobTop) { MG4_ERR("%s: top_n %d (0 .. %d)", what, rec->top_n, LlamaDevice::kLogprobTop); return ErrFailedToAddString; }
+        if (rec->top_n > 0 && !rec->top_ids) { MG4_ERR("%s: NULL top_ids_out with top_n %d", what, rec->top_n); return ErrFailedToAddString; }
     }
-    if (pen && !penalty_valid(pen->q, p.mirostat, "sample_until_penalized")) return ErrFailedToAddString;
-    if (!ids_out || !n_out || !group_valid(e, n, "sample_until")) return ErrFailedToAddString;
-    for (int i = 0; rec && i < n; ++i)
-        if (e[i]->n_past_ == 0) { MG4_ERR("sample_until_logprobs: context %d: the conversation is empty", i); return ErrFailedToAddString; }
-    if (pen) {
-        const int n_vocab = e[0]->llm_->dims().n_vocab;
-        size_t at = 0;
-        for (int i = 0; i < n; ++i) {
-            const int n_last = pen->n_last ? pen->n_last[i] : 0;
-            if (!history_valid(pen->last_ids ? pen->last_ids + at : nullptr, n_last, n_vocab, "sample_until_penalized")) return ErrFailedToAddString;
-            at += (size_t)std::max(0, n_last);
+    if (!u) { MG4_ERR("%s: NULL params", what); return ErrFailedToAddString; }
+    if (!ids_out || !n_out || !group_valid(e, n, what)) return ErrFailedToAddString;
+    const int n_vocab = e[0]->llm_->dims().n_vocab;
+    for (int i = 0; i < n; ++i) {   // each context's own settings, as the single calls check them
+        const UntilArgs &g = u[i];
+        if (e[i]->tp.world > 1) { MG4_ERR("%s: context %d is tensor-parallel", what, i); return ErrFailedToAddString; }
+        if (g.max_steps < 1) { MG4_ERR("%s: context %d: %d steps", what, i, g.max_steps); return ErrFailedToAddString; }
+        if (g.stop.size() > (size_t)LlamaDevice::kStopMax) {
+            MG4_ERR("%s: context %d: stop text of %zu bytes (at most %d)", what, i, g.stop.size(), LlamaDevice::kStopMax); return ErrFailedToAddString;
         }
-        if (pen->q.neutral()) pen = nullptr;   // no logit changes: exactly sample_until's work
-    }
-    if (max_steps < 1) { MG4_ERR("sample_until: %d steps", max_steps); return ErrFailedToAddString; }
-    const std::string st = stop ? stop : "###";   // the reference's EOS_SUFFIX
-    if (st.size() > (size_t)LlamaDevice::kStopMax) { MG4_ERR("sample_until: stop text of %zu bytes (at most %d)", st.size(), LlamaDevice::kStopMax); return ErrFailedToAddString; }
-    if (p.mirostat && any_constrained(e, n)) { MG4_ERR("sample_until: mirostat on a constrained context"); return ErrFailedToAddString; }
-    for (int i = 0; i < n; ++i) {
-        if (e[i]->tp.world > 1) { MG4_ERR("sample_until: context %d is tensor-parallel", i); return ErrFailedToAddString; }
+        if (!penalty_valid(g.q, g.p.mirostat, what) || !history_valid(g.last_ids, g.n_last, n_vocab, what)) return ErrFailedToAddString;
+        if (g.p.mirostat && e[i]->cons_) { MG4_ERR("%s: mirostat on constrained context %d", what, i); return ErrFailedToAddString; }
+        if (rec && e[i]->n_past_ == 0) { MG4_ERR("%s: context %d: the conversation is empty", what, i); return ErrFailedToAddString; }
         const int n_ctx = e[i]->llm_->dims().n_ctx;
-        if (e[i]->n_past_ + max_steps > n_ctx) { MG4_ERR("sample_until: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, max_steps, n_ctx); return ErrFailedToAddString; }
+        if (e[i]->n_past_ + g.max_steps > n_ctx) { MG4_ERR("%s: context %d: %d + %d > n_ctx %d", what, i, e[i]->n_past_, g.max_steps, n_ctx); return ErrFailedToAddString; }
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
     e[0]->ensure_token_table();
@@ -224,9 +216,9 @@ Error Engine::sample_until(Engine *const *e, int n, int max_steps, const char *s
     for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
     SampleConstraint cons[LlamaDevice::kMaxBatch];
     sample_constraints(e, n, cons);
-    const float ms = LlamaDevice::sample_until(L, n, max_steps, np, p, rng, mu, st, tail, ids_out, n_out, stopped, cons, rec, pen);
+    const float ms = LlamaDevice::sample_until(L, n, u, np, rng, mu, tail, ids_out, n_out, stopped, cons, rec);
     for (int i = 0; i < n; ++i) {
-        set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
+        set_sampler_state(*e[i]->sampler_, u[i].p, rng[i], mu[i]);
         e[i]->n_past_ += n_out[i];
         for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
     }

@@ -32,12 +32,13 @@ public:
     // `steps` decode steps of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
     // own generator and mirostat μ (see minigpt4_b200_sample_steps / _mirostat); ids_out[s * n + i]; all or nothing
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
-    // sample_steps that stops each context where the reference's chat loop stops its reply (see minigpt4_b200_sample_until); stop NULL:
-    // "###"; all or nothing
+    // sample_steps that stops each context where the reference's chat loop stops its reply, each with its own settings u[i]: sampling
+    // arguments, budget, stop text and penalties (see minigpt4_b200_generate_batch; the uniform calls minigpt4_b200_sample_until,
+    // _mirostat, _penalized and _logprobs pass the same settings for every context); ids_out[s * n + i], s < max u[i].max_steps.  All or
+    // nothing: every context's settings are checked before any device work.  what: the caller's name in the messages
     // rec (may be null): also each fed id's record (see minigpt4_b200_sample_until_logprobs), with its further refusals
-    // pen (may be null): sample from the penalised logits (see minigpt4_b200_sample_until_penalized), with its further refusals
-    static Error sample_until(Engine *const *e, int n, int max_steps, const char *stop, const SamplingArgs &p, int32_t *ids_out, int32_t *n_out,
-                              int32_t *stopped, float *ms_out, const LogprobRequest *rec = nullptr, const PenaltyRequest *pen = nullptr);
+    static Error sample_until(Engine *const *e, int n, const UntilArgs *u, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out,
+                              const LogprobRequest *rec = nullptr, const char *what = "sample_until");
     // minigpt4_end_chat with the context's host sampler over the penalised copy of its logits (see minigpt4_b200_end_chat_penalized)
     Error end_chat_penalized(const SamplingParams &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token, int32_t *id_out);
     // the penalty arguments that need no context (mirostat 0..2 too: the penalised calls take all three modes); what: the caller's name

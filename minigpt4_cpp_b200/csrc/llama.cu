@@ -120,16 +120,16 @@ struct SamplerScratch {
 // sample_until's per-context state (llama_sample.cuh): the ReplyState and the logits snapshot on the device, a pinned mirror of the
 // ReplyState, and the done flags and chunk events of the calls this context leads (its column 0)
 struct ReplyScratch {
-    smp::ReplyState *r = nullptr, *h_r = nullptr;
+    smp::UntilState *r = nullptr, *h_r = nullptr;
     float *snap = nullptr;
     int *h_done = nullptr;   // [2][kMaxBatch] pinned: the done flags after the last two chunks issued
     cudaEvent_t ev[2] = {};
     size_t bytes = 0;
     explicit ReplyScratch(int n_vocab) {
-        bytes = sizeof(smp::ReplyState) + (size_t)n_vocab * 4;
+        bytes = sizeof(smp::UntilState) + (size_t)n_vocab * 4;
         CUDA_CHECK(cudaMalloc((void **)&r, bytes));
         snap = (float *)(r + 1);
-        CUDA_CHECK(cudaHostAlloc((void **)&h_r, sizeof(smp::ReplyState), cudaHostAllocDefault));
+        CUDA_CHECK(cudaHostAlloc((void **)&h_r, sizeof(smp::UntilState), cudaHostAllocDefault));
         CUDA_CHECK(cudaHostAlloc((void **)&h_done, 2 * kMaxBatch * sizeof(int), cudaHostAllocDefault));
         for (cudaEvent_t &e : ev) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
@@ -1380,21 +1380,11 @@ void LlamaDevice::ensure_sampler() {
     owned_bytes_ += smp_->bytes;
 }
 
-static smp::SampleArgsWide sample_args(const SamplingArgs &p, int n_vocab) {
-    smp::SampleArgsWide a{};
-    a.n_vocab = n_vocab; a.top_k = p.top_k; a.temp = p.temp; a.top_p = p.top_p; a.tfs_z = p.tfs_z; a.typical_p = p.typical_p;
-    return a;
-}
-static smp::MirostatArgs mirostat_args(const SamplingArgs &p) {
-    smp::MirostatArgs m{};
-    m.mode = p.mirostat; m.tau = p.mirostat_tau; m.eta = p.mirostat_eta;
-    return m;
-}
 // a launch of at most 8 contexts takes the 8-column tables: the first 8 columns of the wide ones
 static smp::SampleArgs narrow(const smp::SampleArgsWide &w) {
     smp::SampleArgs a{};
     memcpy(a.c, w.c, sizeof(a.c));
-    a.n_vocab = w.n_vocab; a.step = w.step; a.top_k = w.top_k; a.temp = w.temp; a.top_p = w.top_p; a.tfs_z = w.tfs_z; a.typical_p = w.typical_p;
+    a.n_vocab = w.n_vocab; a.step = w.step;
     return a;
 }
 static smp::StopArgs narrow(const smp::StopArgsWide &w) {
@@ -1402,10 +1392,10 @@ static smp::StopArgs narrow(const smp::StopArgsWide &w) {
     memcpy(s.r, w.r, sizeof(s.r)); memcpy(s.snap, w.snap, sizeof(s.snap)); s.tab = w.tab;
     return s;
 }
-// one sampling step of n contexts in one launch (grid n): the 8-column kernels up to 8 contexts, the wide ones above
+// one sampling step of n contexts in one launch (grid n): the 8-column kernels up to 8 contexts, the wide ones above; mirostat: the
+// mirostat kernels (every column's c.args.mirostat is 1 or 2)
 // k (may be null): the constrained twins, which take every column's constraint table
-static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArgs &p, const smp::MirostatArgs &m, cudaStream_t s,
-                          const smp::ConsArgsWide *k = nullptr) {
+static void launch_sample(const smp::SampleArgsWide &a, int n, bool mirostat, cudaStream_t s, const smp::ConsArgsWide *k = nullptr) {
     if (k) {
         if (n <= 8) {
             smp::ConsArgs k8{};
@@ -1416,13 +1406,13 @@ static void launch_sample(const smp::SampleArgsWide &a, int n, const SamplingArg
     }
     if (n <= 8) {
         const smp::SampleArgs a8 = narrow(a);
-        if (p.mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, m);
+        if (mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8);
         else smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a8);
-    } else if (p.mirostat) smp::sample_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, m);
+    } else if (mirostat) smp::sample_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
     else smp::sample_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
 }
-static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArgsWide &sa, int n, const SamplingArgs &p, const smp::MirostatArgs &m,
-                                cudaStream_t s, const smp::ConsArgsWide *k = nullptr) {
+static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArgsWide &sa, int n, bool mirostat, cudaStream_t s,
+                                const smp::ConsArgsWide *k = nullptr) {
     if (k) {
         if (n <= 8) {
             smp::ConsArgs k8{};
@@ -1434,18 +1424,19 @@ static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArg
     if (n <= 8) {
         const smp::SampleArgs a8 = narrow(a);
         const smp::StopArgs s8 = narrow(sa);
-        if (p.mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8, m);
+        if (mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8);
         else smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8);
-    } else if (p.mirostat) smp::sample_until_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, m);
+    } else if (mirostat) smp::sample_until_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
     else smp::sample_until_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
 }
 // the bytes of a context's sampler state that a call moves: the generator, and μ after it with mirostat
 static size_t sampler_state_bytes(const SamplingArgs &p) { return 625 * 4 + (p.mirostat ? sizeof(MirostatState) : 0); }
 
-cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
+cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu,
                                          smp::SampleArgsWide &a, const SampleConstraint *cons, smp::ConsArgsWide *k) {
     LlamaDevice &L0 = *c[0];
-    a = sample_args(p, L0.d_.n_vocab);
+    a = smp::SampleArgsWide{};
+    a.n_vocab = L0.d_.n_vocab;
     cudaStream_t s = L0.stream_;
     if (n >= 2) {   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
         for (int i = 0; i < n; ++i) c[i]->sync();
@@ -1459,13 +1450,14 @@ cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int
         L.ensure_sampler();
         SessionSlot *slot = n >= 2 ? L0.group_->slots + i : nullptr;
         a.c[i] = L.smp_->ctx(L.logits_, L.state_, slot, n_past[i]);
-        if (p.temp > 0.f) {
+        a.c[i].args = p[i];
+        if (p[i].temp > 0.f) {
             memcpy(L.smp_->h_rng, rng[i], 625 * 4);
-            if (p.mirostat) *L.smp_->h_mu = mu[i];
-            CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, sampler_state_bytes(p), cudaMemcpyHostToDevice, s));
+            if (p[i].mirostat) *L.smp_->h_mu = mu[i];
+            CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, sampler_state_bytes(p[i]), cudaMemcpyHostToDevice, s));
         }
         if (k) k->c[i] = smp::ConsCol{nullptr, nullptr, nullptr};
-        if (k && cons[i].off) {
+        if (k && cons && cons[i].off) {
             *L.smp_->h_cons = cons[i].state;
             CUDA_CHECK(cudaMemcpyAsync(L.smp_->cons, L.smp_->h_cons, sizeof(int), cudaMemcpyHostToDevice, s));
             k->c[i] = smp::ConsCol{cons[i].off, cons[i].tr, L.smp_->cons};
@@ -1493,15 +1485,14 @@ void LlamaDevice::sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaS
 }
 
 // after `steps` steps: the fed ids, generators and μ to the host, one synchronisation; returns the device ms since ev0_
-float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
+float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
                                 cudaStream_t s) {
     LlamaDevice &L0 = *c[0];
-    const bool sampled = p.temp > 0.f;
     CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_ids, L.smp_->ids, (size_t)steps * 4, cudaMemcpyDeviceToHost, s));
-        if (sampled) CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_rng, L.smp_->mt, sampler_state_bytes(p), cudaMemcpyDeviceToHost, s));
+        if (p[i].temp > 0.f) CUDA_CHECK(cudaMemcpyAsync(L.smp_->h_rng, L.smp_->mt, sampler_state_bytes(p[i]), cudaMemcpyDeviceToHost, s));
     }
     if (n == 1) L0.sync_decode();
     else {
@@ -1511,9 +1502,10 @@ float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const S
     float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, L0.ev0_, L0.ev1_));
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
+        const bool sampled = p[i].temp > 0.f;
         for (int t = 0; t < steps; ++t) ids_out[(size_t)t * n + i] = L.smp_->h_ids[t];
         if (sampled) memcpy(rng[i], L.smp_->h_rng, 625 * 4);
-        if (sampled && p.mirostat) mu[i] = *L.smp_->h_mu;
+        if (sampled && p[i].mirostat) mu[i] = *L.smp_->h_mu;
     }
     return ms;
 }
@@ -1528,15 +1520,16 @@ float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const i
     smp::SampleArgsWide a;
     smp::ConsArgsWide k;
     const smp::ConsArgsWide *kp = any_constrained(cons, n) ? &k : nullptr;
-    const smp::MirostatArgs m = mirostat_args(p);
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, kp ? &k : nullptr);
+    SamplingArgs ps[kMaxBatch];
+    std::fill(ps, ps + n, p);
+    cudaStream_t s = begin_sampling(c, n, n_past, ps, rng, mu, a, cons, kp ? &k : nullptr);
     CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
     for (int t = 0; t < steps; ++t) {
         a.step = t;
-        launch_sample(a, n, p, m, s, kp);
+        launch_sample(a, n, p.mirostat != 0, s, kp);
         sampled_decode(c, n, n_past[0] + t, s);
     }
-    return end_sampling(c, n, steps, p, rng, mu, ids_out, s);
+    return end_sampling(c, n, steps, ps, rng, mu, ids_out, s);
 }
 
 void LlamaDevice::ensure_reply() {
@@ -1607,65 +1600,87 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
     r.stop_len = (int)stop.size();
 }
 
-float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                                MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                                const SampleConstraint *cons, const LogprobRequest *rec, const PenaltyRequest *pen) {
+// the columns of one kind in a step's sampling launch (the chain with greedy and constrained columns, or mirostat), in slot order: each
+// column's SampleCtx carries its slot, and its StopArgs / ConsArgs entries follow it
+struct UntilLaunch {
+    smp::SampleArgsWide a{};
+    smp::StopArgsWide s{};
+    smp::ConsArgsWide k{};
+    int n = 0;
+    bool cons = false;
+};
+
+float LlamaDevice::sample_until(LlamaDevice *const *c, int n, const UntilArgs *u, const int *n_past, uint32_t (*rng)[625], MirostatState *mu,
+                                const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped, const SampleConstraint *cons,
+                                const LogprobRequest *rec) {
     LlamaDevice &L0 = *c[0];
+    SamplingArgs p[kMaxBatch];
+    int S = 0;   // the longest budget: the most steps the call runs
+    for (int i = 0; i < n; ++i) { p[i] = u[i].p; S = std::max(S, u[i].max_steps); }
     smp::SampleArgsWide a;
     smp::ConsArgsWide k;
-    const smp::ConsArgsWide *kp = any_constrained(cons, n) ? &k : nullptr;
-    const smp::MirostatArgs m = mirostat_args(p);
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, kp ? &k : nullptr);
+    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, &k);
     smp::StopArgsWide sa{};
     sa.tab = L0.group_->tokens;
     lp::LogprobArgs la{};
     pen::PenaltyArgs pa{};
-    size_t hist = 0;   // where context i's history starts in pen->last_ids
+    int n_pen = 0;
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         L.ensure_reply();
-        reply_init(*L.reply_->h_r, stop, tail[i]);
-        CUDA_CHECK(cudaMemcpyAsync(L.reply_->r, L.reply_->h_r, sizeof(smp::ReplyState), cudaMemcpyHostToDevice, s));
+        reply_init(*L.reply_->h_r, u[i].stop, tail[i]);
+        L.reply_->h_r->budget = u[i].max_steps;
+        L.reply_->h_r->by_budget = 0;
+        CUDA_CHECK(cudaMemcpyAsync(L.reply_->r, L.reply_->h_r, sizeof(smp::UntilState), cudaMemcpyHostToDevice, s));
         sa.r[i] = L.reply_->r; sa.snap[i] = L.reply_->snap;
         if (rec) {
             L.ensure_logprob();
             la.c[i] = lp::LogprobCol{L.logits_, L.state_, L.reply_->r, L.logprob_->rec};
         }
-        if (pen) {   // the history's last repeat_last_n ids go up once; the step's sampling reads the penalised row
-            const int n_last = pen->n_last ? pen->n_last[i] : 0, T = std::min(pen->q.repeat_last_n, n_last);
+        if (!u[i].q.neutral()) {   // the history's last repeat_last_n ids go up once; the step's sampling reads the penalised row
+            const int n_last = u[i].last_ids ? u[i].n_last : 0, T = std::min(u[i].q.repeat_last_n, n_last);
             L.ensure_penalty(T);
             if (T > 0) {
-                memcpy(L.pen_->h_tail, pen->last_ids + hist + (n_last - T), (size_t)T * 4);
+                memcpy(L.pen_->h_tail, u[i].last_ids + (n_last - T), (size_t)T * 4);
                 CUDA_CHECK(cudaMemcpyAsync(L.pen_->tail, L.pen_->h_tail, (size_t)T * 4, cudaMemcpyHostToDevice, s));
             }
-            hist += (size_t)n_last;
-            pa.c[i] = pen::PenaltyCol{L.logits_, L.pen_->row, L.pen_->count, L.pen_->tail, L.smp_->ids, L.state_, L.reply_->r, T};
+            pa.c[n_pen++] = pen::PenaltyCol{L.logits_, L.pen_->row, L.pen_->count, L.pen_->tail, L.smp_->ids, L.state_, L.reply_->r, T, u[i].q,
+                                            p[i].temp <= 0.f ? 1 : 0};
             a.c[i].logits = L.pen_->row;
         }
     }
     la.n_vocab = L0.d_.n_vocab; la.top_n = rec ? rec->top_n : 0;
-    if (pen) {
-        pa.n_vocab = L0.d_.n_vocab; pa.repeat_last_n = pen->q.repeat_last_n; pa.penalize_nl = pen->q.penalize_nl; pa.greedy = p.temp <= 0.f;
-        pa.repeat_penalty = pen->q.repeat_penalty; pa.alpha_presence = pen->q.alpha_presence; pa.alpha_frequency = pen->q.alpha_frequency;
+    pa.n_vocab = L0.d_.n_vocab;
+    UntilLaunch kind[2];   // [0] the chain, greedy and constrained columns; [1] mirostat
+    for (int i = 0; i < n; ++i) {
+        UntilLaunch &K = kind[p[i].mirostat ? 1 : 0];
+        K.a.c[K.n] = a.c[i]; K.s.r[K.n] = sa.r[i]; K.s.snap[K.n] = sa.snap[i]; K.k.c[K.n] = k.c[i];
+        K.cons = K.cons || (cons && cons[i].off);
+        ++K.n;
     }
+    for (UntilLaunch &K : kind) { K.a.n_vocab = a.n_vocab; K.s.tab = sa.tab; }
     ReplyScratch &R0 = *L0.reply_;
     CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
     int issued = 0;
-    for (int j = 0; issued < max_steps; ++j) {
+    for (int j = 0; issued < S; ++j) {
         if (j >= 2) {   // chunk j - 2's flags; chunk j - 1 keeps the device busy meanwhile
             CUDA_CHECK(cudaEventSynchronize(R0.ev[j % 2]));
             bool all = true;
             for (int i = 0; i < n; ++i) all = all && R0.h_done[(j % 2) * kMaxBatch + i] != 0;
             if (all) break;
         }
-        for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
-            a.step = issued;
-            if (pen) {   // the rows this step samples from
+        for (const int end = std::min(S, issued + kReplyChunk); issued < end; ++issued) {
+            if (n_pen) {   // the rows this step samples from
                 pa.step = issued;
-                pen::penalty_rows_kernel<<<n, pen::kThreads, 0, s>>>(pa);
+                pen::penalty_rows_kernel<<<n_pen, pen::kThreads, 0, s>>>(pa);
                 ++L0.launches_;
             }
-            launch_sample_until(a, sa, n, p, m, s, kp);
+            for (int m = 0; m < 2; ++m) {
+                UntilLaunch &K = kind[m];
+                if (!K.n) continue;
+                K.a.step = issued;
+                launch_sample_until(K.a, K.s, K.n, m == 1, s, K.cons ? &K.k : nullptr);
+            }
             if (rec) {   // the logits the step sampled from, before the decode step replaces them
                 la.step = issued;
                 lp::logprob_rows_kernel<<<n, lp::kThreads, 0, s>>>(la);
@@ -1678,14 +1693,14 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
         CUDA_CHECK(cudaEventRecord(R0.ev[j % 2], s));
     }
     for (int i = 0; i < n; ++i)
-        CUDA_CHECK(cudaMemcpyAsync(c[i]->reply_->h_r, c[i]->reply_->r, sizeof(smp::ReplyState), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaMemcpyAsync(c[i]->reply_->h_r, c[i]->reply_->r, sizeof(smp::UntilState), cudaMemcpyDeviceToHost, s));
     const float ms = end_sampling(c, n, issued, p, rng, mu, ids_out, s);
     // a context that stopped before the last issued step gets back what its stopping step left
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
-        const smp::ReplyState &r = *L.reply_->h_r;
+        const smp::UntilState &r = *L.reply_->h_r;
         n_out[i] = r.n_fed;
-        if (stopped) stopped[i] = r.done != 0 ? 1 : 0;
+        if (stopped) stopped[i] = r.done != 0 && !r.by_budget ? 1 : 0;
         for (int t = r.n_fed; t < issued; ++t) ids_out[(size_t)t * n + i] = -1;
         if (r.done == 2) {
             CUDA_CHECK(cudaMemcpyAsync(L.logits_, L.reply_->snap, (size_t)L.d_.n_vocab * 4, cudaMemcpyDeviceToDevice, s));
@@ -1696,10 +1711,10 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, int max_steps, con
             CUDA_CHECK(cudaMemcpyAsync(L.logprob_->h_rec, L.logprob_->rec, (size_t)r.n_fed * sizeof(lp::Record), cudaMemcpyDeviceToHost, s));
     }
     CUDA_CHECK(cudaStreamSynchronize(s));
-    for (int t = issued; t < max_steps; ++t)
+    for (int t = issued; t < S; ++t)
         for (int i = 0; i < n; ++i) ids_out[(size_t)t * n + i] = -1;
     if (rec)
-        for (int i = 0; i < n; ++i) scatter_records(c[i]->logprob_->h_rec, n_out[i], i, n, max_steps, *rec);
+        for (int i = 0; i < n; ++i) scatter_records(c[i]->logprob_->h_rec, n_out[i], i, n, S, *rec);
     return ms;
 }
 
@@ -1921,9 +1936,8 @@ void LlamaDevice::test_penalize(const float *logits, int rows, int n_vocab, cons
     CUDA_CHECK(cudaMemcpy(tail, tails.data(), tails.size() * 4, cudaMemcpyHostToDevice));
     pen::PenaltyArgs a{};
     for (int r = 0; r < rows; ++r)
-        a.c[r] = pen::PenaltyCol{lg + r * V, row + r * V, count + r * V, tail + off[(size_t)r], nullptr, nullptr, nullptr, T[(size_t)r]};
-    a.n_vocab = n_vocab; a.step = 0; a.repeat_last_n = q.repeat_last_n; a.penalize_nl = q.penalize_nl; a.greedy = 0;
-    a.repeat_penalty = q.repeat_penalty; a.alpha_presence = q.alpha_presence; a.alpha_frequency = q.alpha_frequency;
+        a.c[r] = pen::PenaltyCol{lg + r * V, row + r * V, count + r * V, tail + off[(size_t)r], nullptr, nullptr, nullptr, T[(size_t)r], q, 0};
+    a.n_vocab = n_vocab; a.step = 0;
     pen::penalty_rows_kernel<<<rows, pen::kThreads>>>(a);
     CUDA_CHECK(cudaGetLastError());
     if (kernel_ms) {
@@ -1952,15 +1966,16 @@ void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingAr
     CUDA_CHECK(cudaMemcpy(ss.mt, rng, 625 * 4, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemset(ss.mu, 0, sizeof(MirostatState)));
     if (mu_out && p.mirostat) CUDA_CHECK(cudaMalloc((void **)&mu_d, (size_t)n_draws * 4));
-    smp::SampleArgsWide a = sample_args(p, n_vocab);
+    smp::SampleArgsWide a{};
+    a.n_vocab = n_vocab;
     a.c[0] = ss.ctx(lg, st, nullptr, 0);
-    const smp::MirostatArgs m = mirostat_args(p);
+    a.c[0].args = p;
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     CUDA_CHECK(cudaEventRecord(e0, 0));
     for (int i = 0; i < n_draws; ++i) {
         a.step = i;
-        launch_sample(a, 1, p, m, 0);
+        launch_sample(a, 1, p.mirostat != 0, 0);
         CUDA_CHECK(cudaGetLastError());
         if (mu_d) CUDA_CHECK(cudaMemcpyAsync(mu_d + i, &ss.mu->mu[p.mirostat - 1], 4, cudaMemcpyDeviceToDevice, 0));
     }

@@ -80,9 +80,16 @@ struct PenaltyParams {
     int repeat_last_n; float repeat_penalty, alpha_presence, alpha_frequency; int penalize_nl;
     bool neutral() const { return repeat_last_n == 0 || (repeat_penalty == 1.0f && alpha_presence == 0.0f && alpha_frequency == 0.0f); }
 };
-// sample_until's penalty request: the parameters and each context's history, context i's n_last[i] ids after those of contexts 0 .. i-1
-// in last_ids (n_last null: no history)
-struct PenaltyRequest { PenaltyParams q; const int32_t *last_ids; const int32_t *n_last; };
+// one context's settings in sample_until: its sampling arguments, its budget (max_steps >= 1), its stop text (0..kStopMax bytes, "" no text
+// stop), and its penalties with its history (n_last ids at last_ids; may be null / 0).  Neutral penalties issue no penalty work.
+struct UntilArgs {
+    SamplingArgs p;
+    int max_steps;
+    std::string stop;
+    PenaltyParams q;
+    const int32_t *last_ids;
+    int n_last;
+};
 struct PenaltyScratch; // a context's penalised row, window counts and history tail (llama.cu, llama_penalty.cuh)
 struct ScoreCall;      // the outputs of a score_rows call, which eval_rows_batch's passes fill (llama.cu)
 
@@ -136,12 +143,15 @@ public:
     // cons (may be null: none): context i samples over its constraint's allowed ids when cons[i].off is set (no mirostat then).
     static float sample_steps(LlamaDevice *const *ctx, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                               MirostatState *mu, int32_t *ids_out, const SampleConstraint *cons = nullptr);
-    // sample_steps that stops each context after the step whose id's text (not exactly "##") makes its reply end with `stop` (0..32
-    // bytes, "" no text stop), or after max_steps.  tail[i]: context i's reply so far (its last 32 bytes decide).  The steps are issued
-    // kReplyChunk at a time; the host waits for chunk j - 1's done flags before it issues chunk j + 1 and stops issuing once every
-    // context is done, so at most 2 kReplyChunk - 1 steps run past the last stop.  Afterwards context i holds what n_out[i] steps left
-    // (logits, DeviceState, arg-max; rng[i], mu[i]), and ids_out[s * n + i] = -1 for s >= n_out[i]; stopped[i] = the text ended it.  Needs
-    // the group's token table (set_token_table).  One wait per chunk, none of them stalling the device; returns the device ms.
+    // sample_steps with each context's own settings u[i] that stops context i after the step whose id's text (not exactly "##") makes
+    // its reply end with u[i].stop, or after u[i].max_steps.  tail[i]: context i's reply so far (its last 32 bytes decide).  Each step
+    // samples in one launch per kind of column present (the chain with greedy and constrained columns, mirostat), each over its own
+    // columns.  The steps are issued kReplyChunk at a time, at most S = max u[i].max_steps; the host waits for chunk j - 1's done flags
+    // before it issues chunk j + 1 and stops issuing once every context is done, so at most 2 kReplyChunk - 1 steps run past the last
+    // stop.  A done batched column is parked on its last fed id and position (llama_sample.cuh), so those steps write nothing of a context
+    // beyond its final n_past.  Afterwards context i holds what n_out[i] steps left (logits, DeviceState, arg-max; rng[i], mu[i]), and
+    // ids_out[s * n + i] (s < S) = -1 for s >= n_out[i]; stopped[i] = the text ended it.  Needs the group's token table (set_token_table).
+    // One wait per chunk, none of them stalling the device; returns the device ms.
     static constexpr int kReplyChunk = 4;
     static constexpr int kStopMax = 32;   // longest stop text
     // cons as in sample_steps; a constrained context also stops after the step that feeds id 2 (stopped[i] = 1).
@@ -149,13 +159,13 @@ public:
     // sampling launch and its decode step, and each context's first n_out[i] records come back in one copy at the end, scattered into rec's
     // arrays (entries without a record: -1 / NaN).  A context's first such call allocates its records (kLogprobRecordBytes n_ctx,
     // owned_bytes_).  The caller validates (n_past >= 1: there are logits to report on).
-    // pen (may be null: none, and no extra work is issued): every step first runs penalty_rows_kernel (llama_penalty.cuh), which writes
-    // each context's penalised logits into its own row, and the sampling launch reads that row; the raw logits stay as the decode step
-    // left them.  A context's first such call allocates its row, counts and history tail (kPenaltyBytesPerId n_vocab + 4 n_ctx bytes,
-    // owned_bytes_; a history tail longer than n_ctx ids grows the tail).  The caller validates and passes only non-neutral penalties.
-    static float sample_until(LlamaDevice *const *ctx, int n, int max_steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
-                              MirostatState *mu, const std::string &stop, const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped,
-                              const SampleConstraint *cons = nullptr, const LogprobRequest *rec = nullptr, const PenaltyRequest *pen = nullptr);
+    // Penalties (none of them non-neutral: no extra work is issued): every step first runs penalty_rows_kernel (llama_penalty.cuh) over
+    // the penalised columns, which writes each one's penalised logits into its own row, and the sampling launch reads that row; the raw
+    // logits stay as the decode step left them.  A context's first penalised call allocates its row, counts and history tail
+    // (kPenaltyBytesPerId n_vocab + 4 n_ctx bytes, owned_bytes_; a history tail longer than n_ctx ids grows the tail).  The caller validates.
+    static float sample_until(LlamaDevice *const *ctx, int n, const UntilArgs *u, const int *n_past, uint32_t (*rng)[625], MirostatState *mu,
+                              const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped, const SampleConstraint *cons = nullptr,
+                              const LogprobRequest *rec = nullptr);
     static constexpr int kPenaltyBytesPerId = 8;      // the penalised row (F32) and the window counts (int32), per vocabulary id
     // test seam: penalty_rows_kernel over `rows` (1..kMaxBatch) host rows of logits, row r's window the last min(repeat_last_n, n_last[r])
     // of its ids (rows' histories one after another in last_ids) into out [rows][n_vocab]; kernel_ms (may be null): the average
@@ -311,13 +321,13 @@ private:
     void ensure_logprob();
     std::unique_ptr<PenaltyScratch> pen_;   // sample_until's penalised row, from the context's first call with penalties (owned_bytes_)
     void ensure_penalty(int n_tail);        // ... with room for a history tail of n_tail ids
-    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, generator and mirostat μ;
-    // returns the stream the steps run on
+    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, its column's parameters
+    // p[i], generator and mirostat μ; returns the stream the steps run on
     // cons (may be null): each constrained context's state goes to its device copy, and k takes every column's tables
-    static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu,
+    static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu,
                                        smp::SampleArgsN<kMaxBatch> &a, const SampleConstraint *cons = nullptr, smp::ConsArgsN<kMaxBatch> *k = nullptr);
     static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
-    static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs &p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
+    static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
                               cudaStream_t s);
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)
     void free_weights();             // by the last context of the group

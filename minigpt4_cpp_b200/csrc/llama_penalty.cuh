@@ -2,7 +2,8 @@
 // §4.15).
 //
 // A step of sample_until with penalties runs one extra launch before its sampling launch.  penalty_rows_kernel copies each context's raw
-// logits into its penalised row, then rewrites the ids of the step's window there (Sampler::penalize, text.cpp).  The sampling launch's
+// logits into its penalised row, then rewrites the ids of the step's window there (Sampler::penalize, text.cpp).  Each column carries its
+// own parameters, and the launch covers the penalised columns only: the others sample their raw logits and cost nothing here.  The sampling launch's
 // columns read that row instead of the raw logits, so the sampling kernels run unchanged; the raw logits, which the decode step writes,
 // are never touched.  Greedy columns also get the first arg-max of the penalised row in DeviceState::tokens[0], the id the greedy
 // sampling path feeds.
@@ -23,15 +24,16 @@ struct PenaltyCol {
     DeviceState *state;               // greedy: tokens[0] takes the first arg-max of the row (null: not written)
     const smp::ReplyState *reply;     // done != 0: the column stopped (null: it runs, the test seam)
     int n_tail;
+    PenaltyParams q;                  // the column's penalties
+    int greedy;                       // the column samples greedily (temp <= 0)
 };
 struct PenaltyArgs {
     PenaltyCol c[LlamaDevice::kMaxBatch];
-    int n_vocab, step, repeat_last_n, penalize_nl, greedy;
-    float repeat_penalty, alpha_presence, alpha_frequency;
+    int n_vocab, step;
 };
 
 // z' of an id with c >= 1 copies in the window (every operation rounded on its own: the build passes -fmad=false)
-__device__ __forceinline__ float penalized(float z, int c, const PenaltyArgs &a) {
+__device__ __forceinline__ float penalized(float z, int c, const PenaltyParams &a) {
     const float z1 = a.repeat_penalty == 1.0f ? z : (z <= 0.f ? z * a.repeat_penalty : z / a.repeat_penalty);
     return (a.alpha_frequency == 0.f && a.alpha_presence == 0.f) ? z1 : z1 - ((float)c * a.alpha_frequency + a.alpha_presence);
 }
@@ -57,17 +59,17 @@ __global__ void __launch_bounds__(kThreads) penalty_rows_kernel(const __grid_con
     for (int i = i0 + tid; i < V; i += kThreads) out[i] = z[i];
     if (done) return;
     // ---- counts of the window's ids, then each entry rewrites its id (copies of one id write the same value)
-    const int T = col.n_tail, end = T + a.step, first = end - min(a.repeat_last_n, end);
+    const int T = col.n_tail, end = T + a.step, first = end - min(col.q.repeat_last_n, end);
     for (int j = first + tid; j < end; j += kThreads) atomicAdd(&col.count[j < T ? col.tail[j] : col.fed[j - T]], 1);
     __syncthreads();
-    const bool keep_nl = !a.penalize_nl && V > 13;
+    const bool keep_nl = !col.q.penalize_nl && V > 13;
     for (int j = first + tid; j < end; j += kThreads) {
         const int v = j < T ? col.tail[j] : col.fed[j - T];
-        if (!(keep_nl && v == 13)) out[v] = penalized(z[v], col.count[v], a);
+        if (!(keep_nl && v == 13)) out[v] = penalized(z[v], col.count[v], col.q);
     }
     __syncthreads();
     for (int j = first + tid; j < end; j += kThreads) col.count[j < T ? col.tail[j] : col.fed[j - T]] = 0;
-    if (!a.greedy || !col.state) return;
+    if (!col.greedy || !col.state) return;
     // ---- greedy: the first arg-max of the penalised row (the largest smp::desc_key: logit desc, then the lower id)
     __shared__ unsigned long long best;
     if (tid == 0) best = 0ull;

@@ -239,12 +239,12 @@ struct SampleCtx {
     int *ids;                    // [n_ctx] the id fed at each step of a call
     unsigned long long *keys;    // [pow2 >= n_vocab] sort keys; the discrete distribution's cumulative doubles afterwards
     int *id; float *logit, *p, *aux;   // [n_vocab] candidates (id, logit, probability); tail_free's d2 / typical's terms
+    SamplingArgs args;           // the column's sampling parameters (mirostat 1 / 2: the mirostat kernels, which ignore top_k .. typical_p)
 };
 // a sampling launch's arguments, one column per CTA; the table is passed by value, so its capacity N is part of the kernel's parameters
 template <int N> struct SampleArgsN {
     SampleCtx c[N];
-    int n_vocab, step, top_k;
-    float temp, top_p, tfs_z, typical_p;
+    int n_vocab, step;
 };
 struct SampleArgs : SampleArgsN<8> {};                               // the kernels of 1..8 contexts
 using SampleArgsWide = SampleArgsN<LlamaDevice::kMaxBatch>;          // the wide kernels of 9..kMaxBatch contexts
@@ -398,10 +398,9 @@ struct AllowedIds {
     int n;
     __device__ __forceinline__ bool listed() const { return tr != nullptr; }
 };
-// the sampling parameters of a constrained column with its candidates
+// a constrained launch's column: its candidates
 struct ListedArgs {
-    int n_vocab, top_k;
-    float temp, top_p, tfs_z, typical_p;
+    int n_vocab;
     AllowedIds src;
 };
 template <class A> struct CandTraits { static constexpr bool kListed = false; };
@@ -415,9 +414,10 @@ __device__ __forceinline__ bool cand_listed(const ListedArgs &a) { return a.src.
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits over the
-// candidates of a (cand_*) as Sampler::sample (Sampler::sample_allowed for listed candidates) does and hands the id to fed(id, greedy) on thread 0.
-// temp <= 0: the greedy id the logits epilogue already left in tokens[0] (greedy = true; the generator is not read), or for listed
-// candidates their arg-max, the lower id on ties (greedy = false).  Otherwise the generator is written back after fed returns.
+// candidates of a (cand_*) as Sampler::sample (Sampler::sample_allowed for listed candidates) does with the column's parameters c.args,
+// and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in tokens[0] (greedy =
+// true; the generator is not read), or for listed candidates their arg-max, the lower id on ties (greedy = false).  Otherwise the
+// generator is written back after fed returns.
 // ---------------------------------------------------------------------------------------------------------------------------------
 template <class A, class Fed> __device__ __forceinline__ void sample_body(const A &a, const SampleCtx &c, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
@@ -427,7 +427,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     __shared__ int sh_need, sh_done, sh_n;
     __shared__ float red;
     const int tid = threadIdx.x, n = cand_size(a);
-    if (a.temp <= 0.f) {
+    if (c.args.temp <= 0.f) {
         if constexpr (CandTraits<A>::kListed) {
             if (cand_listed(a)) {
                 if (tid == 0) sh_prefix = 0ull;
@@ -447,7 +447,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     if (tid == 0) mt.p = c.mt->p;
 
     // ---- top_k: the k largest (logit desc, id asc) keys; k = top_k (<= 0: all candidates) clamped to [1, candidates] as Sampler::top_k does
-    const int k = min(max(a.top_k <= 0 ? n : a.top_k, 1), n);
+    const int k = min(max(c.args.top_k <= 0 ? n : c.args.top_k, 1), n);
     if (k == n) {
         if constexpr (CandTraits<A>::kListed) {
             for (int j = tid; j < n; j += blockDim.x) { const int i = cand_id(a, j); c.id[j] = i; c.logit[j] = c.logits[i]; }
@@ -493,7 +493,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     bool sorted = true;
 
     // ---- tail_free
-    if (a.tfs_z < 1.0f && m > 2) {
+    if (c.args.tfs_z < 1.0f && m > 2) {
         softmax_sorted(c, m, &red);
         for (int i = tid; i < m - 2; i += blockDim.x) {
             const float d1a = c.p[i] - c.p[i + 1], d1b = c.p[i + 1] - c.p[i + 2];
@@ -504,7 +504,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
             float s = 0.f;
             walk(c.aux, m - 2, [&](int, float v) { s += v; return true; });
             float cum = 0.f; int last = m;
-            walk(c.aux, m - 2, [&](int i, float v) { cum += v / s; if (cum > a.tfs_z && i >= 1) { last = i; return false; } return true; });
+            walk(c.aux, m - 2, [&](int i, float v) { cum += v / s; if (cum > c.args.tfs_z && i >= 1) { last = i; return false; } return true; });
             sh_n = last;
         }
         __syncthreads();
@@ -512,7 +512,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     }
 
     // ---- typical: the candidates in order of |-log p - H| (ties by index) until their mass exceeds typical_p; leaves them unsorted
-    if (a.typical_p < 1.0f) {
+    if (c.args.typical_p < 1.0f) {
         softmax_sorted(c, m, &red);
         for (int i = tid; i < m; i += blockDim.x) c.aux[i] = -c.p[i] * glibc_logf(c.p[i]);
         __syncthreads();
@@ -535,7 +535,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
         bitonic_desc(buf, P, sbuf);
         if (tid == 0) {
             float cum = 0.f; int last = m;
-            for (int i = 0; i < m; ++i) { cum += c.p[key_id(buf[i])]; if (cum > a.typical_p) { last = i + 1; break; } }
+            for (int i = 0; i < m; ++i) { cum += c.p[key_id(buf[i])]; if (cum > c.args.typical_p) { last = i + 1; break; } }
             sh_n = last;
         }
         __syncthreads();
@@ -552,12 +552,12 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     }
 
     // ---- top_p
-    if (a.top_p < 1.0f) {
+    if (c.args.top_p < 1.0f) {
         if (!sorted) { sort_by_logit(c, m, sbuf); sorted = true; }
         softmax_sorted(c, m, &red);
         if (tid == 0) {
             float cum = 0.f; int last = m;
-            walk(c.p, m, [&](int i, float v) { cum += v; if (cum >= a.top_p) { last = i + 1; return false; } return true; });
+            walk(c.p, m, [&](int i, float v) { cum += v; if (cum >= c.args.top_p) { last = i + 1; return false; } return true; });
             sh_n = last;
         }
         __syncthreads();
@@ -565,7 +565,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
     }
 
     // ---- temperature, then draw: softmax, std::discrete_distribution<int> over the float probabilities
-    for (int i = tid; i < m; i += blockDim.x) c.logit[i] = c.logit[i] / a.temp;
+    for (int i = tid; i < m; i += blockDim.x) c.logit[i] = c.logit[i] / c.args.temp;
     __syncthreads();
     if (!sorted) sort_by_logit(c, m, sbuf);
     softmax_sorted(c, m, &red);
@@ -577,33 +577,33 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // one context's mirostat step, the body of sample_mirostat_kernel and sample_until_mirostat_kernel: Sampler::sample's mirostat branch
-// (mode 1 or 2) with its μ in `ms`, handing the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id, and neither μ nor the
-// generator is read.  Otherwise μ is set to 2 tau at the mode's first use, as on the host, and updated after the draw.
+// (c.args.mirostat 1 or 2, its tau and eta) with its μ in `ms`, handing the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy
+// id, and neither μ nor the generator is read.  Otherwise μ is set to 2 tau at the mode's first use, as on the host, and updated after
+// the draw.
 // ---------------------------------------------------------------------------------------------------------------------------------
-struct MirostatArgs { int mode; float tau, eta; };   // mode 1 or 2
-
 // a context's μ: right after its generator in its SamplerScratch (llama.cu), so that one copy moves both
 __device__ __forceinline__ MirostatState &mirostat_state(const SampleCtx &c) { return *(MirostatState *)(c.mt + 1); }
 
 template <class A, class Fed>
-__device__ __forceinline__ void mirostat_body(const A &a, const MirostatArgs &ma, const SampleCtx &c, MirostatState &ms, Fed fed) {
+__device__ __forceinline__ void mirostat_body(const A &a, const SampleCtx &c, MirostatState &ms, Fed fed) {
     __shared__ unsigned long long sbuf[kSmemSort];
     __shared__ MtState mt;
     __shared__ int sh_n;
     __shared__ float red;
-    const int tid = threadIdx.x, n = a.n_vocab, v = ma.mode - 1;
-    if (a.temp <= 0.f) {
+    const SamplingArgs &ma = c.args;
+    const int tid = threadIdx.x, n = a.n_vocab, v = ma.mirostat - 1;
+    if (ma.temp <= 0.f) {
         if (tid == 0) fed(c.state->tokens[0], true);
         return;
     }
     for (int i = tid; i < kMtN; i += blockDim.x) mt.x[i] = c.mt->x[i];
     if (tid == 0) {
         mt.p = c.mt->p;
-        if (!ms.init[v]) { ms.mu[v] = 2.0f * ma.tau; ms.init[v] = 1; }
+        if (!ms.init[v]) { ms.mu[v] = 2.0f * ma.mirostat_tau; ms.init[v] = 1; }
         sh_n = n;
     }
     // temperature over the whole vocabulary, then the sort by the divided logit and the softmax
-    for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i] / a.temp; }
+    for (int i = tid; i < n; i += blockDim.x) { c.id[i] = i; c.logit[i] = c.logits[i] / ma.temp; }
     __syncthreads();
     sort_by_logit(c, n, sbuf);
     softmax_sorted(c, n, &red);
@@ -632,10 +632,10 @@ __device__ __forceinline__ void mirostat_body(const A &a, const MirostatArgs &ma
         fed(c.id[idx], false);
         // μ -= eta (surprise - tau) with the drawn candidate's probability after the draw's softmax, NaNs as on x86
         const float s = neg(glibc_log2f(c.p[idx]));
-        float d = s - ma.tau;
-        if (isnan(d)) d = x86_nan(s, ma.tau);
-        float e = ma.eta * d;
-        if (isnan(e)) e = x86_nan(ma.eta, d);
+        float d = s - ma.mirostat_tau;
+        if (isnan(d)) d = x86_nan(s, ma.mirostat_tau);
+        float e = ma.mirostat_eta * d;
+        if (isnan(e)) e = x86_nan(ma.mirostat_eta, d);
         float r = mu - e;
         if (isnan(r)) r = x86_nan(mu, e);
         ms.mu[v] = r;
@@ -661,15 +661,15 @@ template <class A> __device__ __forceinline__ void sample_step(const A &a) {
     const SampleCtx &c = a.c[blockIdx.x];
     sample_body(a, c, [&](int id, bool greedy) { feed(a, c, id, greedy); });
 }
-template <class A> __device__ __forceinline__ void sample_mirostat_step(const A &a, const MirostatArgs &m) {
+template <class A> __device__ __forceinline__ void sample_mirostat_step(const A &a) {
     const SampleCtx &c = a.c[blockIdx.x];
-    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { feed(a, c, id, greedy); });
+    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { feed(a, c, id, greedy); });
 }
 __global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) { sample_step(a); }
 __global__ void __launch_bounds__(kThreads) sample_wide_kernel(const SampleArgsWide a) { sample_step(a); }
 // sample_kernel with the mirostat step
-__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a, const MirostatArgs m) { sample_mirostat_step(a, m); }
-__global__ void __launch_bounds__(kThreads) sample_mirostat_wide_kernel(const SampleArgsWide a, const MirostatArgs m) { sample_mirostat_step(a, m); }
+__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a) { sample_mirostat_step(a); }
+__global__ void __launch_bounds__(kThreads) sample_mirostat_wide_kernel(const SampleArgsWide a) { sample_mirostat_step(a); }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // stop on the reply's text (minigpt4_b200_sample_until; host side LlamaDevice::sample_until): the reference's chat loop
@@ -687,6 +687,10 @@ struct ReplyState {                  // one context's stop state in a call (the 
     int done;                        // 0 running; 1 stopped at the previous step; 2 stopped, logits and state in the snapshot
     int n_fed;                       // steps that fed an id
     DeviceState snap;
+};
+struct UntilState : ReplyState {     // a context's state in a sample_until call (beam search keeps bare ReplyStates)
+    int budget;                      // the context's max_steps: it is done once n_fed reaches it
+    int by_budget;                   // 1: the budget, not the text (or </s>), ended it
 };
 
 // the reply takes id's text; returns true if that step ends it.  One thread; no local arrays.
@@ -711,20 +715,22 @@ __device__ __forceinline__ bool reply_take(ReplyState &r, TokenTable t, int id) 
 }
 
 template <int N> struct StopArgsN {
-    ReplyState *r[N];
+    UntilState *r[N];
     float *snap[N];   // [n_vocab] each context's logits after its last step
     TokenTable tab;
 };
 struct StopArgs : StopArgsN<8> {};
 using StopArgsWide = StopArgsN<LlamaDevice::kMaxBatch>;
-static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) + sizeof(MirostatArgs) <= 32764, "the widest kernel's parameters fit the 32 764-byte limit");
+static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) <= 32764, "the widest kernel's parameters fit the 32 764-byte limit");
 
-// one step of sample_kernel that stops each context on its reply's text.  A stopped context does not draw (its generator stays); at
-// the next step it saves its logits and DeviceState, which the host restores at the end of the call, and later steps only keep its
-// batched column moving, so the decode work that still runs for it writes K/V above its final position.
+// one step of sample_kernel that stops each context on its reply's text or its budget.  A stopped context does not draw (its generator
+// stays); at the next step it saves its logits and DeviceState, which the host restores at the end of the call.  The decode work that
+// still runs for a batched column is parked: it feeds the column's last fed id again at that id's own position, so it rewrites the same
+// K / V bits (the batched step is bit-exact per column) and never writes past the context's final n_past, which its budget keeps within
+// n_ctx while other columns run on.
 // the start of a step of the stopping kernels (sh_state: a __shared__ int of the kernel): false for a context that has stopped (it saves
-// its snapshot once and keeps its column moving), true for one that samples
-template <class A, class S> __device__ __forceinline__ bool until_running(const A &a, const S &s, const SampleCtx &c, ReplyState &r, int &sh_state) {
+// its snapshot once and parks its column), true for one that samples
+template <class A, class S> __device__ __forceinline__ bool until_running(const A &a, const S &s, const SampleCtx &c, UntilState &r, int &sh_state) {
     if (threadIdx.x == 0) sh_state = r.done;   // (read once: thread 0 writes r.done when it feeds)
     __syncthreads();
     const int done = sh_state;
@@ -734,47 +740,53 @@ template <class A, class S> __device__ __forceinline__ bool until_running(const 
             for (int i = threadIdx.x; i < a.n_vocab; i += blockDim.x) snap[i] = c.logits[i];
             if (threadIdx.x == 0) { r.snap = *c.state; r.done = 2; }
         }
-        if (threadIdx.x == 0 && c.slot) c.slot->n_past = c.n_past0 + a.step;
+        if (threadIdx.x == 0 && c.slot) {   // (after the snapshot: tokens[0] is that of the state it saved)
+            const int last = r.n_fed - 1;
+            c.slot->n_past = c.n_past0 + last;
+            c.state->tokens[0] = c.ids[last];
+        }
         return false;
     }
     return true;
 }
-// the id a step of the stopping kernels feeds, and the stop check on it
-template <class A, class S> __device__ __forceinline__ void until_feed(const A &a, const S &s, const SampleCtx &c, ReplyState &r, int id, bool greedy) {
+// the id a step of the stopping kernels feeds, and the stop checks on it: the text (or `end`), then the budget
+template <class A, class S>
+__device__ __forceinline__ void until_feed(const A &a, const S &s, const SampleCtx &c, UntilState &r, int id, bool greedy, bool end = false) {
     feed(a, c, id, greedy);
     r.n_fed = a.step + 1;
-    if (reply_take(r, s.tab, id)) r.done = 1;
+    if (reply_take(r, s.tab, id) || end) r.done = 1;
+    else if (r.n_fed == r.budget) { r.done = 1; r.by_budget = 1; }
 }
 
 __global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs a, const StopArgs s) {
     const SampleCtx &c = a.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
+    UntilState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
     sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
 __global__ void __launch_bounds__(kThreads) sample_until_wide_kernel(const SampleArgsWide a, const StopArgsWide s) {
     const SampleCtx &c = a.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
+    UntilState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
     sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
 
 // sample_until_kernel with the mirostat step
-__global__ void __launch_bounds__(kThreads) sample_until_mirostat_kernel(const SampleArgs a, const StopArgs s, const MirostatArgs m) {
+__global__ void __launch_bounds__(kThreads) sample_until_mirostat_kernel(const SampleArgs a, const StopArgs s) {
     const SampleCtx &c = a.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
+    UntilState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
-    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
-__global__ void __launch_bounds__(kThreads) sample_until_mirostat_wide_kernel(const SampleArgsWide a, const StopArgsWide s, const MirostatArgs m) {
+__global__ void __launch_bounds__(kThreads) sample_until_mirostat_wide_kernel(const SampleArgsWide a, const StopArgsWide s) {
     const SampleCtx &c = a.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
+    UntilState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
-    mirostat_body(a, m, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -798,9 +810,7 @@ template <class A> __device__ __forceinline__ AllowedIds allowed_ids(const A &a,
     const int s = *k.state, o = k.off[s];
     return AllowedIds{k.tr + o, k.off[s + 1] - o};
 }
-template <class A> __device__ __forceinline__ ListedArgs listed_args(const A &a, const AllowedIds &src) {
-    return ListedArgs{a.n_vocab, a.top_k, a.temp, a.top_p, a.tfs_z, a.typical_p, src};
-}
+template <class A> __device__ __forceinline__ ListedArgs listed_args(const A &a, const AllowedIds &src) { return ListedArgs{a.n_vocab, src}; }
 // thread 0, after the draw: the state the fed id leads to (a binary search for it in the row)
 __device__ __forceinline__ void cons_advance(const ConsCol &k, const AllowedIds &src, int id) {
     if (!src.listed()) return;
@@ -823,14 +833,13 @@ template <class A, class K> __device__ __forceinline__ void sample_cons_step(con
 template <class A, class S, class K> __device__ __forceinline__ void sample_until_cons_step(const A &a, const S &s, const K &k) {
     const SampleCtx &c = a.c[blockIdx.x];
     const ConsCol &kc = k.c[blockIdx.x];
-    ReplyState &r = *s.r[blockIdx.x];
+    UntilState &r = *s.r[blockIdx.x];
     __shared__ int sh_state;
     if (!until_running(a, s, c, r, sh_state)) return;
     const AllowedIds src = allowed_ids(a, kc);
     sample_body(listed_args(a, src), c, [&](int id, bool greedy) {
-        until_feed(a, s, c, r, id, greedy);
+        until_feed(a, s, c, r, id, greedy, src.listed() && id == 2);
         cons_advance(kc, src, id);
-        if (src.listed() && id == 2) r.done = 1;
     });
 }
 __global__ void __launch_bounds__(kThreads) sample_cons_kernel(const SampleArgs a, const ConsArgs k) { sample_cons_step(a, k); }

@@ -9,6 +9,7 @@ points of ``include/minigpt4_b200.h``.
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import enum
 import os
 import sys
@@ -196,6 +197,35 @@ class Stats(C.Structure):
                 ("prefill_gemm", C.c_int)]
 
 
+class GenParamsC(C.Structure):  # include/minigpt4_b200.h struct MiniGPT4B200GenParams
+    _fields_ = [("size", C.c_int32), ("max_steps", C.c_int32), ("stop", C.c_char_p), ("temp", C.c_float), ("top_k", C.c_int32),
+                ("top_p", C.c_float), ("tfs_z", C.c_float), ("typical_p", C.c_float), ("mirostat", C.c_int32), ("mirostat_tau", C.c_float),
+                ("mirostat_eta", C.c_float), ("repeat_last_n", C.c_int32), ("repeat_penalty", C.c_float), ("alpha_presence", C.c_float),
+                ("alpha_frequency", C.c_float), ("penalize_nl", C.c_int32), ("n_last", C.c_int32), ("last_ids", C.POINTER(C.c_int32))]
+
+
+@dataclasses.dataclass
+class GenParams:
+    """one context's settings in B200.generate_batch: B200.sample_until's defaults (mirostat 1 / 2 ignores top_k .. typical_p), with
+    neutral penalties (repeat_penalty 1, both alphas 0); last_ids is the penalty history (None: none)"""
+    max_steps: int
+    stop: str | bytes | None = None
+    temp: float = 0.8
+    top_k: int = 40
+    top_p: float = 0.9
+    tfs_z: float = 1.0
+    typical_p: float = 1.0
+    mirostat: int = 0
+    mirostat_tau: float = 5.0
+    mirostat_eta: float = 1.0
+    repeat_last_n: int = 64
+    repeat_penalty: float = 1.0
+    alpha_presence: float = 0.0
+    alpha_frequency: float = 0.0
+    penalize_nl: bool = True
+    last_ids: Optional[list] = None
+
+
 _VP = C.c_void_p
 _EXT = {
     "minigpt4_b200_device_count": ([], _I),
@@ -238,6 +268,7 @@ _EXT = {
     "minigpt4_b200_op_logprobs": ([_VP, _I, _I, _VP, _I, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_sample_until_penalized": ([_VP, _I, _I, _S, _F, _I, _F, _F, _F, _I, _F, _F, _I, _F, _F, _F, _I, _VP, _VP, _VP, _VP, _VP,
                                               C.POINTER(C.c_float)], _I),
+    "minigpt4_b200_generate_batch": ([_VP, _I, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)], _I),
     "minigpt4_b200_end_chat_penalized": ([_CTX, C.POINTER(_S), _F, _I, _F, _F, _F, _I, _F, _F, _F, _I, _I, _F, _F, _VP, _I,
                                           C.POINTER(C.c_int32)], _I),
     "minigpt4_b200_op_penalize": ([_VP, _I, _I, _VP, _VP, _I, _F, _F, _F, _I, _I, _VP, C.POINTER(C.c_float)], _I),
@@ -541,6 +572,42 @@ class B200:
                                                               alpha_presence, alpha_frequency, int(penalize_nl), _ptr(hist), _ptr(n_last),
                                                               _ptr(ids), _ptr(n_out), _ptr(stopped), C.byref(ms)))
         return [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]], ms.value
+
+    @staticmethod
+    def gen_params_c(params: list[GenParams]) -> tuple:
+        """the C array of params and the buffers it points into (keep them alive for the call)"""
+        arr = (GenParamsC * max(1, len(params)))()
+        keep = []
+        for i, g in enumerate(params):
+            st = g.stop.encode() if isinstance(g.stop, str) else g.stop
+            hist = np.ascontiguousarray(g.last_ids if g.last_ids is not None else [], np.int32)
+            keep += [st, hist]
+            arr[i] = GenParamsC(C.sizeof(GenParamsC), g.max_steps, st, g.temp, g.top_k, g.top_p, g.tfs_z, g.typical_p, g.mirostat, g.mirostat_tau,
+                                g.mirostat_eta, g.repeat_last_n, g.repeat_penalty, g.alpha_presence, g.alpha_frequency, int(g.penalize_nl), hist.size,
+                                hist.ctypes.data_as(C.POINTER(C.c_int32)) if hist.size else None)
+        return arr, keep
+
+    def generate_batch(self, ctxs, params: list[GenParams], top_n: int = 0, logprobs: bool = False) -> tuple:
+        """device-sampled replies of every context in `ctxs` (1..64 of one group), context i with its own settings params[i] (sampler,
+        penalties, stop text, budget), in one batched call; each context ends where it would end alone.  Returns each context's fed ids,
+        whether the stop text ended it, with logprobs its records (as sample_until_logprobs returns them; top_n 0..20) and the device ms."""
+        n = len(ctxs)
+        arr, _keep = self.gen_params_c(params)
+        S = max([g.max_steps for g in params] + [1])
+        shape = (S, max(1, n))
+        ids = np.zeros(shape, np.int32)
+        n_out, stopped = np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.int32)
+        lp, rk = np.zeros(shape, np.float32), np.zeros(shape, np.int32)
+        tid, tlp = np.zeros(shape + (max(1, top_n),), np.int32), np.zeros(shape + (max(1, top_n),), np.float32)
+        ms = C.c_float(0)
+        self._chk(self.L.minigpt4_b200_generate_batch(C.cast(self._ctx_array(ctxs), C.c_void_p), n, C.cast(arr, C.c_void_p), top_n, _ptr(ids),
+                                                      _ptr(n_out), _ptr(stopped), _ptr(lp) if logprobs else None, _ptr(rk) if logprobs else None,
+                                                      _ptr(tid) if logprobs else None, _ptr(tlp) if logprobs else None, C.byref(ms)))
+        out = [ids[:n_out[i], i].tolist() for i in range(n)], [bool(x) for x in stopped[:n]]
+        if not logprobs:
+            return (*out, ms.value)
+        recs = [(lp[:k, i].copy(), rk[:k, i].copy(), tid[:k, i, :top_n].copy(), tlp[:k, i, :top_n].copy()) for i, k in enumerate(n_out[:n].tolist())]
+        return (*out, recs, ms.value)
 
     def end_chat_penalized(self, ctx, last_ids=None, repeat_last_n: int = 64, repeat_penalty: float = 1.1, alpha_presence: float = 0.0,
                            alpha_frequency: float = 0.0, penalize_nl: bool = True, temp: float = 0.8, top_k: int = 40, top_p: float = 0.9,
