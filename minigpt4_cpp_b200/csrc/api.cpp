@@ -124,7 +124,7 @@ int minigpt4_end_chat_image(struct MiniGPT4Context *ctx, const char **token, siz
                             float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {
     Engine *e = E(ctx);
     if (e->constraint() && (mirostat == 1 || mirostat == 2)) { MG4_ERR("end_chat: mirostat on a constrained context"); return ErrFailedToAddString; }
-    SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    SamplingArgs sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     const int32_t id = e->sample_token(sp);
     *token = e->id_to_token(id);
     e->add_tokens({id});  // the reference ignores this return value too (minigpt4.cpp:2715)
@@ -266,7 +266,7 @@ int minigpt4_b200_state_load(struct MiniGPT4Context *ctx, const void *buf, long 
 int minigpt4_b200_end_chat_batch(struct MiniGPT4Context **ctxs, int n, const char **tokens, float temp, int32_t top_k, float top_p, float tfs_z,
                                  float typical_p, int32_t /*repeat_last_n*/, float /*repeat_penalty*/, float /*alpha_presence*/,
                                  float /*alpha_frequency*/, int mirostat, float mirostat_tau, float mirostat_eta, int /*penalize_nl*/) {
-    SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    SamplingArgs sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     return Engine::end_chat_batch(reinterpret_cast<Engine *const *>(ctxs), n, tokens, sp);
 }
 int minigpt4_b200_sample_steps(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int32_t top_k, float top_p, float tfs_z, float typical_p,
@@ -301,13 +301,13 @@ int minigpt4_b200_op_beam_rank(const float *logits, int n_live, const float *S, 
 int minigpt4_b200_sample_steps_mirostat(struct MiniGPT4Context **ctxs, int n, int steps, float temp, int mirostat, float mirostat_tau,
                                         float mirostat_eta, int32_t *ids_out, float *ms_out) {
     if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
-    return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta},
+    return Engine::sample_steps(reinterpret_cast<Engine *const *>(ctxs), n, steps, sampling_args(temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta),
                                 ids_out, ms_out);
 }
 int minigpt4_b200_sample_until_mirostat(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int mirostat,
                                         float mirostat_tau, float mirostat_eta, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out) {
     if (!ctxs || (mirostat != 1 && mirostat != 2)) return ErrFailedToAddString;
-    const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta});
+    const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, sampling_args(temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta));
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out);
 }
 int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, int max_steps, const char *stop, float temp, int32_t top_k,
@@ -316,8 +316,7 @@ int minigpt4_b200_sample_until_logprobs(struct MiniGPT4Context **ctxs, int n, in
                                         int32_t *top_ids_out, float *top_logprob_out, float *ms_out) {
     if (!ctxs) return ErrFailedToAddString;
     // the sampling arguments of the call this one stands for
-    const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
-                                    : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
+    const SamplingArgs p = sampling_args(temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta);
     const LogprobRequest rec{top_n, logprob_out, rank_out, top_ids_out, top_logprob_out};
     const std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, p);
     return Engine::sample_until(reinterpret_cast<Engine *const *>(ctxs), n, u.data(), ids_out, n_out, stopped, ms_out, &rec, "sample_until_logprobs");
@@ -338,8 +337,7 @@ int minigpt4_b200_sample_until_penalized(struct MiniGPT4Context **ctxs, int n, i
                                          float *ms_out) {
     if (!ctxs) return ErrFailedToAddString;
     // the sampling arguments of the call this one stands for
-    const SamplingArgs p = mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}
-                                    : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
+    const SamplingArgs p = sampling_args(temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta);
     std::vector<UntilArgs> u = uniform_until(n, max_steps, stop, p);
     size_t at = 0;   // context i's history: its n_last[i] ids after those of contexts 0 .. i-1
     for (int i = 0; i < (int)u.size() && i < n; ++i) {
@@ -365,8 +363,7 @@ int minigpt4_b200_generate_batch(struct MiniGPT4Context **ctxs, int n, const str
             MG4_ERR("generate_batch: params[%d].size %d (%zu)", i, g.size, sizeof(MiniGPT4B200GenParams)); return ErrFailedToAddString;
         }
         // mirostat 1 / 2 ignores top_k .. typical_p, as sample_until_mirostat does
-        const SamplingArgs p = g.mirostat ? SamplingArgs{g.temp, 0, 1.f, 1.f, 1.f, g.mirostat, g.mirostat_tau, g.mirostat_eta}
-                                          : SamplingArgs{g.temp, g.top_k, g.top_p, g.tfs_z, g.typical_p};
+        const SamplingArgs p = sampling_args(g.temp, g.top_k, g.top_p, g.tfs_z, g.typical_p, g.mirostat, g.mirostat_tau, g.mirostat_eta);
         u[(size_t)i] = UntilArgs{p, g.max_steps, g.stop ? g.stop : "###",
                                  PenaltyParams{g.repeat_last_n, g.repeat_penalty, g.alpha_presence, g.alpha_frequency, g.penalize_nl}, g.last_ids, g.n_last};
     }
@@ -379,7 +376,7 @@ int minigpt4_b200_end_chat_penalized(struct MiniGPT4Context *ctx, const char **t
                                      int penalize_nl, int mirostat, float mirostat_tau, float mirostat_eta, const int32_t *last_ids, int n_last,
                                      int32_t *id_out) {
     if (!ctx) return ErrFailedToAddString;
-    const SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    const SamplingArgs sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     return E(ctx)->end_chat_penalized(sp, PenaltyParams{repeat_last_n, repeat_penalty, alpha_presence, alpha_frequency, penalize_nl}, last_ids, n_last,
                                       token, id_out);
 }
@@ -523,7 +520,7 @@ int minigpt4_b200_host_tokenize(const char *llm_model, const char *text, int add
 int minigpt4_b200_host_sample(const float *logits, int n_vocab, int seed, float temp, int32_t top_k, float top_p, float tfs_z, float typical_p,
                               int mirostat, float mirostat_tau, float mirostat_eta, int n_draws, int32_t *out_ids) {
     Sampler s(seed);
-    SamplingParams sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
+    SamplingArgs sp{temp, top_k, top_p, tfs_z, typical_p, mirostat, mirostat_tau, mirostat_eta};
     for (int i = 0; i < n_draws; ++i) out_ids[i] = s.sample(logits, n_vocab, sp);
     return 0;
 }
@@ -545,7 +542,7 @@ int minigpt4_b200_op_sample_mirostat(const float *logits, int n_vocab, int seed,
         return ErrFailedToAddString;
     if (!on_device) {
         Sampler s(seed);
-        const SamplingParams sp{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta};
+        const SamplingArgs sp = sampling_args(temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta);
         for (int d = 0; d < n_draws; ++d) {
             ids_out[d] = s.sample(logits, n_vocab, sp);
             float mu[2]; bool init[2];
@@ -558,7 +555,7 @@ int minigpt4_b200_op_sample_mirostat(const float *logits, int n_vocab, int seed,
     if (!(temp > 0.f)) return ErrFailedToAddString;   // greedy: not the sampler
     uint32_t rng[625];
     Sampler(seed).get_rng(rng);
-    LlamaDevice::test_sample(logits, n_vocab, SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta}, rng, n_draws, ids_out, kernel_ms,
+    LlamaDevice::test_sample(logits, n_vocab, sampling_args(temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta), rng, n_draws, ids_out, kernel_ms,
                              mu_out);
     return 0;
 }

@@ -80,4 +80,13 @@ struct HostTensor {
 
 double now_ms();
 
+// Sampler::sample's arguments, on the host (text.h) and the device (llama_sample.cuh): the non-mirostat chain (mirostat 0), or mirostat
+// 1 / 2, which ignores top_k .. typical_p
+struct SamplingArgs { float temp; int32_t top_k; float top_p, tfs_z, typical_p; int mirostat; float mirostat_tau, mirostat_eta; };
+// the arguments of a call with these settings: with mirostat 1 / 2 top_k .. typical_p are neutral, with the chain tau and eta are 0
+inline SamplingArgs sampling_args(float temp, int32_t top_k, float top_p, float tfs_z, float typical_p, int mirostat, float mirostat_tau,
+                                  float mirostat_eta) {
+    return mirostat ? SamplingArgs{temp, 0, 1.f, 1.f, 1.f, mirostat, mirostat_tau, mirostat_eta} : SamplingArgs{temp, top_k, top_p, tfs_z, typical_p};
+}
+
 }  // namespace mg4

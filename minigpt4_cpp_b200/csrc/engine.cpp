@@ -122,7 +122,7 @@ Error Engine::decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t 
     for (int i = 0; i < n; ++i) e[i]->n_past_ += 1;
     return ErrNone;
 }
-Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p) {
+Error Engine::end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingArgs &p) {
     if (!tokens || !batch_valid(e, n, nullptr)) return ErrFailedToAddString;   // (before any sampler draws)
     if ((p.mirostat == 1 || p.mirostat == 2) && any_constrained(e, n)) { MG4_ERR("end_chat_batch: mirostat on a constrained context"); return ErrFailedToAddString; }
     if (!flush_group(e, n)) return ErrFailedToAddString;   // so that each sample_token finds its queue empty
@@ -150,14 +150,26 @@ bool Engine::any_constrained(Engine *const *e, int n) {
     for (int i = 0; i < n; ++i) if (e[i]->cons_) return true;
     return false;
 }
-void Engine::sample_constraints(Engine *const *e, int n, SampleConstraint *out) {
+template <class Call>
+float Engine::device_sampling(Engine *const *e, int n, const SamplingArgs *p, const int32_t *fed, const int32_t *ids_out, Call call) {
+    LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch]; MirostatState mu[LlamaDevice::kMaxBatch]; SampleConstraint cons[LlamaDevice::kMaxBatch];
+    std::vector<uint32_t> rng_words((size_t)n * 625);   // (625 words a generator: 160 KB at kMaxBatch, off the stack)
+    uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
     for (int i = 0; i < n; ++i) {
-        out[i] = SampleConstraint{};
-        const Constraint *c = e[i]->cons_.get();
-        if (!c) continue;
-        const int *off = (const int *)c->dev->dev;
-        out[i] = SampleConstraint{off, (const int2 *)(off + constraint_pairs_at(*c)), e[i]->cons_state_};
+        L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]);
+        cons[i] = SampleConstraint{};
+        if (const Constraint *c = e[i]->cons_.get()) {
+            const int *off = (const int *)c->dev->dev;
+            cons[i] = SampleConstraint{off, (const int2 *)(off + constraint_pairs_at(*c)), e[i]->cons_state_};
+        }
     }
+    const float ms = call(L, np, rng, mu, cons);
+    for (int i = 0; i < n; ++i) {
+        set_sampler_state(*e[i]->sampler_, p[i], rng[i], mu[i]);
+        e[i]->n_past_ += fed[i];
+        for (int t = 0; t < fed[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
+    }
+    return ms;
 }
 
 Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out) {
@@ -170,18 +182,14 @@ Error Engine::sample_steps(Engine *const *e, int n, int steps, const SamplingArg
         if (e[i]->n_past_ + steps > n_ctx) { MG4_ERR("sample_steps: context %d: %d + %d > n_ctx %d", i, e[i]->n_past_, steps, n_ctx); return ErrFailedToAddString; }
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
-    LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch]; MirostatState mu[LlamaDevice::kMaxBatch];
-    std::vector<uint32_t> rng_words((size_t)n * 625);   // (625 words a generator: 160 KB at kMaxBatch, off the stack)
-    uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
-    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); }
-    SampleConstraint cons[LlamaDevice::kMaxBatch];
-    sample_constraints(e, n, cons);
-    const float ms = LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out, cons);
-    for (int i = 0; i < n; ++i) {
-        set_sampler_state(*e[i]->sampler_, p, rng[i], mu[i]);
-        e[i]->n_past_ += steps;
-        for (int t = 0; t < steps; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
-    }
+    SamplingArgs ps[LlamaDevice::kMaxBatch];
+    int32_t fed[LlamaDevice::kMaxBatch];
+    std::fill(ps, ps + n, p);
+    std::fill(fed, fed + n, steps);
+    const float ms = device_sampling(e, n, ps, fed, ids_out, [&](LlamaDevice *const *L, const int *np, uint32_t (*rng)[625], MirostatState *mu,
+                                                                 const SampleConstraint *cons) {
+        return LlamaDevice::sample_steps(L, n, steps, np, p, rng, mu, ids_out, cons);
+    });
     if (ms_out) *ms_out = ms;
     return ErrNone;
 }
@@ -210,18 +218,13 @@ Error Engine::sample_until(Engine *const *e, int n, const UntilArgs *u, int32_t 
     }
     if (!flush_group(e, n)) return ErrFailedToAddString;
     e[0]->ensure_token_table();
-    LlamaDevice *L[LlamaDevice::kMaxBatch]; int np[LlamaDevice::kMaxBatch]; MirostatState mu[LlamaDevice::kMaxBatch]; std::string tail[LlamaDevice::kMaxBatch];
-    std::vector<uint32_t> rng_words((size_t)n * 625);
-    uint32_t (*rng)[625] = reinterpret_cast<uint32_t (*)[625]>(rng_words.data());
-    for (int i = 0; i < n; ++i) { L[i] = e[i]->llm_.get(); np[i] = e[i]->n_past_; sampler_state(*e[i]->sampler_, rng[i], mu[i]); tail[i] = e[i]->reply_; }
-    SampleConstraint cons[LlamaDevice::kMaxBatch];
-    sample_constraints(e, n, cons);
-    const float ms = LlamaDevice::sample_until(L, n, u, np, rng, mu, tail, ids_out, n_out, stopped, cons, rec);
-    for (int i = 0; i < n; ++i) {
-        set_sampler_state(*e[i]->sampler_, u[i].p, rng[i], mu[i]);
-        e[i]->n_past_ += n_out[i];
-        for (int t = 0; t < n_out[i]; ++t) e[i]->reply_take_id(ids_out[(size_t)t * n + i]);
-    }
+    SamplingArgs p[LlamaDevice::kMaxBatch];
+    std::string tail[LlamaDevice::kMaxBatch];
+    for (int i = 0; i < n; ++i) { p[i] = u[i].p; tail[i] = e[i]->reply_; }
+    const float ms = device_sampling(e, n, p, n_out, ids_out, [&](LlamaDevice *const *L, const int *np, uint32_t (*rng)[625], MirostatState *mu,
+                                                                  const SampleConstraint *cons) {
+        return LlamaDevice::sample_until(L, n, u, np, rng, mu, tail, ids_out, n_out, stopped, cons, rec);
+    });
     if (ms_out) *ms_out = ms;
     return ErrNone;
 }
@@ -239,7 +242,7 @@ bool Engine::history_valid(const int32_t *ids, int n, int n_vocab, const char *w
     for (int j = 0; j < n; ++j) if (ids[j] < 0 || ids[j] >= n_vocab) { MG4_ERR("%s: history id %d out of range", what, ids[j]); return false; }
     return true;
 }
-Error Engine::end_chat_penalized(const SamplingParams &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token,
+Error Engine::end_chat_penalized(const SamplingArgs &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token,
                                  int32_t *id_out) {
     if (!token || !penalty_valid(q, p.mirostat, "end_chat_penalized")) return ErrFailedToAddString;
     const int V = llm_->dims().n_vocab;
@@ -571,7 +574,7 @@ bool Engine::flush() {
     return ok;
 }
 
-int32_t Engine::sample_token(const SamplingParams &p) {
+int32_t Engine::sample_token(const SamplingArgs &p) {
     flush();
     if (cons_) {   // the chain over the allowed ids (greedy too: the arg-max among them, not the device's over every id)
         llm_->logits_to_host(logits_.data());

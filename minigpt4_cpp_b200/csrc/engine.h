@@ -28,7 +28,7 @@ public:
     // one decode step of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group, weights streamed once (see minigpt4_b200_decode_batch); all or nothing
     static Error decode_batch(Engine *const *e, int n, const int32_t *ids, int32_t *ids_out);
     // minigpt4_end_chat on each context (own logits, own sampler), then one decode_batch of the sampled ids
-    static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingParams &p);
+    static Error end_chat_batch(Engine *const *e, int n, const char **tokens, const SamplingArgs &p);
     // `steps` decode steps of n (1..64, LlamaDevice::kMaxBatch) distinct contexts of one group, each fed the id the device sampler draws from its logits with its
     // own generator and mirostat μ (see minigpt4_b200_sample_steps / _mirostat); ids_out[s * n + i]; all or nothing
     static Error sample_steps(Engine *const *e, int n, int steps, const SamplingArgs &p, int32_t *ids_out, float *ms_out);
@@ -40,7 +40,7 @@ public:
     static Error sample_until(Engine *const *e, int n, const UntilArgs *u, int32_t *ids_out, int32_t *n_out, int32_t *stopped, float *ms_out,
                               const LogprobRequest *rec = nullptr, const char *what = "sample_until");
     // minigpt4_end_chat with the context's host sampler over the penalised copy of its logits (see minigpt4_b200_end_chat_penalized)
-    Error end_chat_penalized(const SamplingParams &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token, int32_t *id_out);
+    Error end_chat_penalized(const SamplingArgs &p, const PenaltyParams &q, const int32_t *last_ids, int n_last, const char **token, int32_t *id_out);
     // the penalty arguments that need no context (mirostat 0..2 too: the penalised calls take all three modes); what: the caller's name
     static bool penalty_valid(const PenaltyParams &q, int mirostat, const char *what);
     // the n_hyp best replies of e[0]'s conversation by beam search over n (1..16) contexts of its group (see minigpt4_b200_beam_search);
@@ -69,7 +69,7 @@ public:
     Error add_tokens(const std::vector<int32_t> &tokens);
     Error add_strings(const char *s);
     Error add_embedding(const float *rows, int n_rows);
-    int32_t sample_token(const SamplingParams &p);
+    int32_t sample_token(const SamplingArgs &p);
     const char *id_to_token(int32_t id) const;
     void reset() { n_past_ = 0; pend_ids_.clear(); pend_emb_.clear(); reply_clear(); }
     // the current reply's last LlamaDevice::kStopMax bytes (the reference's `chat` of a turn): a new turn or prompt clears it, every
@@ -106,7 +106,12 @@ private:
     static bool batch_valid(Engine *const *e, int n, const int32_t *ids);
     static bool flush_group(Engine *const *e, int n);
     static bool any_constrained(Engine *const *e, int n);
-    static void sample_constraints(Engine *const *e, int n, SampleConstraint *out);   // each context's tables and state for a sampling call
+    // the handoff around a device sampling call: each context's device twin, position, generator, μ and constraint go to call, which
+    // returns the device ms; afterwards context i's sampler takes back its generator and μ (settings p[i]), and its position and reply move
+    // on by its fed[i] ids in ids_out[s * n + i] (fed is read after the call)
+    // (call(L, n_past, rng, mu, cons): LlamaDevice's call over the arrays of the contexts' device twins and their state)
+    template <class Call>
+    static float device_sampling(Engine *const *e, int n, const SamplingArgs *p, const int32_t *fed, const int32_t *ids_out, Call call);
     // a history of n ids for the penalties: n >= 0, ids non-null if n > 0, every id in 0 .. n_vocab - 1
     static bool history_valid(const int32_t *ids, int n, int n_vocab, const char *what);
     // shared by the sessions of one model (the last context of the group frees them, lanes before lane 0)

@@ -1007,7 +1007,7 @@ void LlamaDevice::build_batch_graph(int B) {
     G.graph_kernels[B] = (int)n;
 }
 
-void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids, const int *n_past, int32_t *ids_out) {
+cudaStream_t LlamaDevice::open_batch(LlamaDevice *const *c, int n, const int32_t *ids, const int *n_past) {
     LlamaDevice &L0 = *c[0];
     LlamaGroup &G = *L0.group_;
     // a context's own decode step may still be running on its stream (decode_step returns before it finishes): it has to be done
@@ -1015,8 +1015,15 @@ void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids,
     for (int i = 0; i < n; ++i) c[i]->sync();
     if (!G.x) L0.build_group_workspace();
     if (!G.graph[n]) L0.build_batch_graph(n);
-    for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], ids[i], c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
+    for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], ids ? ids[i] : -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
     CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, G.stream));
+    return G.stream;
+}
+
+void LlamaDevice::decode_batch(LlamaDevice *const *c, int n, const int32_t *ids, const int *n_past, int32_t *ids_out) {
+    LlamaDevice &L0 = *c[0];
+    LlamaGroup &G = *L0.group_;
+    open_batch(c, n, ids, n_past);
     CUDA_CHECK(cudaGraphLaunch(G.graph[n], G.stream));
     CUDA_CHECK(cudaStreamSynchronize(G.stream));   // (h_slots / h_ids are reused by the next step)
     L0.launches_ += (unsigned long long)G.graph_kernels[n];
@@ -1380,71 +1387,68 @@ void LlamaDevice::ensure_sampler() {
     owned_bytes_ += smp_->bytes;
 }
 
-// a launch of at most 8 contexts takes the 8-column tables: the first 8 columns of the wide ones
-static smp::SampleArgs narrow(const smp::SampleArgsWide &w) {
-    smp::SampleArgs a{};
-    memcpy(a.c, w.c, sizeof(a.c));
-    a.n_vocab = w.n_vocab; a.step = w.step;
-    return a;
+// the columns of one kind in a step's sampling launch (the chain with greedy and constrained columns, or mirostat), in slot order: each
+// column's SampleCtx carries its slot, and its StopArgsN / ConsArgsN entries follow it
+struct SampleLaunch {
+    smp::SampleArgsN<LlamaDevice::kMaxBatch> a{};
+    smp::StopArgsN<LlamaDevice::kMaxBatch> s{};
+    smp::ConsArgsN<LlamaDevice::kMaxBatch> k{};
+    int n = 0;
+    bool mirostat = false;   // the mirostat kernel (every column's args.mirostat is 1 or 2)
+    bool cons = false;       // the constrained kernel, which takes every column's constraint table
+};
+template <int N>
+static void launch_sample(const smp::SampleArgsN<N> &a, const smp::StopArgsN<N> &sa, const smp::ConsArgsN<N> &k, int n, bool mirostat, bool cons,
+                          bool stop, cudaStream_t s) {
+    using Stop = smp::StopArgsN<N>;
+    if (cons && stop) smp::sample_cons_kernel<N, Stop><<<n, smp::kThreads, 0, s>>>(a, sa, k);
+    else if (cons) smp::sample_cons_kernel<N><<<n, smp::kThreads, 0, s>>>(a, k);
+    else if (mirostat && stop) smp::sample_kernel<N, true, Stop><<<n, smp::kThreads, 0, s>>>(a, sa);
+    else if (mirostat) smp::sample_kernel<N, true><<<n, smp::kThreads, 0, s>>>(a);
+    else if (stop) smp::sample_kernel<N, false, Stop><<<n, smp::kThreads, 0, s>>>(a, sa);
+    else smp::sample_kernel<N, false><<<n, smp::kThreads, 0, s>>>(a);
 }
-static smp::StopArgs narrow(const smp::StopArgsWide &w) {
-    smp::StopArgs s{};
-    memcpy(s.r, w.r, sizeof(s.r)); memcpy(s.snap, w.snap, sizeof(s.snap)); s.tab = w.tab;
-    return s;
+// one sampling step of K's columns in one launch (grid K.n) of the kernel of its kind; stop: sample_until's step, which takes K.s.  Up to
+// 8 columns the launch takes the 8-column tables, the first 8 columns of those of K's that the kernel reads.
+static void launch_sample(const SampleLaunch &K, bool stop, cudaStream_t s) {
+    if (K.n > 8) return launch_sample(K.a, K.s, K.k, K.n, K.mirostat, K.cons, stop, s);
+    smp::SampleArgsN<8> a{};
+    memcpy(a.c, K.a.c, sizeof(a.c));
+    a.n_vocab = K.a.n_vocab; a.step = K.a.step;
+    smp::StopArgsN<8> sa{};
+    if (stop) { memcpy(sa.r, K.s.r, sizeof(sa.r)); memcpy(sa.snap, K.s.snap, sizeof(sa.snap)); sa.tab = K.s.tab; }
+    smp::ConsArgsN<8> k{};
+    if (K.cons) memcpy(k.c, K.k.c, sizeof(k.c));
+    launch_sample(a, sa, k, K.n, K.mirostat, K.cons, stop, s);
 }
-// one sampling step of n contexts in one launch (grid n): the 8-column kernels up to 8 contexts, the wide ones above; mirostat: the
-// mirostat kernels (every column's c.args.mirostat is 1 or 2)
-// k (may be null): the constrained twins, which take every column's constraint table
-static void launch_sample(const smp::SampleArgsWide &a, int n, bool mirostat, cudaStream_t s, const smp::ConsArgsWide *k = nullptr) {
-    if (k) {
-        if (n <= 8) {
-            smp::ConsArgs k8{};
-            memcpy(k8.c, k->c, sizeof(k8.c));
-            smp::sample_cons_kernel<<<n, smp::kThreads, 0, s>>>(narrow(a), k8);
-        } else smp::sample_cons_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, *k);
-        return;
+// the columns of `all` by kind: kind[0] the chain, greedy and constrained columns, kind[1] mirostat
+static void split_kinds(const SampleLaunch &all, SampleLaunch kind[2]) {
+    for (int i = 0; i < all.n; ++i) {
+        SampleLaunch &K = kind[all.a.c[i].args.mirostat ? 1 : 0];
+        K.a.c[K.n] = all.a.c[i]; K.s.r[K.n] = all.s.r[i]; K.s.snap[K.n] = all.s.snap[i]; K.k.c[K.n] = all.k.c[i];
+        K.cons = K.cons || all.k.c[i].off;
+        ++K.n;
     }
-    if (n <= 8) {
-        const smp::SampleArgs a8 = narrow(a);
-        if (mirostat) smp::sample_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8);
-        else smp::sample_kernel<<<n, smp::kThreads, 0, s>>>(a8);
-    } else if (mirostat) smp::sample_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
-    else smp::sample_wide_kernel<<<n, smp::kThreads, 0, s>>>(a);
+    for (int m = 0; m < 2; ++m) { kind[m].a.n_vocab = all.a.n_vocab; kind[m].s.tab = all.s.tab; kind[m].mirostat = m == 1; }
 }
-static void launch_sample_until(const smp::SampleArgsWide &a, const smp::StopArgsWide &sa, int n, bool mirostat, cudaStream_t s,
-                                const smp::ConsArgsWide *k = nullptr) {
-    if (k) {
-        if (n <= 8) {
-            smp::ConsArgs k8{};
-            memcpy(k8.c, k->c, sizeof(k8.c));
-            smp::sample_until_cons_kernel<<<n, smp::kThreads, 0, s>>>(narrow(a), narrow(sa), k8);
-        } else smp::sample_until_cons_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa, *k);
-        return;
+// the sampling launches of step t: one per kind present
+static void launch_kinds(SampleLaunch kind[2], int t, bool stop, cudaStream_t s) {
+    for (int m = 0; m < 2; ++m) {
+        if (!kind[m].n) continue;
+        kind[m].a.step = t;
+        launch_sample(kind[m], stop, s);
     }
-    if (n <= 8) {
-        const smp::SampleArgs a8 = narrow(a);
-        const smp::StopArgs s8 = narrow(sa);
-        if (mirostat) smp::sample_until_mirostat_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8);
-        else smp::sample_until_kernel<<<n, smp::kThreads, 0, s>>>(a8, s8);
-    } else if (mirostat) smp::sample_until_mirostat_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
-    else smp::sample_until_wide_kernel<<<n, smp::kThreads, 0, s>>>(a, sa);
 }
 // the bytes of a context's sampler state that a call moves: the generator, and μ after it with mirostat
 static size_t sampler_state_bytes(const SamplingArgs &p) { return 625 * 4 + (p.mirostat ? sizeof(MirostatState) : 0); }
 
 cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu,
-                                         smp::SampleArgsWide &a, const SampleConstraint *cons, smp::ConsArgsWide *k) {
+                                         const SampleConstraint *cons, SampleLaunch &all) {
     LlamaDevice &L0 = *c[0];
-    a = smp::SampleArgsWide{};
+    smp::SampleArgsN<kMaxBatch> &a = all.a;
     a.n_vocab = L0.d_.n_vocab;
-    cudaStream_t s = L0.stream_;
-    if (n >= 2) {   // (as decode_batch: a context's own work must be done before the group stream uses its memory)
-        for (int i = 0; i < n; ++i) c[i]->sync();
-        LlamaGroup &G = *L0.group_;
-        if (!G.x) L0.build_group_workspace();
-        if (!G.graph[n]) L0.build_batch_graph(n);
-        s = G.stream;
-    }
+    all.n = n;
+    const cudaStream_t s = n >= 2 ? open_batch(c, n, nullptr, n_past) : L0.stream_;
     for (int i = 0; i < n; ++i) {
         LlamaDevice &L = *c[i];
         L.ensure_sampler();
@@ -1456,32 +1460,41 @@ cudaStream_t LlamaDevice::begin_sampling(LlamaDevice *const *c, int n, const int
             if (p[i].mirostat) *L.smp_->h_mu = mu[i];
             CUDA_CHECK(cudaMemcpyAsync(L.smp_->mt, L.smp_->h_rng, sampler_state_bytes(p[i]), cudaMemcpyHostToDevice, s));
         }
-        if (k) k->c[i] = smp::ConsCol{nullptr, nullptr, nullptr};
-        if (k && cons && cons[i].off) {
+        if (cons && cons[i].off) {
             *L.smp_->h_cons = cons[i].state;
             CUDA_CHECK(cudaMemcpyAsync(L.smp_->cons, L.smp_->h_cons, sizeof(int), cudaMemcpyHostToDevice, s));
-            k->c[i] = smp::ConsCol{cons[i].off, cons[i].tr, L.smp_->cons};
+            all.k.c[i] = smp::ConsCol{cons[i].off, cons[i].tr, L.smp_->cons};
         }
-    }
-    if (n >= 2) {
-        LlamaGroup &G = *L0.group_;
-        for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n_past[i], -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
-        CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
     }
     return s;
 }
 
-// the decode step after a sampling launch (counted with it): every column is fed its DeviceState::tokens[0]
-void LlamaDevice::sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s) {
+void LlamaDevice::decode_columns(LlamaDevice *const *c, int n, int n_past, cudaStream_t s) {
     LlamaDevice &L0 = *c[0];
     CUDA_CHECK(cudaGetLastError());
-    if (n == 1) {
-        L0.decode_step(-1, n_past);
-        ++L0.launches_;
-    } else {
+    if (n == 1) L0.decode_step(-1, n_past);
+    else {
         CUDA_CHECK(cudaGraphLaunch(L0.group_->graph[n], s));
-        L0.launches_ += (unsigned long long)L0.group_->graph_kernels[n] + 1;
+        L0.launches_ += (unsigned long long)L0.group_->graph_kernels[n];
     }
+}
+
+// steps issued kReplyChunk at a time on s, at most `steps`: step(t) issues step t, and after each chunk j flags(j % 2) queues the copy of
+// its done flags and ev[j % 2] is recorded.  Before chunk j >= 2 the host waits for chunk j - 2's flags (chunk j - 1 keeps the device busy
+// meanwhile) and issues no more once done(j % 2) reads from them that every context is done.  Returns the steps issued.
+template <class Step, class Flags, class Done>
+static int issue_chunks(int steps, cudaStream_t s, const cudaEvent_t ev[2], Step step, Flags flags, Done done) {
+    int issued = 0;
+    for (int j = 0; issued < steps; ++j) {
+        if (j >= 2) {
+            CUDA_CHECK(cudaEventSynchronize(ev[j % 2]));
+            if (done(j % 2)) break;
+        }
+        for (const int end = std::min(steps, issued + LlamaDevice::kReplyChunk); issued < end; ++issued) step(issued);
+        flags(j % 2);
+        CUDA_CHECK(cudaEventRecord(ev[j % 2], s));
+    }
+    return issued;
 }
 
 // after `steps` steps: the fed ids, generators and μ to the host, one synchronisation; returns the device ms since ev0_
@@ -1510,24 +1523,19 @@ float LlamaDevice::end_sampling(LlamaDevice *const *c, int n, int steps, const S
     return ms;
 }
 
-static bool any_constrained(const SampleConstraint *cons, int n) {
-    for (int i = 0; cons && i < n; ++i) if (cons[i].off) return true;
-    return false;
-}
-
 float LlamaDevice::sample_steps(LlamaDevice *const *c, int n, int steps, const int *n_past, const SamplingArgs &p, uint32_t (*rng)[625],
                                 MirostatState *mu, int32_t *ids_out, const SampleConstraint *cons) {
-    smp::SampleArgsWide a;
-    smp::ConsArgsWide k;
-    const smp::ConsArgsWide *kp = any_constrained(cons, n) ? &k : nullptr;
+    LlamaDevice &L0 = *c[0];
     SamplingArgs ps[kMaxBatch];
     std::fill(ps, ps + n, p);
-    cudaStream_t s = begin_sampling(c, n, n_past, ps, rng, mu, a, cons, kp ? &k : nullptr);
-    CUDA_CHECK(cudaEventRecord(c[0]->ev0_, s));
+    SampleLaunch all, kind[2];   // (uniform settings: one kind, one launch a step)
+    const cudaStream_t s = begin_sampling(c, n, n_past, ps, rng, mu, cons, all);
+    split_kinds(all, kind);
+    CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
     for (int t = 0; t < steps; ++t) {
-        a.step = t;
-        launch_sample(a, n, p.mirostat != 0, s, kp);
-        sampled_decode(c, n, n_past[0] + t, s);
+        launch_kinds(kind, t, false, s);
+        ++L0.launches_;
+        decode_columns(c, n, n_past[0] + t, s);
     }
     return end_sampling(c, n, steps, ps, rng, mu, ids_out, s);
 }
@@ -1600,27 +1608,16 @@ static void reply_init(smp::ReplyState &r, const std::string &stop, const std::s
     r.stop_len = (int)stop.size();
 }
 
-// the columns of one kind in a step's sampling launch (the chain with greedy and constrained columns, or mirostat), in slot order: each
-// column's SampleCtx carries its slot, and its StopArgs / ConsArgs entries follow it
-struct UntilLaunch {
-    smp::SampleArgsWide a{};
-    smp::StopArgsWide s{};
-    smp::ConsArgsWide k{};
-    int n = 0;
-    bool cons = false;
-};
-
 float LlamaDevice::sample_until(LlamaDevice *const *c, int n, const UntilArgs *u, const int *n_past, uint32_t (*rng)[625], MirostatState *mu,
                                 const std::string *tail, int32_t *ids_out, int32_t *n_out, int32_t *stopped, const SampleConstraint *cons,
                                 const LogprobRequest *rec) {
     LlamaDevice &L0 = *c[0];
-    SamplingArgs p[kMaxBatch];
+    SamplingArgs p[kMaxBatch]{};
     int S = 0;   // the longest budget: the most steps the call runs
     for (int i = 0; i < n; ++i) { p[i] = u[i].p; S = std::max(S, u[i].max_steps); }
-    smp::SampleArgsWide a;
-    smp::ConsArgsWide k;
-    cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, a, cons, &k);
-    smp::StopArgsWide sa{};
+    SampleLaunch all, kind[2];
+    const cudaStream_t s = begin_sampling(c, n, n_past, p, rng, mu, cons, all);
+    smp::StopArgsN<kMaxBatch> &sa = all.s;
     sa.tab = L0.group_->tokens;
     lp::LogprobArgs la{};
     pen::PenaltyArgs pa{};
@@ -1646,52 +1643,35 @@ float LlamaDevice::sample_until(LlamaDevice *const *c, int n, const UntilArgs *u
             }
             pa.c[n_pen++] = pen::PenaltyCol{L.logits_, L.pen_->row, L.pen_->count, L.pen_->tail, L.smp_->ids, L.state_, L.reply_->r, T, u[i].q,
                                             p[i].temp <= 0.f ? 1 : 0};
-            a.c[i].logits = L.pen_->row;
+            all.a.c[i].logits = L.pen_->row;
         }
     }
     la.n_vocab = L0.d_.n_vocab; la.top_n = rec ? rec->top_n : 0;
     pa.n_vocab = L0.d_.n_vocab;
-    UntilLaunch kind[2];   // [0] the chain, greedy and constrained columns; [1] mirostat
-    for (int i = 0; i < n; ++i) {
-        UntilLaunch &K = kind[p[i].mirostat ? 1 : 0];
-        K.a.c[K.n] = a.c[i]; K.s.r[K.n] = sa.r[i]; K.s.snap[K.n] = sa.snap[i]; K.k.c[K.n] = k.c[i];
-        K.cons = K.cons || (cons && cons[i].off);
-        ++K.n;
-    }
-    for (UntilLaunch &K : kind) { K.a.n_vocab = a.n_vocab; K.s.tab = sa.tab; }
+    split_kinds(all, kind);
     ReplyScratch &R0 = *L0.reply_;
     CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
-    int issued = 0;
-    for (int j = 0; issued < S; ++j) {
-        if (j >= 2) {   // chunk j - 2's flags; chunk j - 1 keeps the device busy meanwhile
-            CUDA_CHECK(cudaEventSynchronize(R0.ev[j % 2]));
-            bool all = true;
-            for (int i = 0; i < n; ++i) all = all && R0.h_done[(j % 2) * kMaxBatch + i] != 0;
-            if (all) break;
+    const int issued = issue_chunks(S, s, R0.ev, [&](int t) {
+        if (n_pen) {   // the rows this step samples from
+            pa.step = t;
+            pen::penalty_rows_kernel<<<n_pen, pen::kThreads, 0, s>>>(pa);
+            ++L0.launches_;
         }
-        for (const int end = std::min(S, issued + kReplyChunk); issued < end; ++issued) {
-            if (n_pen) {   // the rows this step samples from
-                pa.step = issued;
-                pen::penalty_rows_kernel<<<n_pen, pen::kThreads, 0, s>>>(pa);
-                ++L0.launches_;
-            }
-            for (int m = 0; m < 2; ++m) {
-                UntilLaunch &K = kind[m];
-                if (!K.n) continue;
-                K.a.step = issued;
-                launch_sample_until(K.a, K.s, K.n, m == 1, s, K.cons ? &K.k : nullptr);
-            }
-            if (rec) {   // the logits the step sampled from, before the decode step replaces them
-                la.step = issued;
-                lp::logprob_rows_kernel<<<n, lp::kThreads, 0, s>>>(la);
-                ++L0.launches_;
-            }
-            sampled_decode(c, n, n_past[0] + issued, s);
+        launch_kinds(kind, t, true, s);
+        ++L0.launches_;
+        if (rec) {   // the logits the step sampled from, before the decode step replaces them
+            la.step = t;
+            lp::logprob_rows_kernel<<<n, lp::kThreads, 0, s>>>(la);
+            ++L0.launches_;
         }
+        decode_columns(c, n, n_past[0] + t, s);
+    }, [&](int b) {
         for (int i = 0; i < n; ++i)
-            CUDA_CHECK(cudaMemcpyAsync(R0.h_done + (j % 2) * kMaxBatch + i, &c[i]->reply_->r->done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        CUDA_CHECK(cudaEventRecord(R0.ev[j % 2], s));
-    }
+            CUDA_CHECK(cudaMemcpyAsync(R0.h_done + b * kMaxBatch + i, &c[i]->reply_->r->done, sizeof(int), cudaMemcpyDeviceToHost, s));
+    }, [&](int b) {
+        for (int i = 0; i < n; ++i) if (R0.h_done[b * kMaxBatch + i] == 0) return false;
+        return true;
+    });
     for (int i = 0; i < n; ++i)
         CUDA_CHECK(cudaMemcpyAsync(c[i]->reply_->h_r, c[i]->reply_->r, sizeof(smp::UntilState), cudaMemcpyDeviceToHost, s));
     const float ms = end_sampling(c, n, issued, p, rng, mu, ids_out, s);
@@ -1765,14 +1745,12 @@ float LlamaDevice::beam_search(LlamaDevice *const *c, int n, int max_steps, int 
     const int32_t argmax0 = L0.argmax();
     cudaStream_t s = L0.stream_;
     if (n >= 2) {
-        if (!G.x) L0.build_group_workspace();
-        if (!G.graph[n]) L0.build_batch_graph(n);
+        int np[kMaxBeams];
+        std::fill(np, np + n, n0);
+        s = open_batch(c, n, nullptr, np);
         copy_state(L0, c + 1, n - 1, n0);   // every slot starts from the conversation; its rows below n0 are not written again
-        s = G.stream;
         CUDA_CHECK(cudaMemcpyAsync(G.beam_snap, L0.logits_, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(G.beam_snap_state, L0.state_, sizeof(DeviceState), cudaMemcpyDeviceToDevice, s));
-        for (int i = 0; i < n; ++i) G.h_slots[i] = SessionSlot{n0, -1, c[i]->kcache_, c[i]->vcache_, c[i]->logits_, c[i]->state_};
-        CUDA_CHECK(cudaMemcpyAsync(G.slots, G.h_slots, (size_t)n * sizeof(SessionSlot), cudaMemcpyHostToDevice, s));
     }
     beam::BeamState &h = *G.h_beam;
     memset(&h, 0, sizeof h);
@@ -1793,29 +1771,18 @@ float LlamaDevice::beam_search(LlamaDevice *const *c, int n, int max_steps, int 
     ra.row = (long long)L0.n_embd_local_ * 2 / 16; ra.plane = (long long)L0.d_.n_ctx * ra.row; ra.n_layer = L0.d_.n_layer; ra.n0 = n0;
     const dim3 rgrid((unsigned)std::max(1, 8 * L0.sm_count_ / (2 * L0.d_.n_layer)), (unsigned)(2 * L0.d_.n_layer));
     CUDA_CHECK(cudaEventRecord(L0.ev0_, s));
-    int issued = 0;
-    for (int j = 0; issued < max_steps; ++j) {
-        if (j >= 2) {   // chunk j - 2's flag; chunk j - 1 keeps the device busy meanwhile
-            CUDA_CHECK(cudaEventSynchronize(G.beam_ev[j % 2]));
-            if (G.h_beam_done[j % 2]) break;
+    issue_chunks(max_steps, s, G.beam_ev, [&](int t) {
+        beam::beam_rank_kernel<<<n, beam::kRankThreads, 0, s>>>(a);
+        beam::beam_merge_kernel<<<1, beam::kMergeThreads, 0, s>>>(a);
+        L0.launches_ += 2;
+        if (n >= 2) {
+            beam::beam_reorder_kernel<<<rgrid, beam::kCopyThreads, 0, s>>>(ra);
+            ++L0.launches_;
         }
-        for (const int end = std::min(max_steps, issued + kReplyChunk); issued < end; ++issued) {
-            beam::beam_rank_kernel<<<n, beam::kRankThreads, 0, s>>>(a);
-            beam::beam_merge_kernel<<<1, beam::kMergeThreads, 0, s>>>(a);
-            L0.launches_ += 2;
-            if (n == 1) {
-                CUDA_CHECK(cudaGetLastError());
-                L0.decode_step(-1, n0 + issued);
-            } else {
-                beam::beam_reorder_kernel<<<rgrid, beam::kCopyThreads, 0, s>>>(ra);
-                CUDA_CHECK(cudaGetLastError());
-                CUDA_CHECK(cudaGraphLaunch(G.graph[n], s));
-                L0.launches_ += (unsigned long long)G.graph_kernels[n] + 1;
-            }
-        }
-        CUDA_CHECK(cudaMemcpyAsync(G.h_beam_done + j % 2, &G.beam->done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        CUDA_CHECK(cudaEventRecord(G.beam_ev[j % 2], s));
-    }
+        decode_columns(c, n, n0 + t, s);
+    }, [&](int b) {
+        CUDA_CHECK(cudaMemcpyAsync(G.h_beam_done + b, &G.beam->done, sizeof(int), cudaMemcpyDeviceToHost, s));
+    }, [&](int b) { return G.h_beam_done[b] != 0; });
     CUDA_CHECK(cudaEventRecord(L0.ev1_, s));
     std::vector<int32_t> hid((size_t)n * stride);
     CUDA_CHECK(cudaMemcpyAsync(G.h_beam, G.beam, sizeof(beam::BeamState), cudaMemcpyDeviceToHost, s));
@@ -1966,16 +1933,18 @@ void LlamaDevice::test_sample(const float *logits, int n_vocab, const SamplingAr
     CUDA_CHECK(cudaMemcpy(ss.mt, rng, 625 * 4, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemset(ss.mu, 0, sizeof(MirostatState)));
     if (mu_out && p.mirostat) CUDA_CHECK(cudaMalloc((void **)&mu_d, (size_t)n_draws * 4));
-    smp::SampleArgsWide a{};
-    a.n_vocab = n_vocab;
-    a.c[0] = ss.ctx(lg, st, nullptr, 0);
-    a.c[0].args = p;
+    SampleLaunch K;
+    K.a.n_vocab = n_vocab;
+    K.a.c[0] = ss.ctx(lg, st, nullptr, 0);
+    K.a.c[0].args = p;
+    K.n = 1;
+    K.mirostat = p.mirostat != 0;
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     CUDA_CHECK(cudaEventRecord(e0, 0));
     for (int i = 0; i < n_draws; ++i) {
-        a.step = i;
-        launch_sample(a, 1, p.mirostat != 0, 0);
+        K.a.step = i;
+        launch_sample(K, false, 0);
         CUDA_CHECK(cudaGetLastError());
         if (mu_d) CUDA_CHECK(cudaMemcpyAsync(mu_d + i, &ss.mu->mu[p.mirostat - 1], 4, cudaMemcpyDeviceToDevice, 0));
     }

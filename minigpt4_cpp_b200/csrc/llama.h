@@ -52,12 +52,10 @@ struct SessionSlot {   // one column of a batched decode step (device table of t
     DeviceState *state;
 };
 
-// Sampler::sample's arguments: the non-mirostat chain, or mirostat 1 / 2 (which ignores top_k .. typical_p); mirostat 0: the chain
-struct SamplingArgs { float temp; int top_k; float top_p, tfs_z, typical_p; int mirostat; float mirostat_tau, mirostat_eta; };
 struct MirostatState { float mu[2]; int init[2]; };   // a context's mirostat μ of v1 / v2 and whether each is set (Sampler::get_mu)
 struct SamplerScratch; // a context's device sampler: mt19937 state, candidate scratch, the ids of a call (llama.cu, llama_sample.cuh)
 struct ReplyScratch;   // a context's stop state in sample_until: reply tail, stop text, done flag, snapshot (llama.cu, llama_sample.cuh)
-namespace smp { template <int N> struct SampleArgsN; template <int N> struct ConsArgsN; }
+struct SampleLaunch;   // the columns of one sampling launch (llama.cu)
 
 struct LlamaGroup;     // what the contexts of one model share besides the weights: the batch workspace and its graphs (llama.cu)
 // device memory for tables the contexts of a group share that may outlive its last context (constraint tables): counted in the group's
@@ -321,12 +319,17 @@ private:
     void ensure_logprob();
     std::unique_ptr<PenaltyScratch> pen_;   // sample_until's penalised row, from the context's first call with penalties (owned_bytes_)
     void ensure_penalty(int n_tail);        // ... with room for a history tail of n_tail ids
-    // the set-up both sampling calls share: the batch graph and slot table (n >= 2), each context's sampler, its column's parameters
-    // p[i], generator and mirostat μ; returns the stream the steps run on
-    // cons (may be null): each constrained context's state goes to its device copy, and k takes every column's tables
+    // the start of a batched step over n >= 2 contexts of one group: each context's own work done, the group workspace and the batch
+    // graph of n columns, and the slot table, column i fed ids[i] (ids null: its DeviceState::tokens[0]) at n_past[i]; returns the group stream
+    static cudaStream_t open_batch(LlamaDevice *const *c, int n, const int32_t *ids, const int *n_past);
+    // the set-up both sampling calls share: the batch (n >= 2), each context's sampler, its column in `all` with its parameters p[i],
+    // generator and mirostat μ; returns the stream the steps run on
+    // cons (may be null): each constrained context's state goes to its device copy, and its column takes its tables
     static cudaStream_t begin_sampling(LlamaDevice *const *c, int n, const int *n_past, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu,
-                                       smp::SampleArgsN<kMaxBatch> &a, const SampleConstraint *cons = nullptr, smp::ConsArgsN<kMaxBatch> *k = nullptr);
-    static void sampled_decode(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
+                                       const SampleConstraint *cons, SampleLaunch &all);
+    // the decode step of the n columns after a step's device work (n = 1: the context's own graph or megakernel; n >= 2: the batch graph,
+    // every column fed its DeviceState::tokens[0]); counts the decode's launches only
+    static void decode_columns(LlamaDevice *const *c, int n, int n_past, cudaStream_t s);
     static float end_sampling(LlamaDevice *const *c, int n, int steps, const SamplingArgs *p, uint32_t (*rng)[625], MirostatState *mu, int32_t *ids_out,
                               cudaStream_t s);
     void alloc_context();            // the per-context buffers (KV cache, activations, state, stream)

@@ -241,13 +241,12 @@ struct SampleCtx {
     int *id; float *logit, *p, *aux;   // [n_vocab] candidates (id, logit, probability); tail_free's d2 / typical's terms
     SamplingArgs args;           // the column's sampling parameters (mirostat 1 / 2: the mirostat kernels, which ignore top_k .. typical_p)
 };
-// a sampling launch's arguments, one column per CTA; the table is passed by value, so its capacity N is part of the kernel's parameters
+// a sampling launch's arguments, one column per CTA; the table is passed by value, so its capacity N is part of the kernel's parameters:
+// N = 8 for launches of 1..8 contexts, kMaxBatch for wider ones
 template <int N> struct SampleArgsN {
     SampleCtx c[N];
     int n_vocab, step;
 };
-struct SampleArgs : SampleArgsN<8> {};                               // the kernels of 1..8 contexts
-using SampleArgsWide = SampleArgsN<LlamaDevice::kMaxBatch>;          // the wide kernels of 9..kMaxBatch contexts
 
 // float -> key that orders like the float (-0 as +0, so that equal logits are equal keys), and back
 __device__ __forceinline__ unsigned ord_key(float v) {
@@ -413,7 +412,7 @@ __device__ __forceinline__ int cand_id(const ListedArgs &a, int j) { return a.sr
 __device__ __forceinline__ bool cand_listed(const ListedArgs &a) { return a.src.listed(); }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// one context's sampling step, the body of sample_kernel and sample_until_kernel (a CTA of kThreads): samples c's logits over the
+// one context's sampling step, the body of sample_kernel and sample_cons_kernel (a CTA of kThreads): samples c's logits over the
 // candidates of a (cand_*) as Sampler::sample (Sampler::sample_allowed for listed candidates) does with the column's parameters c.args,
 // and hands the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy id the logits epilogue already left in tokens[0] (greedy =
 // true; the generator is not read), or for listed candidates their arg-max, the lower id on ties (greedy = false).  Otherwise the
@@ -576,7 +575,7 @@ template <class A, class Fed> __device__ __forceinline__ void sample_body(const 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// one context's mirostat step, the body of sample_mirostat_kernel and sample_until_mirostat_kernel: Sampler::sample's mirostat branch
+// one context's mirostat step, the body of sample_kernel<N, true>: Sampler::sample's mirostat branch
 // (c.args.mirostat 1 or 2, its tau and eta) with its μ in `ms`, handing the id to fed(id, greedy) on thread 0.  temp <= 0: the greedy
 // id, and neither μ nor the generator is read.  Otherwise μ is set to 2 tau at the mode's first use, as on the host, and updated after
 // the draw.
@@ -653,25 +652,6 @@ template <class A> __device__ __forceinline__ void feed(const A &a, const Sample
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits, writes the id into tokens[0] and
-// ids[step], and moves a batched column to its next position.  The *_wide_kernel variants take the kMaxBatch-column table (n > 8) and
-// share the body, so every column computes what it computes in the 8-column kernels.
-// ---------------------------------------------------------------------------------------------------------------------------------
-template <class A> __device__ __forceinline__ void sample_step(const A &a) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    sample_body(a, c, [&](int id, bool greedy) { feed(a, c, id, greedy); });
-}
-template <class A> __device__ __forceinline__ void sample_mirostat_step(const A &a) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { feed(a, c, id, greedy); });
-}
-__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgs a) { sample_step(a); }
-__global__ void __launch_bounds__(kThreads) sample_wide_kernel(const SampleArgsWide a) { sample_step(a); }
-// sample_kernel with the mirostat step
-__global__ void __launch_bounds__(kThreads) sample_mirostat_kernel(const SampleArgs a) { sample_mirostat_step(a); }
-__global__ void __launch_bounds__(kThreads) sample_mirostat_wide_kernel(const SampleArgsWide a) { sample_mirostat_step(a); }
-
-// ---------------------------------------------------------------------------------------------------------------------------------
 // stop on the reply's text (minigpt4_b200_sample_until; host side LlamaDevice::sample_until): the reference's chat loop
 // (MiniGPT4ChatBot.generate) appends each token's text to the reply and stops after a token that is not exactly "##" once the reply
 // ends with "###".  The text of an id is the C string of Engine::id_to_token, from the group's token table.
@@ -719,9 +699,8 @@ template <int N> struct StopArgsN {
     float *snap[N];   // [n_vocab] each context's logits after its last step
     TokenTable tab;
 };
-struct StopArgs : StopArgsN<8> {};
-using StopArgsWide = StopArgsN<LlamaDevice::kMaxBatch>;
-static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) <= 32764, "the widest kernel's parameters fit the 32 764-byte limit");
+static_assert(sizeof(SampleArgsN<LlamaDevice::kMaxBatch>) + sizeof(StopArgsN<LlamaDevice::kMaxBatch>) <= 32764,
+              "the widest kernel's parameters fit the 32 764-byte limit");
 
 // one step of sample_kernel that stops each context on its reply's text or its budget.  A stopped context does not draw (its generator
 // stays); at the next step it saves its logits and DeviceState, which the host restores at the end of the call.  The decode work that
@@ -758,41 +737,38 @@ __device__ __forceinline__ void until_feed(const A &a, const S &s, const SampleC
     else if (r.n_fed == r.budget) { r.done = 1; r.by_budget = 1; }
 }
 
-__global__ void __launch_bounds__(kThreads) sample_until_kernel(const SampleArgs a, const StopArgs s) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    UntilState &r = *s.r[blockIdx.x];
-    __shared__ int sh_state;
-    if (!until_running(a, s, c, r, sh_state)) return;
-    sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
-}
-__global__ void __launch_bounds__(kThreads) sample_until_wide_kernel(const SampleArgsWide a, const StopArgsWide s) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    UntilState &r = *s.r[blockIdx.x];
-    __shared__ int sh_state;
-    if (!until_running(a, s, c, r, sh_state)) return;
-    sample_body(a, c, [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
-}
+// the stop parameter of a stopping kernel: the one element of its parameter pack
+template <class S> __device__ __forceinline__ const S &stop_args(const S &s) { return s; }
 
-// sample_until_kernel with the mirostat step
-__global__ void __launch_bounds__(kThreads) sample_until_mirostat_kernel(const SampleArgs a, const StopArgs s) {
+// ---------------------------------------------------------------------------------------------------------------------------------
+// one sampling step of n contexts: grid n, block kThreads.  CTA i samples context i's logits (kMirostat: the mirostat step), writes the
+// id into tokens[0] and ids[step], and moves a batched column to its next position.  N is the capacity of the column tables: 8 for up to
+// 8 contexts, kMaxBatch above; every column computes the same whatever N.  With a stop parameter (S: StopArgsN<N>) it is sample_until's
+// step, which stops each context on its reply's text or its budget.  The stop parameter comes after every parameter of the plain step,
+// so those keep their offsets.
+// ---------------------------------------------------------------------------------------------------------------------------------
+template <int N, bool kMirostat, class... S>
+__global__ void __launch_bounds__(kThreads) sample_kernel(const SampleArgsN<N> a, const S... s) {
     const SampleCtx &c = a.c[blockIdx.x];
-    UntilState &r = *s.r[blockIdx.x];
-    __shared__ int sh_state;
-    if (!until_running(a, s, c, r, sh_state)) return;
-    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
-}
-__global__ void __launch_bounds__(kThreads) sample_until_mirostat_wide_kernel(const SampleArgsWide a, const StopArgsWide s) {
-    const SampleCtx &c = a.c[blockIdx.x];
-    UntilState &r = *s.r[blockIdx.x];
-    __shared__ int sh_state;
-    if (!until_running(a, s, c, r, sh_state)) return;
-    mirostat_body(a, c, mirostat_state(c), [&](int id, bool greedy) { until_feed(a, s, c, r, id, greedy); });
+    const auto step = [&](auto fed) {
+        if constexpr (kMirostat) mirostat_body(a, c, mirostat_state(c), fed);
+        else sample_body(a, c, fed);
+    };
+    if constexpr (sizeof...(S) == 0) {
+        step([&](int id, bool greedy) { feed(a, c, id, greedy); });
+    } else {
+        const StopArgsN<N> &st = stop_args(s...);
+        UntilState &r = *st.r[blockIdx.x];
+        __shared__ int sh_state;
+        if (!until_running(a, st, c, r, sh_state)) return;
+        step([&](int id, bool greedy) { until_feed(a, st, c, r, id, greedy); });
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// constrained sampling (minigpt4_b200_constraint_*, DESIGN.md §4.12): twins of the four kernels above that take each column's constraint
-// table.  A constrained column samples over its state's allowed ids only and thread 0 moves its state after feeding; an unconstrained
-// column (off null) runs exactly what the kernels above run, so one launch takes a mix of both.
+// constrained sampling (minigpt4_b200_constraint_*, DESIGN.md §4.12): the twin of sample_kernel's chain that takes each column's
+// constraint table.  A constrained column samples over its state's allowed ids only and thread 0 moves its state after feeding; an
+// unconstrained column (off null) runs exactly what sample_kernel runs, so one launch takes a mix of both.
 // ---------------------------------------------------------------------------------------------------------------------------------
 struct ConsCol {
     const int *off;      // the table's row offsets (n_states + 2; row n_states the finished state); null: unconstrained
@@ -800,9 +776,8 @@ struct ConsCol {
     int *state;          // the column's state, which the host uploads before the call
 };
 template <int N> struct ConsArgsN { ConsCol c[N]; };
-struct ConsArgs : ConsArgsN<8> {};
-using ConsArgsWide = ConsArgsN<LlamaDevice::kMaxBatch>;
-static_assert(sizeof(SampleArgsWide) + sizeof(StopArgsWide) + sizeof(ConsArgsWide) <= 32764, "the widest constrained kernel's parameters fit the 32 764-byte limit");
+static_assert(sizeof(SampleArgsN<LlamaDevice::kMaxBatch>) + sizeof(StopArgsN<LlamaDevice::kMaxBatch>) + sizeof(ConsArgsN<LlamaDevice::kMaxBatch>) <= 32764,
+              "the widest constrained kernel's parameters fit the 32 764-byte limit");
 
 // the candidates of column k in its current state (read by every thread before thread 0 can write the next one)
 template <class A> __device__ __forceinline__ AllowedIds allowed_ids(const A &a, const ConsCol &k) {
@@ -842,13 +817,11 @@ template <class A, class S, class K> __device__ __forceinline__ void sample_unti
         cons_advance(kc, src, id);
     });
 }
-__global__ void __launch_bounds__(kThreads) sample_cons_kernel(const SampleArgs a, const ConsArgs k) { sample_cons_step(a, k); }
-__global__ void __launch_bounds__(kThreads) sample_cons_wide_kernel(const SampleArgsWide a, const ConsArgsWide k) { sample_cons_step(a, k); }
-__global__ void __launch_bounds__(kThreads) sample_until_cons_kernel(const SampleArgs a, const StopArgs s, const ConsArgs k) {
-    sample_until_cons_step(a, s, k);
-}
-__global__ void __launch_bounds__(kThreads) sample_until_cons_wide_kernel(const SampleArgsWide a, const StopArgsWide s, const ConsArgsWide k) {
-    sample_until_cons_step(a, s, k);
+// the constrained step (S: none) or sample_until's (S: StopArgsN<N>, before the constraint tables as sample_until_cons_step takes them)
+template <int N, class... S>
+__global__ void __launch_bounds__(kThreads) sample_cons_kernel(const SampleArgsN<N> a, const S... s, const ConsArgsN<N> k) {
+    if constexpr (sizeof...(S) == 0) sample_cons_step(a, k);
+    else sample_until_cons_step(a, stop_args(s...), k);
 }
 
 // seam: reply_take over ids[0, n) from r's tail; *stop_at = the index of the id that ends the reply, -1 if none does

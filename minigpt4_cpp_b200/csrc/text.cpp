@@ -152,7 +152,7 @@ void Sampler::set_rng(const uint32_t state[625]) {
 void Sampler::get_mu(float mu[2], bool init[2]) const { mu[0] = mu_v1_; mu[1] = mu_v2_; init[0] = mu_v1_init_; init[1] = mu_v2_init_; }
 void Sampler::set_mu(const float mu[2], const bool init[2]) { mu_v1_ = mu[0]; mu_v2_ = mu[1]; mu_v1_init_ = init[0]; mu_v2_init_ = init[1]; }
 
-int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingParams &sp) {
+int32_t Sampler::sample(const float *logits, int n_vocab, const SamplingArgs &sp) {
     if (sp.temp <= 0) return greedy(logits, n_vocab);
     std::vector<Candidate> c((size_t)n_vocab);
     for (int i = 0; i < n_vocab; ++i) c[(size_t)i] = Candidate{i, logits[i], 0.f};
@@ -205,7 +205,7 @@ void Sampler::penalize(float *logits, int n_vocab, const int32_t *ids, int n, fl
     }
 }
 
-int32_t Sampler::chain(std::vector<Candidate> &c, int k, const SamplingParams &sp) {
+int32_t Sampler::chain(std::vector<Candidate> &c, int k, const SamplingArgs &sp) {
     bool sorted = false;
     top_k(c, sorted, k, 1);
     tail_free(c, sorted, sp.tfs_z, 1);
@@ -215,7 +215,7 @@ int32_t Sampler::chain(std::vector<Candidate> &c, int k, const SamplingParams &s
     return draw(c, sorted);
 }
 
-int32_t Sampler::sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingParams &sp) {
+int32_t Sampler::sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingArgs &sp) {
     if (sp.temp <= 0) {   // the first arg-max over the allowed ids, which are ascending: the lower id on ties
         int best = 0;
         for (int j = 1; j < n; ++j) if (logits[ids[j]] > logits[ids[best]]) best = j;

@@ -23,11 +23,6 @@ private:
     std::unordered_map<std::string, int32_t> index_;
 };
 
-struct SamplingParams {
-    float temp; int32_t top_k; float top_p; float tfs_z; float typical_p;
-    int mirostat; float mirostat_tau; float mirostat_eta;
-};
-
 struct Candidate { int32_t id; float logit; float p; };
 
 class Sampler {
@@ -36,7 +31,7 @@ public:
     // Mirrors MiniGPT4::sample_token (reference minigpt4.cpp:2425-2483).  Repeat/presence/frequency penalties
     // and penalize_nl are accepted by the ABI but never applied by the reference; same here (penalize() applies them on request:
     // minigpt4_b200_end_chat_penalized / sample_until_penalized).
-    int32_t sample(const float *logits, int n_vocab, const SamplingParams &p);
+    int32_t sample(const float *logits, int n_vocab, const SamplingArgs &p);
     // llama.cpp's repetition penalty, then its frequency and presence penalties, then main.cpp's penalize_nl, in place over the window
     // ids[0, n) (the caller's last repeat_last_n ids), as include/minigpt4_b200.h states them: for each id v with c >= 1 copies in the
     // window, z1 = repeat_penalty == 1 ? z : z <= 0 ? z * repeat_penalty : z / repeat_penalty, then z1 - (c * alpha_frequency +
@@ -46,7 +41,7 @@ public:
     static int32_t greedy(const float *logits, int n_vocab);  // first arg-max
     // sample over the candidates ids[0, n) only (ascending ids: a constraint's allowed ids), in that order: the chain of sample() with
     // top_k <= 0 as n; temp <= 0: the first arg-max among them.  No mirostat.
-    int32_t sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingParams &p);
+    int32_t sample_allowed(const float *logits, const int32_t *ids, int n, const SamplingArgs &p);
     // individual stages (exposed for unit tests)
     static void top_k(std::vector<Candidate> &c, bool &sorted, int k, size_t min_keep);
     static void softmax(std::vector<Candidate> &c, bool &sorted);
@@ -56,7 +51,7 @@ public:
     static void temperature(std::vector<Candidate> &c, float t);
     int32_t draw(std::vector<Candidate> &c, bool &sorted);
     // the non-mirostat chain over the unsorted candidates c: top_k (k) -> tail_free -> typical -> top_p -> temperature -> draw
-    int32_t chain(std::vector<Candidate> &c, int k, const SamplingParams &p);
+    int32_t chain(std::vector<Candidate> &c, int k, const SamplingArgs &p);
     // the generator's state through its textual representation (operator<< / >>): the 624 words, then the position in them
     void get_rng(uint32_t state[625]) const;
     void set_rng(const uint32_t state[625]);

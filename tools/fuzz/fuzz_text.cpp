@@ -22,7 +22,7 @@ int main(){
     if(mode==2) for(int k=0;k<10;++k) lg[rng()%lg.size()]=-INFINITY;
     if(mode==3) for(int k=0;k<10;++k) lg[rng()%lg.size()]=NAN;
     if(mode==4) for(auto&x:lg) x=0;
-    SamplingParams p{ (float)(rng()%300)/100.f-0.2f, (int)(rng()%100)-10, (float)(rng()%120)/100.f, (float)(rng()%120)/100.f, (float)(rng()%120)/100.f, (int)(rng()%3), (float)(rng()%100)/10.f, (float)(rng()%100)/100.f };
+    SamplingArgs p{ (float)(rng()%300)/100.f-0.2f, (int)(rng()%100)-10, (float)(rng()%120)/100.f, (float)(rng()%120)/100.f, (float)(rng()%120)/100.f, (int)(rng()%3), (float)(rng()%100)/10.f, (float)(rng()%100)/100.f };
     int id=sm.sample(lg.data(),(int)lg.size(),p);
     if(id<0||id>=(int)lg.size()){ printf("bad sample id %d mode %d\n",id,mode); return 1; }
   }

@@ -1,7 +1,7 @@
 """Guard against unintended code-generation changes in kernels that have been measured: md5 of each kernel's SASS (addresses and encodings
 stripped) in build/llama.cu.o and build/vision.cu.o against build/sass_hashes.json (a local record, not committed).
 
-    python tools/sass_guard.py            # compare; lists changed / new / vanished kernels
+    python tools/sass_guard.py            # compare; lists changed / new / vanished / renamed kernels
     python tools/sass_guard.py --write    # record the current build as the baseline (do this right after a measured GPU run)
 
 Use: record after a measured run, then add experimental variants while proving that every measured kernel stayed byte-identical
@@ -47,8 +47,19 @@ if __name__ == "__main__":
     changed = sorted(k for k in base if k in cur and base[k] != cur[k])
     gone = sorted(k for k in base if k not in cur)
     new = sorted(k for k in cur if k not in base)
+    # a vanished kernel whose code a new kernel has, hash for hash, was renamed (a wrapper turned into a template instantiation, say)
+    renamed = []
+    for k in list(gone):
+        match = next((m for m in new if cur[m] == base[k]), None)
+        if match:
+            renamed.append((k, match))
+            gone.remove(k)
+            new.remove(match)
     for title, lst in (("CHANGED", changed), ("VANISHED", gone), ("new", new)):
         for k in lst:
             print(f"{title:9s} {k[:120]}")
-    print(f"{len(base) - len(changed) - len(gone)} of {len(base)} recorded kernels unchanged, {len(changed)} changed, {len(gone)} vanished, {len(new)} new")
+    for old, now in renamed:
+        print(f"RENAMED   {old[:120]} -> {now[:120]}")
+    print(f"{len(base) - len(changed) - len(gone)} of {len(base)} recorded kernels unchanged ({len(renamed)} renamed), {len(changed)} changed, "
+          f"{len(gone)} vanished, {len(new)} new")
     sys.exit(1 if changed or gone else 0)
